@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Headline benchmark: images/sec of DVT stage-1 denoising (ViT-B/14, 518x518, 768+1 views, 2000-iteration
-neural-field fit per image) on N B200s of one node.  One "step" = one image through both hot paths:
+neural-field fit per image) on N H100s of one node.  One "step" = one image through both hot paths:
 HP-1 769 frozen-ViT forwards -> feature bank, HP-2 per-image fit + final 37x37 query.
 
   python bench.py --gpus 1 --steps 3 --warmup 3
@@ -49,6 +49,9 @@ def parse():
     ap.add_argument("--no-kernel-rooflines", action="store_true",
                     help="skip the stand-alone kernel timings (for ncu launch lists of the timed region)")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                    help="after the timed steps, write the last timed image's results (denoised_feats, raw) as DIR/<name>.npy "
+                         "(float32); inputs and weights are seeded, so two builds can be compared output for output")
     ap.add_argument("--no-library-bar", action="store_true",
                     help="skip the unfused cuBLAS / SDPA / torch.optim restatement timed on the same GPU (tools/library_bar.py)")
     return ap.parse_args()
@@ -56,28 +59,20 @@ def parse():
 
 def peaks():
     """HBM copy bandwidth and dense bf16 throughput: the driver-written MEASURED_PEAKS.json (burst figure for a kernel
-    timed alone, sustained one for a path timed inside a long step), else the fallback of B200_PROFILING.md."""
+    timed alone, sustained one for a path timed inside a long step), else the H100 SXM data sheet (dense bf16, HBM3)."""
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.isfile(path):
         d = json.load(open(path))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "bf16_tflops_burst": d["bf16_tflops"], "source": "MEASURED_PEAKS.json"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1400.0, "bf16_tflops_burst": 1400.0, "source": "fallback (B200_PROFILING.md)"}
-
-
-def ncu_traffic(kernel):
-    """DRAM bytes per launch of `kernel` from the committed `ncu --set full` capture (profiles/traffic.json), or None."""
-    path = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.isfile(path):
-        return json.load(open(path)).get(kernel, {}).get("dram_bytes_per_launch")
-    return None
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_burst": 989.0, "source": "H100 SXM data sheet"}
 
 
 def kernel_rooflines(pipe, extract_bsz, dev):
     """The two kernels that dominate the step, each timed ALONE with CUDA events on the stream it is launched on
     (10 launches after 3 warm-ups, L2 flushed by a 256 MB write before every launch), through the library's unit entry
     points -- the same kernels, shapes and epilogues the timed region launches:
-      * gemm_tn_cg2_kernel (bf16 tcgen05 GEMM on CTA pairs): the four GEMMs of one ViT-B block at the extraction batch
+      * gemm_wgmma_kernel (bf16 wgmma GEMM): the four GEMMs of one ViT-B block at the extraction batch
         (QKV, out-proj + LayerScale residual, fc1 + GELU, fc2 + LayerScale residual); algorithmic flops =
         SURVEY.md 8(d) per-view figures (4.85 + 1.62 + 12.93 GF) x views per launch set;
       * fit_adam_table_kernel (dense Adam sweep of the hash table): algorithmic bytes = 24 B x 19 741 760 parameters."""
@@ -142,7 +137,7 @@ def kernel_rooflines(pipe, extract_bsz, dev):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled every 200 ms during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled every 200 ms during the timed region."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -190,7 +185,7 @@ def usable_cpus() -> int:
 
 
 def workload_config(args, world: int) -> dict:
-    """`config` of the JSON line -- identical for the B200 arm and the reference arm (same workload, same sizes)."""
+    """`config` of the JSON line -- identical for the GPU arm and the reference arm (same workload, same sizes)."""
     return {"workload": "stage1_vitb14_518_768views_2000iters", "views_per_image": args.views + 1,
             "fit_iters": args.num_iters, "fit_warmup_iters": args.warmup_iters, "pixel_bsz": 2048, "n_levels": 16,
             "extract_bsz": args.extract_bsz, "images_per_gpu": args.steps,
@@ -261,7 +256,7 @@ class CpuReference:
 
 
 def cpu_reference_rate(args, views_sample: int = 4, fit_steps: int = 10):
-    """`cpu_baseline` of the B200 line: ~10-30 s of CPU work (4 views, 10 + 10 timed steps)."""
+    """`cpu_baseline` of the GPU line: ~10-30 s of CPU work (4 views, 10 + 10 timed steps)."""
     return CpuReference(args).measure(views_sample, fit_steps)
 
 
@@ -297,7 +292,7 @@ def run_reference_arm(args, rank):
 
 
 # ------------------------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # ------------------------------------------------------------------------------------------------------------
 def synthetic_coords(V, h, w, seed, device):
     """Seeded crop-box stream (scale in [0.1, 0.5], ratio in [3/4, 4/3], p(flip) = 0.5) -> patch coordinates in [0,1];
@@ -345,6 +340,7 @@ def main():
         dist.init_process_group("nccl", device_id=dev)
 
     V = args.views + 1
+    torch.manual_seed(0)  # the randomly initialised ViT: identical weights from run to run
     vit = DVT.PretrainedViTWrapper(MODEL, stride=14, allow_random_init=True)
     with torch.no_grad():
         for b in vit.model.blocks:  # non-degenerate LayerScale (DINOv2 init 1e-5 would switch the blocks off)
@@ -369,10 +365,14 @@ def main():
     ev = lambda: torch.cuda.Event(enable_timing=True)  # noqa: E731
     seg = []   # ("hp1" | "hp2", start, end) CUDA events recorded on the stream that runs the path
 
+    last_out = {}
+
     def run_batch(first, n, views, record=False, to_host=False):
         """n images through the public stage-1 call (Stage1Pipeline.run_images): the bank extraction of image i+1 runs
         beside the fit of image i, everything else is ordered by the data dependencies."""
         def finalize(i, out):
+            if record:
+                last_out.update(out)
             if to_host:
                 return out["denoised_feats"].cpu(), out["raw"].cpu()
             return out["denoised_feats"]
@@ -408,6 +408,10 @@ def main():
         run_batch(0, args.warmup, views_dev)
     ms_total, clocks, launches = timed(lambda first, n: run_batch(first, n, views_dev, record=True), args.steps, collate=True)
     torch.cuda.synchronize()
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name in ("denoised_feats", "raw"):  # 2 x 4.2 MB
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), last_out[name].float().cpu().numpy())
     value = world * args.steps / (ms_total / 1000.0)
     # per-path durations INSIDE the timed region (the two paths of neighbouring images overlap, so they do not add up
     # to ms_per_step; each is stretched by the other's share of the SMs / HBM)
@@ -463,16 +467,15 @@ def main():
         pk = peaks()
         n_p2 = args.num_iters - 1 - int(0.5 * args.num_iters)
         n_p1 = args.num_iters - n_p2
-        # kernel level (the contract).  Largest shares of the ncu launch list of this command
-        # (profiles/*_launch_shares.txt): the dense Adam sweep, then the bf16 GEMM.
+        # kernel level: the dense Adam sweep and the bf16 GEMM.
         gemm = {"bound": "tensor", "achieved": kr["gemm_tflops"], "peak": pk["bf16_tflops_burst"], "unit": "TFLOP/s",
-                    "frac": kr["gemm_tflops"] / pk["bf16_tflops_burst"], "traffic": ncu_traffic("gemm_tn_cg2_kernel"),
-                    "kernel": "gemm_tn_cg2_kernel (bf16 tcgen05 cta_group::2 GEMM on CTA pairs, the 4 GEMMs of one ViT-B block)",
+                    "frac": kr["gemm_tflops"] / pk["bf16_tflops_burst"], "traffic": None,
+                    "kernel": "gemm_wgmma_kernel (bf16 wgmma GEMM, the 4 GEMMs of one ViT-B block)",
                     "algorithmic_flops_per_launch_set": kr["gemm_flops"], "ms_per_launch": kr["gemm_ms"],
                     "views_per_launch": args.extract_bsz, "timed": "alone, CUDA events, L2 flushed between launches",
                     "peak_source": pk["source"] + " (bf16 cuBLAS burst: kernel timed alone)"}
         dominant = {"bound": "hbm", "achieved": kr["sweep_gbs"], "peak": pk["hbm_gbs"], "unit": "GB/s",
-                    "frac": kr["sweep_gbs"] / pk["hbm_gbs"], "traffic": ncu_traffic("fit_adam_table_kernel"),
+                    "frac": kr["sweep_gbs"] / pk["hbm_gbs"], "traffic": None,
                     "kernel": "fit_adam_table_kernel (dense Adam sweep of the 19.74 M-parameter hash table), launched as in the "
                               f"timed region: {kr['sweep_ctas']} persistent 1024-thread CTAs (it shares the GPU with the GEMM "
                               "chains of the next two steps, so it is deliberately kept off the other SMs)",
@@ -487,7 +490,7 @@ def main():
         hp1_tf = V * FLOPS_PER_VIEW / (hp1_ms / 1e3) / 1e12
         hp2_gbs = (n_p1 * FIT_BYTES_P1 + n_p2 * FIT_BYTES_P2) / (hp2_ms / 1e3) / 1e9
         r1 = {"bound": "tensor", "achieved": hp1_tf, "peak": pk["bf16_tflops"], "unit": "TFLOP/s",
-              "frac": hp1_tf / pk["bf16_tflops"], "traffic": None, "kernel": "path HP-1: 769 ViT-B/14 forwards (tcgen05 GEMMs "
+              "frac": hp1_tf / pk["bf16_tflops"], "traffic": None, "kernel": "path HP-1: 769 ViT-B/14 forwards (wgmma GEMMs "
               "+ flash attention + LayerNorm)", "ms_per_image": hp1_ms, "peak_source": pk["source"] + " (sustained bf16 cuBLAS)"}
         r2 = {"bound": "hbm", "achieved": hp2_gbs, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": hp2_gbs / pk["hbm_gbs"],
               "traffic": None, "kernel": "path HP-2: 2000-step neural-field fit (SURVEY 8(d) algorithmic bytes / span)",

@@ -42,7 +42,6 @@ int hashgrid_fwd(int n_levels, const float* scale, const uint32_t* res, const ui
                  const uint32_t* hashed, const float* table, const float* coords, int n, float* out, cudaStream_t st);
 int hashgrid_bwd(int n_levels, const float* scale, const uint32_t* res, const uint32_t* size, const uint32_t* offset,
                  const uint32_t* hashed, const float* coords, int n, const float* dout, float* gtable, cudaStream_t st);
-void attention_set_debug_buffer(unsigned long long* p);
 int launch_attention_bwd(const __nv_bfloat16* qkv, const __nv_bfloat16* out, const __nv_bfloat16* dout, const float* lse,
                          __nv_bfloat16* dqkv, float* dq_acc, float* delta, int B, int N, int heads, cudaStream_t stream);
 int launch_layernorm_bwd(const float* x, const float* gamma, const float* dy, float* dx_accum, float* dgamma, float* dbeta,
@@ -80,8 +79,8 @@ int dvt_device_error(unsigned int* code_out) {
 long long dvt_launch_count(void) { return dvt::launch_count(); }
 
 int dvt_set_debug_impl(int impl) {
-  if (impl != 0 && impl != 1 && impl != 2 && impl != -1) {
-    dvt::set_last_error("dvt_set_debug_impl: impl must be -1, 0, 1 or 2");
+  if (impl != 0 && impl != 1 && impl != -1) {
+    dvt::set_last_error("dvt_set_debug_impl: impl must be -1, 0 or 1");
     return DVT_ERR_INVALID;
   }
   dvt::g_debug_impl_override = impl;
@@ -250,9 +249,6 @@ int dvt_gemm_bf16_ex(const void* A, int lda, int a_mn, const void* B, int ldb, i
 static unsigned long long* g_debug_ts = nullptr;
 int dvt_debug_set_timestamp_buffer(unsigned long long* dev_buf16) {
   g_debug_ts = dev_buf16;
-  // DVT_ATTN_DEBUG_TS=1: the buffer has 16 + 8 * 16 slots and the attention kernel records its per-tile milestones behind
-  // the first 16 (attention.cu: d_att_dbg; tools/attention_timeline.py)
-  if (getenv("DVT_ATTN_DEBUG_TS")) attention_set_debug_buffer(dev_buf16);
   return DVT_OK;
 }
 

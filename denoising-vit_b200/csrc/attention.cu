@@ -1,26 +1,20 @@
-// Multi-head self-attention forward for head_dim 64 on tcgen05 tensor cores (flash-style, O(N) memory).
+// Multi-head self-attention forward for head_dim 64 on Hopper tensor cores (flash-style, O(N) memory).
 //
 //   qkv  : bf16 [B, N, 3*C]  (the QKV projection output, C = heads*64; q at col h*64, k at C + h*64, v at 2C + h*64)
 //   out  : bf16 [B, N, C]    (col = h*64 + d; directly the A operand of the out-projection GEMM)
+//   lse  : optional f32 [B, heads, N], log2-domain log-sum-exp of the scaled scores (read by the backward kernel)
 //
-// One CTA per (query tile of 128 rows, head, image), 6 warps:
-//   warp 0     TMA producer: Q tile once, then K (1 slot) / V (2 slots) tiles of 128 keys x 64 (3-D tensor map
-//              over [3C, N, B]; keys past N are zero-filled)
-//   warp 1     MMA issuer: S = Q.K^T (M128 N128 K16 x4, K-major operands) into TMEM;
-//              O_j = P_j.V_j (M128 N64 K16 x8; P from smem K-major, V straight from its TMA tile as an MN-major
-//              operand) into one of two TMEM buffers
-//   warps 2-5  softmax: one thread per query row (TMEM lane = row): tcgen05.ld S, online max / exp2 / sum in
-//              fp32, P -> bf16 into 128B-swizzled smem.
-//              LAZY = true (default): O accumulates in TMEM across all key tiles; the running maximum a row uses is only
-//              raised when it grows by more than 2^8 (then the row's O is rescaled in TMEM: tcgen05.ld / st, a rare,
-//              warp-uniform branch), so the S tile is read from TMEM once, lives in registers, and there is no per-tile
-//              fold of O.  exp2(s - m_stale) <= 256 is harmless in fp32 / bf16 and cancels in the final O / l.
-//              LAZY = false (DVT_ATTN_LAZY=0): O accumulated in registers (acc = (acc + O_{j-1}) * alpha), two O buffers.
+// One CTA per (query tile of 128 rows, head, image), 9 warps:
+//   warps 0-7  two consumer warpgroups, 64 query rows each.  Per key tile of 128 keys: S = Q.K^T (wgmma m64n128k16,
+//              Q and K K-major from their TMA tiles), online softmax on the accumulator registers (row max / sum over the
+//              four threads that share a row), P -> bf16 registers, O += P.V (wgmma m64n64k16 with A = P from registers,
+//              B = V as an MN-major operand straight from its TMA tile).  O stays in registers; its rescaling by
+//              exp2(m_old - m_new) is one multiply per element and key tile.
+//   warp 8     TMA producer: Q once, then K / V tiles of 128 keys x 64 through a two-stage ring (3-D tensor map over
+//              [3C, N, B]; keys past N are zero-filled and masked out of the softmax).
 // Reference semantics: timm Attention.forward, restated at evaluation/vitdet/vision_transformer.py:73-91
 // (scale d^-0.5, no mask, softmax over keys).
 #include "common.cuh"
-
-#include <cstdlib>
 
 namespace dvt {
 
@@ -29,33 +23,13 @@ namespace {
 constexpr int ATT_D = 64;
 constexpr int ATT_BQ = 128;
 constexpr int ATT_BK = 128;
-constexpr int ATT_THREADS = 192;
+constexpr int ATT_THREADS = 288;
 constexpr int ATT_TILE_BYTES = 128 * 128;  // 128 rows x 64 bf16
-// smem layout (offsets from a 1024-aligned base)
-// Sized so that TWO CTAs are resident per SM (<= 113 KB smem, 256 TMEM columns each): the softmax of one CTA overlaps
-// the tensor-core work of the other, which hides most of the exp/max latency a single softmax warpgroup exposes.
-// KST = K stages.  With ONE (round 1) the load of K_{j+1} can only be issued when QK_j has completed, and S_{j+1} cannot be
-// computed before it lands: the kernel ran at one TMA round trip (1.5-2 us under load) per key tile -- 4700 clk per tile
-// against ~2000 of softmax.  With TWO, K_{j+1} is requested a whole tile ahead.  The second stage only fits beside a
-// second resident CTA without the 1 KB alignment slack and without the PAIR-mode exchange buffer (2 x (112 KB + 1 KB) per SM).
 constexpr int ATT_OFF_Q = 0;
-constexpr int ATT_OFF_K = ATT_OFF_Q + ATT_TILE_BYTES;
-constexpr int ATT_NUM_BARS = 1 + 2 + 2 + 2 + 2 + 1 + 1 + 1 + 2;
-template <int KST, bool PAIR>
-struct AttSmem {
-  static constexpr int OFF_V = ATT_OFF_K + KST * ATT_TILE_BYTES;    // 2 stages
-  static constexpr int OFF_P = OFF_V + 2 * ATT_TILE_BYTES;          // 1 buffer x 2 k-atoms x 16 KB
-  static constexpr int OFF_BAR = OFF_P + 2 * ATT_TILE_BYTES;
-  static constexpr int OFF_TMEM = OFF_BAR + ATT_NUM_BARS * 8;
-  static constexpr int OFF_XCH = OFF_TMEM + 16;                     // PAIR mode: row-max / row-sum exchange, [2 parity][2 half][128]
-  static constexpr bool SLACK = KST == 1;                           // KST == 2: the dynamic smem base must be 1024-aligned (checked)
-  static constexpr int TOTAL = OFF_XCH + (PAIR ? 2 * 2 * 128 * 4 : 0) + (SLACK ? 1024 : 0);
-};
-static_assert(2 * (AttSmem<2, false>::TOTAL + 1024) <= 228 * 1024, "two CTAs with two K stages must fit one SM");
-// TMEM columns: S [0,128) O0 [128,192) O1 [192,256)
-constexpr uint32_t ATT_TMEM_COLS = 256;
-constexpr uint32_t ATT_TM_S = 0, ATT_TM_O = 128;
-constexpr uint32_t ATT_TM_P = 192;   // MODE 5: P (bf16 pairs, 64 columns) as the TMEM A operand of P.V
+constexpr int ATT_OFF_K = ATT_OFF_Q + ATT_TILE_BYTES;      // 2 stages
+constexpr int ATT_OFF_V = ATT_OFF_K + 2 * ATT_TILE_BYTES;  // 2 stages
+constexpr int ATT_OFF_BAR = ATT_OFF_V + 2 * ATT_TILE_BYTES;
+constexpr int ATT_SMEM = ATT_OFF_BAR + 5 * 8 + 1024;  // + alignment slack
 
 __device__ __forceinline__ float ex2(float x) {
   float y;
@@ -63,72 +37,18 @@ __device__ __forceinline__ float ex2(float x) {
   return y;
 }
 
-// MODE 0: O accumulated in registers.  MODE 1 (LAZY): O in TMEM, lazy rescaling, one softmax thread per query row.
-// MODE 2 (LAZY + PAIR): as MODE 1 with TWO threads per query row (8 softmax warps: warp w and w + 4 share a TMEM lane
-// quadrant and take 64 of the 128 keys of a tile each; row maxima / sums are exchanged through shared memory) -- twice
-// the warps per scheduler to hide the ALU / MUFU / TMEM latencies the single thread per row exposes.
-// exp2 on the FMA / ALU pipes (range reduction by the 1.5 * 2^23 trick + degree-4 polynomial of 2^f on [-0.5, 0.5],
-// relative error 4e-5 -- P is rounded to bf16 (4e-3) right after): the MUFU (XU) pipe is the busiest unit of this kernel
-// (ncu: 50 %), so MODE 3 evaluates one exponential in four here instead of with ex2.approx.
-__device__ __forceinline__ float ex2_fma(float x) {
-  x = fmaxf(x, -120.0f);
-  const float r = x + 12582912.0f;     // round-to-nearest integer n of x sits in the low mantissa bits of r
-  const float f = x - (r - 12582912.0f);
-  float p = 0.0096181291f;
-  p = fmaf(p, f, 0.0555041087f);
-  p = fmaf(p, f, 0.2402265070f);
-  p = fmaf(p, f, 0.6931471806f);
-  p = fmaf(p, f, 1.0f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(r) << 23));   // p * 2^n
-}
-
-// Profiling aid (dvt_debug_set_timestamp_buffer with >= 16 + 8 * 16 slots): clock64 milestones of CTA (0, 0, 0), per key tile
-// j < 16 at slot 16 + 8 j + k -- softmax warp 2: 0 waiting for S_j, 1 S_j ready, 2 S_j in registers, 3 P_j computed,
-// 4 PV_{j-1} done, 5 P_j stored; MMA warp: 6 QK_{j+1} issued, 7 PV_j issued.
-// MODE 4 (round 2): MODE 1 with the per-element arithmetic in packed fp32 pairs (FFMA2 for s * scale - m, FADD2 for the
-// row sums): 3.0 instead of 4.0 issue slots per score (FMNMX3/2 + FFMA2/2 + MUFU + FADD2/2 + F2FP/2); the softmax warps
-// are issue / latency bound (profiles/r2z_attention_timeline.txt), not MUFU bound.  Measured 0.366 -> 0.352 ms (default).
-// MODE 5: MODE 4 with P handed to the tensor core through TENSOR MEMORY (tcgen05.st into columns [192, 256), P.V issued
-// with the A operand from TMEM) instead of a swizzled shared-memory tile: no 32 KB st.shared per tile, no
-// fence.proxy.async, no shared-memory operand reads for A (the timeline charges ~570 clk per key tile to that hand-over).
-// Parity-green, measured SLOWER (0.416 ms, profiles/r2z10_attention_epilogue_ab.txt): kept as a tested experiment.
-// MODE 6: MODE 4 with each 32-key chunk of P stored to shared memory as soon as it is packed (the stores drain under the
-// remaining exponentials, the proxy fence at the end only has the last chunk to wait for, 48 fewer live registers), and the
-// wait for PV_{j-1} (P buffer free) moved in front of the exponentials -- by then PV_{j-1} has had the S load and the
-// row-max pass to finish.  The rare rescaling of O stays behind the exponentials (it needs 64 registers).
-// Parity-green, measured 0.364 ms against 0.352 ms of MODE 4 (profiles/r2z11_validate.txt): not adopted.
-__device__ unsigned long long* d_att_dbg = nullptr;
-
-template <int MODE, int KST = 1>
-__global__ void __launch_bounds__(MODE == 2 ? 320 : ATT_THREADS, 2)
+__global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_tc_kernel(const __grid_constant__ CUtensorMap tm_qkv, __nv_bfloat16* __restrict__ out, int N, int C,
                     float scale_log2e, float* __restrict__ lse) {
-  constexpr bool LAZY = MODE >= 1;
-  constexpr bool PAIR = MODE == 2;
-  constexpr bool POLY = MODE == 3;   // MODE 3 = MODE 1 with a quarter of the exponentials on the FMA pipe
-  constexpr bool PK = MODE >= 4;     // packed fp32 pairs in the exponent / row-sum arithmetic
-  constexpr bool EARLY = MODE == 6;  // P stored chunk by chunk under the exponentials, PV_{j-1} awaited before them
-  constexpr bool PTM = MODE == 5;    // P through tensor memory
-  constexpr int NSOFT = PAIR ? 256 : 128;  // softmax threads
-  using L = AttSmem<KST, PAIR>;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = L::SLACK ? reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023)) : smem_raw;
-  if (!L::SLACK && (smem_u32(smem_raw) & 1023u) != 0) dev_fail(0xA11Du, 0);  // swizzled TMA tiles need 1024-byte alignment
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem + ATT_OFF_Q;
   uint8_t* sK = smem + ATT_OFF_K;
-  uint8_t* sV = smem + L::OFF_V;
-  uint8_t* sP = smem + L::OFF_P;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::OFF_BAR);
+  uint8_t* sV = smem + ATT_OFF_V;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + ATT_OFF_BAR);
   uint64_t* q_full = bars;
-  uint64_t* k_full = bars + 1;   // [2]
-  uint64_t* k_empty = bars + 3;  // [2]
-  uint64_t* v_full = bars + 5;   // [2]
-  uint64_t* v_empty = bars + 7;  // [2]
-  uint64_t* s_full = bars + 9;
-  uint64_t* s_empty = bars + 10;
-  uint64_t* p_full = bars + 11;
-  uint64_t* o_full = bars + 12;  // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + L::OFF_TMEM);
+  uint64_t* kv_full = bars + 1;   // [2]
+  uint64_t* kv_empty = bars + 3;  // [2]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -136,521 +56,131 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap tm_qkv, __nv_bfloat16* _
   const int head = blockIdx.y;
   const int b = blockIdx.z;
   const int T = (N + ATT_BK - 1) / ATT_BK;  // key tiles
-  unsigned long long* dbg = (blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && lane == 0) ? d_att_dbg : nullptr;
-  // (compiled in with -DDVT_ATTN_TIMELINE only -- DVT_NVCC_EXTRA=-DDVT_ATTN_TIMELINE bash csrc/build.sh: the stamps sit in
-  // the hot loop of the softmax warps)
-  auto stamp = [&](int j, int k) {
-#ifdef DVT_ATTN_TIMELINE
-    if (dbg && j < 16) dbg[16 + 8 * j + k] = (unsigned long long)clock64();
-#else
-    (void)j; (void)k; (void)dbg;
-#endif
-  };
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tm_qkv);
     mbar_init(q_full, 1);
     for (int i = 0; i < 2; ++i) {
-      mbar_init(&k_full[i], 1);
-      mbar_init(&k_empty[i], 1);
-    }
-    mbar_init(s_full, 1);
-    mbar_init(s_empty, NSOFT);
-    mbar_init(p_full, NSOFT);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&v_full[i], 1);
-      mbar_init(&v_empty[i], 1);
-      mbar_init(&o_full[i], 1);
+      mbar_init(&kv_full[i], 1);
+      mbar_init(&kv_empty[i], 8);
     }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, ATT_TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();     // PDL: the set-up above overlapped the tail of the QKV GEMM
   pdl_trigger();
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       mbar_expect_tx(q_full, ATT_TILE_BYTES);
       tma_load_3d(sQ, &tm_qkv, q_full, head * ATT_D, q0, b);
       for (int j = 0; j < T; ++j) {
         const int st = j & 1;
-        const uint32_t ph = (j >> 1) & 1;
-        const int ks = j % KST;
-        mbar_wait_relaxed(&k_empty[ks], ((j / KST) & 1) ^ 1, 10);
-        mbar_expect_tx(&k_full[ks], ATT_TILE_BYTES);
-        tma_load_3d(sK + ks * ATT_TILE_BYTES, &tm_qkv, &k_full[ks], C + head * ATT_D, j * ATT_BK, b);
-        mbar_wait_relaxed(&v_empty[st], ph ^ 1, 11);
-        mbar_expect_tx(&v_full[st], ATT_TILE_BYTES);
-        tma_load_3d(sV + st * ATT_TILE_BYTES, &tm_qkv, &v_full[st], 2 * C + head * ATT_D, j * ATT_BK, b);
+        mbar_wait_relaxed(&kv_empty[st], ((j >> 1) & 1) ^ 1, 10);
+        mbar_expect_tx(&kv_full[st], 2 * ATT_TILE_BYTES);
+        tma_load_3d(sK + st * ATT_TILE_BYTES, &tm_qkv, &kv_full[st], C + head * ATT_D, j * ATT_BK, b);
+        tma_load_3d(sV + st * ATT_TILE_BYTES, &tm_qkv, &kv_full[st], 2 * C + head * ATT_D, j * ATT_BK, b);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = make_idesc(1, 128, 128, 0, 0);  // Q (K-major) x K (K-major)
-      constexpr uint32_t idesc_o = make_idesc(1, 128, 64, 0, 1);   // P (K-major) x V (MN-major)
-      auto issue_qk = [&](int j) {
-        const uint32_t ph = j & 1;
-        const int ks = j % KST;
-        mbar_wait(&k_full[ks], (j / KST) & 1, 12);
-        mbar_wait(s_empty, ph ^ 1, 13);
-        tc_fence_after();
-        const uint64_t da = make_smem_desc(smem_u32(sQ), 0, 1024, 2);
-        const uint64_t db = make_smem_desc(smem_u32(sK + ks * ATT_TILE_BYTES), 0, 1024, 2);
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_f16(tmem_base + ATT_TM_S, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc_s, k > 0);
-        umma_commit(&k_empty[ks]);
-        umma_commit(s_full);
-        stamp(j - 1, 6);
-      };
-      mbar_wait(q_full, 0, 14);
-      issue_qk(0);
-      for (int j = 0; j < T; ++j) {
-        if (j + 1 < T) issue_qk(j + 1);
-        const int st = j & 1;
-        const uint32_t ph = (j >> 1) & 1;
-        mbar_wait(&v_full[st], ph, 15);
-        mbar_wait(p_full, j & 1, 16);
-        tc_fence_after();
-        stamp(j, 7);
-        // P buffer: two K-atoms (keys 0-63, 64-127), each a [128 x 128B] swizzled tile
-        const uint32_t p_base = smem_u32(sP);
-        const uint32_t v_base = smem_u32(sV + st * ATT_TILE_BYTES);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const uint64_t da = make_smem_desc(p_base + (k >> 2) * ATT_TILE_BYTES + (k & 3) * 32, 0, 1024, 2);
-          // V tile rows are keys (K dim), 128 B each: 16 keys per MMA = 2048 B; 8-row groups 1024 B apart
-          const uint64_t db = make_smem_desc(v_base + k * 2048, 0, 1024, 2);
-          if (PTM) umma_f16_ts(tmem_base + ATT_TM_O, tmem_base + ATT_TM_P + k * 8, db, idesc_o, (j > 0) || (k > 0));
-          else if (LAZY) umma_f16(tmem_base + ATT_TM_O, da, db, idesc_o, (j > 0) || (k > 0));  // one O, all key tiles
-          else umma_f16(tmem_base + ATT_TM_O + st * 64, da, db, idesc_o, k > 0);
-        }
-        umma_commit(&v_empty[st]);
-        umma_commit(&o_full[LAZY ? 0 : st]);  // LAZY: "PV_j done" (P buffer and O free), phase j & 1
-      }
-    }
-  } else {
-    // ===================== softmax / accumulate / store =====================
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;  // query row within the tile == TMEM lane
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(quad * 32) << 16);
-    if constexpr (PAIR) {
-      const int half = (warp - 2) >> 2;   // keys [half * 64, half * 64 + 64) of every tile; O columns [half * 32, +32)
-      float* xch = reinterpret_cast<float*>(smem + L::OFF_XCH);
-      float m_run = -INFINITY, l_run = 0.f;  // l_run: this thread's half of the row sum
-      for (int j = 0; j < T; ++j) {
-        mbar_wait(s_full, j & 1, 17);
-        tc_fence_after();
-        uint32_t sreg[2][32];
-        tmem_ld_32x32(lane_addr + ATT_TM_S + half * 64, sreg[0]);
-        tmem_ld_32x32(lane_addr + ATT_TM_S + half * 64 + 32, sreg[1]);
-        tmem_ld_wait();
-        tc_fence_before();
-        mbar_arrive(s_empty);
-        const int kbase = j * ATT_BK + half * 64;
-        const bool partial = kbase + 64 > N;
-        float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};  // four independent chains
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          const int nval = partial ? N - kbase - c * 32 : 32;
-          if (nval >= 32) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) mx[i & 3] = fmaxf(mx[i & 3], __uint_as_float(sreg[c][i]));
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (i < nval) mx[i & 3] = fmaxf(mx[i & 3], __uint_as_float(sreg[c][i]));
-          }
-        }
-        const float m_loc = fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3]));
-        float* xj = xch + (j & 1) * 256;
-        xj[half * 128 + row] = m_loc;
-        asm volatile("bar.sync 1, 256;" ::: "memory");  // the eight softmax warps
-        const float m_tile = fmaxf(m_loc, xj[(half ^ 1) * 128 + row]) * scale_log2e;  // finite: >= 1 valid key per tile
-        const float m_new = fmaxf(m_run, m_tile);
-        const bool grow = m_new - m_run > 8.0f;
-        const float m_use = grow ? m_new : m_run;
-        const float alpha = grow ? ex2(m_run - m_new) : 1.0f;
-        float ls[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          const int nval = partial ? N - kbase - c * 32 : 32;
-          if (nval >= 32) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const float p0 = ex2(fmaf(__uint_as_float(sreg[c][2 * i]), scale_log2e, -m_use));
-              const float p1 = ex2(fmaf(__uint_as_float(sreg[c][2 * i + 1]), scale_log2e, -m_use));
-              ls[i & 3] += p0 + p1;
-              sreg[c][i] = pack_bf16x2(p0, p1);       // packed in place: sreg[c][0..15]
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              float p0 = 0.f, p1 = 0.f;
-              if (2 * i < nval) p0 = ex2(fmaf(__uint_as_float(sreg[c][2 * i]), scale_log2e, -m_use));
-              if (2 * i + 1 < nval) p1 = ex2(fmaf(__uint_as_float(sreg[c][2 * i + 1]), scale_log2e, -m_use));
-              ls[i & 3] += p0 + p1;
-              sreg[c][i] = pack_bf16x2(p0, p1);
-            }
-          }
-        }
-        if (j > 0) {
-          mbar_wait(&o_full[0], (j - 1) & 1, 18);  // PV_{j-1} done: P buffer and O are free
-          tc_fence_after();
-          if (__any_sync(0xffffffffu, grow)) {       // same rows, hence same decision, in both warps of the pair
-            uint32_t o[32];
-            tmem_ld_32x32(lane_addr + ATT_TM_O + half * 32, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int d = 0; d < 32; ++d) o[d] = __float_as_uint(__uint_as_float(o[d]) * alpha);
-            tmem_st_32x32(lane_addr + ATT_TM_O + half * 32, o);
-            tmem_st_wait();
-          }
-        }
-        // this thread's 64 keys = k-atom `half`, all eight 16-byte chunks of row `row`
-        uint8_t* atom = sP + half * ATT_TILE_BYTES + row * 128;
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const int chunk = (c * 4 + q) ^ (row & 7);
-            *reinterpret_cast<uint4*>(atom + chunk * 16) =
-                make_uint4(sreg[c][4 * q], sreg[c][4 * q + 1], sreg[c][4 * q + 2], sreg[c][4 * q + 3]);
-          }
-        }
-        fence_async_smem();
-        tc_fence_before();
-        mbar_arrive(p_full);
-        l_run = l_run * alpha + ((ls[0] + ls[1]) + (ls[2] + ls[3]));
-        m_run = m_use;
-      }
-      mbar_wait(&o_full[0], (T - 1) & 1, 19);
-      tc_fence_after();
-      uint32_t o[32];
-      tmem_ld_32x32(lane_addr + ATT_TM_O + half * 32, o);
-      tmem_ld_wait();
-      tc_fence_before();
-      float* xl = xch + (T & 1) * 256;               // the buffer the last tile did not use
-      xl[half * 128 + row] = l_run;
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      const float inv = 1.0f / (l_run + xl[(half ^ 1) * 128 + row]);
-      const int q = q0 + row;
-      if (q < N) {
-        __nv_bfloat16* dst = out + ((size_t)b * N + q) * C + head * ATT_D + half * 32;
-#pragma unroll
-        for (int d8 = 0; d8 < 4; ++d8) {
-          uint32_t w[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-            w[i] = pack_bf16x2(__uint_as_float(o[d8 * 8 + 2 * i]) * inv, __uint_as_float(o[d8 * 8 + 2 * i + 1]) * inv);
-          *reinterpret_cast<uint4*>(dst + d8 * 8) = make_uint4(w[0], w[1], w[2], w[3]);
-        }
-      }
-    } else if constexpr (LAZY) {
-      float m_run = -INFINITY;  // the maximum (of s * scale_log2e) this row's P / O / l are currently relative to
-      float l_run = 0.f;
-      for (int j = 0; j < T; ++j) {
-        if (warp == 2) stamp(j, 0);
-        mbar_wait(s_full, j & 1, 17);
-        tc_fence_after();
-        if (warp == 2) stamp(j, 1);
-        uint32_t sreg[4][32];
-#pragma unroll
-        for (int c = 0; c < 4; ++c) tmem_ld_32x32(lane_addr + ATT_TM_S + c * 32, sreg[c]);
-        tmem_ld_wait();
-        tc_fence_before();
-        mbar_arrive(s_empty);  // S_j lives in registers now: QK of tile j+1 may overwrite the TMEM buffer
-        if (warp == 2) stamp(j, 2);
-        const int kbase = j * ATT_BK;
-        const bool partial = kbase + ATT_BK > N;  // only the last tile can hold keys >= N
-        // eight independent maxima (a single running maximum is a chain of 128 dependent FMNMX: ~500 cycles of exposed
-        // latency per tile with only two softmax warps per scheduler)
-        float mx[8] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY, -INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          const int nval = partial ? N - kbase - c * 32 : 32;  // valid keys in this chunk (warp-uniform)
-          if (nval >= 32) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) mx[i & 7] = fmaxf(mx[i & 7], __uint_as_float(sreg[c][i]));
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (i < nval) mx[i & 7] = fmaxf(mx[i & 7], __uint_as_float(sreg[c][i]));
-          }
-        }
-        float m_tile = fmaxf(fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3])), fmaxf(fmaxf(mx[4], mx[5]), fmaxf(mx[6], mx[7])));
-        m_tile *= scale_log2e;                      // scale > 0: max commutes with the scaling
-        const float m_new = fmaxf(m_run, m_tile);  // finite: every tile has at least one valid key
-        const bool grow = m_new - m_run > 8.0f;     // (first tile: m_run = -inf)
-        const float m_use = grow ? m_new : m_run;
-        const float alpha = grow ? ex2(m_run - m_new) : 1.0f;  // 0 on the first tile
-        auto wait_pv = [&]() {
-          // PV_{j-1} must have completed before the P buffer is overwritten / O is rescaled
-          mbar_wait(&o_full[0], (j - 1) & 1, 18);
-          tc_fence_after();
-          if (warp == 2) stamp(j, 4);
-        };
-        auto store_p_chunk = [&](int c, const uint32_t (&pk)[16]) {
-          // keys [c*32, c*32+32) -> k-atom (c >> 1), 16B chunks ((c & 1) * 4 + q), q = 0..3
-          uint8_t* atom = sP + (c >> 1) * ATT_TILE_BYTES + row * 128;
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const int chunk = ((c & 1) * 4 + q) ^ (row & 7);
-            *reinterpret_cast<uint4*>(atom + chunk * 16) = make_uint4(pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
-          }
-        };
-        if constexpr (EARLY) {
-          if (j > 0) wait_pv();
-        }
-        uint32_t packed[4][16];              // keys [32 c, 32 c + 32) as bf16 pairs
-        float ls[4] = {0.f, 0.f, 0.f, 0.f};  // four independent partial row sums (same reason as the maxima)
-        float2 ls2[4] = {{0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}, {0.f, 0.f}};  // PK: (even key, odd key) partial sums
-        const float2 sc2 = make_float2(scale_log2e, scale_log2e), nm2 = make_float2(-m_use, -m_use);
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          const int nval = partial ? N - kbase - c * 32 : 32;
-          if (nval >= 32) {
-            if constexpr (PK) {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                const float2 x = ffma2(make_float2(__uint_as_float(sreg[c][2 * i]), __uint_as_float(sreg[c][2 * i + 1])), sc2, nm2);
-                const float2 pp = make_float2(ex2(x.x), ex2(x.y));
-                ls2[i & 3] = fadd2(ls2[i & 3], pp);
-                packed[c][i] = pack_bf16x2(pp.x, pp.y);
-              }
-            } else {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const float x0 = fmaf(__uint_as_float(sreg[c][2 * i]), scale_log2e, -m_use);
-              const float x1 = fmaf(__uint_as_float(sreg[c][2 * i + 1]), scale_log2e, -m_use);
-              const float p0 = ex2(x0);
-              const float p1 = (POLY && (i & 1)) ? ex2_fma(x1) : ex2(x1);
-              ls[i & 3] += p0 + p1;
-              packed[c][i] = pack_bf16x2(p0, p1);
-            }
-            }
-          } else {  // tail of the last key tile: keys >= N contribute neither to P nor to the row sum
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              float p0 = 0.f, p1 = 0.f;
-              if (2 * i < nval) p0 = ex2(fmaf(__uint_as_float(sreg[c][2 * i]), scale_log2e, -m_use));
-              if (2 * i + 1 < nval) p1 = ex2(fmaf(__uint_as_float(sreg[c][2 * i + 1]), scale_log2e, -m_use));
-              ls[i & 3] += p0 + p1;
-              packed[c][i] = pack_bf16x2(p0, p1);
-            }
-          }
-          if constexpr (EARLY) store_p_chunk(c, packed[c]);
-        }
-        float l_tile = (ls[0] + ls[1]) + (ls[2] + ls[3]);
-        if constexpr (PK) {
-          const float2 t = fadd2(fadd2(ls2[0], ls2[1]), fadd2(ls2[2], ls2[3]));
-          l_tile += t.x + t.y;
-        }
-        if (warp == 2) stamp(j, 3);
-        if (j > 0) {
-          if constexpr (!EARLY) wait_pv();
-          if (__any_sync(0xffffffffu, grow)) {  // rare after the first tiles; tcgen05.ld / st are warp-collective
-            uint32_t o[2][32];
-            tmem_ld_32x32(lane_addr + ATT_TM_O, o[0]);
-            tmem_ld_32x32(lane_addr + ATT_TM_O + 32, o[1]);
-            tmem_ld_wait();
-#pragma unroll
-            for (int d = 0; d < ATT_D; ++d) o[d >> 5][d & 31] = __float_as_uint(__uint_as_float(o[d >> 5][d & 31]) * alpha);
-            tmem_st_32x32(lane_addr + ATT_TM_O, o[0]);
-            tmem_st_32x32(lane_addr + ATT_TM_O + 32, o[1]);
-            tmem_st_wait();
-          }
-        }
-        if constexpr (PTM) {
-          // row `row` of P = TMEM lane `row`; column 192 + c holds keys (2c, 2c + 1): the K-major A operand of P.V
-          uint32_t h0[32], h1[32];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            h0[i] = packed[0][i]; h0[16 + i] = packed[1][i];
-            h1[i] = packed[2][i]; h1[16 + i] = packed[3][i];
-          }
-          tmem_st_32x32(lane_addr + ATT_TM_P, h0);
-          tmem_st_32x32(lane_addr + ATT_TM_P + 32, h1);
-          tmem_st_wait();
-        } else {
-        if constexpr (!EARLY) {
-#pragma unroll
-          for (int c = 0; c < 4; ++c) store_p_chunk(c, packed[c]);
-        }
-        fence_async_smem();  // generic-proxy writes of P -> visible to tcgen05.mma
-        }
-        tc_fence_before();
-        mbar_arrive(p_full);
-        if (warp == 2) stamp(j, 5);
-        l_run = l_run * alpha + l_tile;
-        m_run = m_use;
-      }
-      // O of all tiles
-      mbar_wait(&o_full[0], (T - 1) & 1, 19);
-      tc_fence_after();
-      uint32_t o[2][32];
-      tmem_ld_32x32(lane_addr + ATT_TM_O, o[0]);
-      tmem_ld_32x32(lane_addr + ATT_TM_O + 32, o[1]);
-      tmem_ld_wait();
-      tc_fence_before();
-      const float inv = 1.0f / l_run;
-      const int q = q0 + row;
-      if (q < N) {
-        // log-sum-exp of the scaled scores in the log2 domain (training: the backward kernel recomputes P from it):
-        // P[q, k] = exp2(s[q, k] * scale_log2e - lse[q]), layout [B, heads, N]
-        if (lse) lse[((size_t)b * gridDim.y + head) * N + q] = m_run + log2f(l_run);
-        __nv_bfloat16* dst = out + ((size_t)b * N + q) * C + head * ATT_D;
-#pragma unroll
-        for (int d8 = 0; d8 < 8; ++d8) {
-          uint32_t w[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int d = d8 * 8 + 2 * i;
-            w[i] = pack_bf16x2(__uint_as_float(o[d >> 5][d & 31]) * inv, __uint_as_float(o[(d + 1) >> 5][(d + 1) & 31]) * inv);
-          }
-          *reinterpret_cast<uint4*>(dst + d8 * 8) = make_uint4(w[0], w[1], w[2], w[3]);
-        }
-      }
-    } else {
-    float acc[ATT_D];
-#pragma unroll
-    for (int d = 0; d < ATT_D; ++d) acc[d] = 0.f;
-    float m_run = -INFINITY;  // running max of s * scale_log2e
-    float l_run = 0.f;
-    float alpha_prev = 0.f;   // rescale factor of the previous tile (acc is kept relative to the max BEFORE it)
-
-    for (int j = 0; j < T; ++j) {
-      mbar_wait(s_full, j & 1, 17);
-      tc_fence_after();
-      // ---- pass 1: row max over this tile (TMEM is re-read in pass 2: cheaper than 128 live registers) ----
-      const int kbase = j * ATT_BK;
-      const bool partial = kbase + ATT_BK > N;  // only the last tile can hold keys >= N
-      float m_tile = -INFINITY;
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t sreg[32];
-        tmem_ld_32x32(lane_addr + ATT_TM_S + c * 32, sreg);
-        tmem_ld_wait();
-        const int nval1 = partial ? N - kbase - c * 32 : 32;  // valid keys in this chunk (warp-uniform)
-        if (nval1 >= 32) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) m_tile = fmaxf(m_tile, __uint_as_float(sreg[i]));
-        } else {  // tail chunks of the last key tile only
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (i < nval1) m_tile = fmaxf(m_tile, __uint_as_float(sreg[i]));
-        }
-      }
-      m_tile *= scale_log2e;                      // scale > 0: max commutes with the scaling
-      const float m_new = fmaxf(m_run, m_tile);  // finite: every tile has at least one valid key
-      const float alpha = ex2(m_run - m_new);     // 0 on the first tile (m_run = -inf)
-      // ---- fold in the previous tile's O (also proves PV_{j-1} has finished reading the single P buffer) ----
-      if (j > 0) {
-        const int pst = (j - 1) & 1;
-        const uint32_t pph = ((j - 1) >> 1) & 1;
-        mbar_wait(&o_full[pst], pph, 18);
-        tc_fence_after();
-        uint32_t o[2][32];
-        tmem_ld_32x32(lane_addr + ATT_TM_O + pst * 64, o[0]);
-        tmem_ld_32x32(lane_addr + ATT_TM_O + pst * 64 + 32, o[1]);
-        tmem_ld_wait();
-        // acc (relative to m_{j-2}) * alpha_{j-1} + O_{j-1} (relative to m_{j-1}): one FFMA per element
-#pragma unroll
-        for (int d = 0; d < ATT_D; ++d) acc[d] = fmaf(acc[d], alpha_prev, __uint_as_float(o[d >> 5][d & 31]));
-      }
-      alpha_prev = alpha;
-      // ---- pass 2: p = exp2(s*scale - m_new), row sum, bf16 pack, swizzled store ----
-      float l_tile = 0.f;
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t sreg[32];
-        tmem_ld_32x32(lane_addr + ATT_TM_S + c * 32, sreg);
-        tmem_ld_wait();
-        if (c == 3) {
-          tc_fence_before();
-          mbar_arrive(s_empty);  // S may now be overwritten by QK of tile j+1
-        }
-        uint32_t packed[16];
-        const int nval = partial ? N - kbase - c * 32 : 32;  // valid keys in this chunk (warp-uniform)
-        if (nval >= 32) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const float p0 = ex2(fmaf(__uint_as_float(sreg[2 * i]), scale_log2e, -m_new));
-            const float p1 = ex2(fmaf(__uint_as_float(sreg[2 * i + 1]), scale_log2e, -m_new));
-            l_tile += p0 + p1;
-            packed[i] = pack_bf16x2(p0, p1);
-          }
-        } else {  // tail of the last key tile: keys >= N contribute neither to P nor to the row sum
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            float p0 = 0.f, p1 = 0.f;
-            if (2 * i < nval) p0 = ex2(fmaf(__uint_as_float(sreg[2 * i]), scale_log2e, -m_new));
-            if (2 * i + 1 < nval) p1 = ex2(fmaf(__uint_as_float(sreg[2 * i + 1]), scale_log2e, -m_new));
-            l_tile += p0 + p1;
-            packed[i] = pack_bf16x2(p0, p1);
-          }
-        }
-        // keys [c*32, c*32+32) -> k-atom (c >> 1), 16B chunks ((c & 1) * 4 + q), q = 0..3
-        uint8_t* atom = sP + (c >> 1) * ATT_TILE_BYTES + row * 128;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const int chunk = ((c & 1) * 4 + q) ^ (row & 7);
-          *reinterpret_cast<uint4*>(atom + chunk * 16) =
-              make_uint4(packed[4 * q], packed[4 * q + 1], packed[4 * q + 2], packed[4 * q + 3]);
-        }
-      }
-      fence_async_smem();  // generic-proxy writes of P -> visible to tcgen05.mma
-      tc_fence_before();
-      mbar_arrive(p_full);
-      l_run = l_run * alpha + l_tile;
-      m_run = m_new;
-    }
-    // last tile's O
-    {
-      const int pst = (T - 1) & 1;
-      const uint32_t pph = ((T - 1) >> 1) & 1;
-      mbar_wait(&o_full[pst], pph, 19);
-      tc_fence_after();
-      uint32_t o[2][32];
-      tmem_ld_32x32(lane_addr + ATT_TM_O + pst * 64, o[0]);
-      tmem_ld_32x32(lane_addr + ATT_TM_O + pst * 64 + 32, o[1]);
-      tmem_ld_wait();
-      tc_fence_before();
-      const float inv = 1.0f / l_run;
-      const int q = q0 + row;
-      if (q < N) {
-        __nv_bfloat16* dst = out + ((size_t)b * N + q) * C + head * ATT_D;
-#pragma unroll
-        for (int d8 = 0; d8 < 8; ++d8) {
-          uint32_t w[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int d = d8 * 8 + 2 * i;
-            const float a0 = fmaf(acc[d], alpha_prev, __uint_as_float(o[d >> 5][d & 31])) * inv;
-            const float a1 = fmaf(acc[d + 1], alpha_prev, __uint_as_float(o[(d + 1) >> 5][(d + 1) & 31])) * inv;
-            w[i] = pack_bf16x2(a0, a1);
-          }
-          *reinterpret_cast<uint4*>(dst + d8 * 8) = make_uint4(w[0], w[1], w[2], w[3]);
-        }
-      }
-    }
-    }  // !LAZY
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, ATT_TMEM_COLS);
+  // ===================== consumer warpgroups =====================
+  const int wg = warp >> 2;
+  const int t4 = lane & 3;
+  // this thread's two query rows (i = 0, 1) within the tile: accumulator rows of the wgmma layout
+  const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const uint64_t dq = make_wgmma_desc(smem_u32(sQ) + wg * 64 * 128, 0, 1024);
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY};  // running maximum of s * scale_log2e
+  float l_run[2] = {0.f, 0.f};              // this thread's share of the row sums
+  mbar_wait(q_full, 0, 14);
+  for (int j = 0; j < T; ++j) {
+    const int st = j & 1;
+    mbar_wait(&kv_full[st], (j >> 1) & 1, 15);
+    // ---- S = Q . K^T ----
+    float s[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) s[i] = 0.f;
+    const uint64_t dk = make_wgmma_desc(smem_u32(sK + st * ATT_TILE_BYTES), 0, 1024);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) wgmma_128_bf16<0, 0>(s, dq + (uint64_t)(2 * k), dk + (uint64_t)(2 * k));
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+    // ---- online softmax (keys >= N: -inf) ----
+    const int nval = N - j * ATT_BK;  // valid keys of this tile (>= 1)
+    if (nval < ATT_BK) {
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+        for (int c = 0; c < 2; ++c)
+          if (8 * jj + 2 * t4 + c >= nval) s[4 * jj + c] = s[4 * jj + 2 + c] = -INFINITY;
+    }
+    float alpha[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) mx = fmaxf(mx, fmaxf(s[4 * jj + 2 * i], s[4 * jj + 2 * i + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[i], mx * scale_log2e);  // scale > 0: max commutes with the scaling; finite
+      alpha[i] = ex2(m_run[i] - m_new);                       // 0 on the first tile (m_run = -inf)
+      m_run[i] = m_new;
+    }
+    uint32_t p[8][4];  // P as the register A operand of P.V: k16 step kk holds keys [16 kk, 16 kk + 16)
+    float ls[2] = {0.f, 0.f};
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const float p0 = ex2(fmaf(s[4 * jj + 2 * i], scale_log2e, -m_run[i]));
+        const float p1 = ex2(fmaf(s[4 * jj + 2 * i + 1], scale_log2e, -m_run[i]));
+        ls[i] += p0 + p1;
+        p[jj >> 1][(jj & 1) * 2 + i] = pack_bf16x2(p0, p1);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) l_run[i] = l_run[i] * alpha[i] + ls[i];
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      o[4 * jj] *= alpha[0];
+      o[4 * jj + 1] *= alpha[0];
+      o[4 * jj + 2] *= alpha[1];
+      o[4 * jj + 3] *= alpha[1];
+    }
+    // ---- O += P . V  (V rows are keys = the K dimension: 16 keys per MMA = 2048 B) ----
+    const uint64_t dv = make_wgmma_desc(smem_u32(sV + st * ATT_TILE_BYTES), 8192, 1024);
+    reg_fence(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) wgmma_64_bf16_rs<1>(o, p[kk], dv + (uint64_t)(kk * 2048 >> 4));
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&kv_empty[st]);  // K / V of this tile are no longer read
+  }
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    float l = l_run[i];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = 1.0f / l;
+    const int q = q0 + row0 + 8 * i;
+    if (q < N) {
+      // P[q, k] = exp2(s[q, k] * scale_log2e - lse[q]), layout [B, heads, N]
+      if (lse && t4 == 0) lse[((size_t)b * gridDim.y + head) * N + q] = m_run[i] + log2f(l);
+      __nv_bfloat16* dst = out + ((size_t)b * N + q) * C + head * ATT_D + 2 * t4;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+        *reinterpret_cast<uint32_t*>(dst + 8 * jj) = pack_bf16x2(o[4 * jj + 2 * i] * inv, o[4 * jj + 2 * i + 1] * inv);
+    }
   }
 }
 
@@ -705,7 +235,7 @@ int launch_attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int N,
   DVT_REQUIRE(B > 0 && N > 0 && heads > 0, "attention: bad shape B=%d N=%d heads=%d", B, N, heads);
   const float scale = 0.125f;  // 64^-0.5
   if (impl == 1) {
-    DVT_REQUIRE(lse == nullptr, "attention (simt debug): the log-sum-exp output needs the tcgen05 kernel");
+    DVT_REQUIRE(lse == nullptr, "attention (simt debug): the log-sum-exp output needs the tensor-core kernel");
     DVT_REQUIRE(N <= 12000, "attention (simt debug): N=%d too large", N);
     dim3 grid(N, heads, B);
     attention_simt_kernel<<<grid, 32, N * sizeof(float), stream>>>(qkv, out, N, C, scale);
@@ -714,54 +244,20 @@ int launch_attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int N,
     return DVT_OK;
   }
   static bool attr_set = false;  // (attention is never launched inside a stream capture)
-  static int mode = 4;  // DVT_ATTN_MODE: 0 O in registers, 1 lazy rescaling, 2 lazy + two threads per row, 3 lazy + a quarter
-                        // of the exponentials on the FMA pipe, 4 (default) lazy + packed fp32 pairs, 5 = 4 + P through TMEM,
-                        // 6 = 4 + P stored chunk by chunk under the exponentials
-  static int kst = 1;   // DVT_ATTN_KSTAGES: K stages of modes 1 / 3 (1 = the round-1 kernel)  [2: validated, measured neutral]
-  constexpr int T1 = AttSmem<1, false>::TOTAL, T1P = AttSmem<1, true>::TOTAL, T2 = AttSmem<2, false>::TOTAL;
   if (!attr_set) {
-    DVT_CUDA_OK(cudaFuncSetAttribute(attention_tc_kernel<0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, T1));
-    DVT_CUDA_OK(cudaFuncSetAttribute(attention_tc_kernel<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, T1));
-    DVT_CUDA_OK(cudaFuncSetAttribute(attention_tc_kernel<1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, T2));
-    DVT_CUDA_OK(cudaFuncSetAttribute(attention_tc_kernel<2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, T1P));
-    DVT_CUDA_OK(cudaFuncSetAttribute(attention_tc_kernel<3, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, T1));
-    DVT_CUDA_OK(cudaFuncSetAttribute(attention_tc_kernel<3, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, T2));
-    DVT_CUDA_OK(cudaFuncSetAttribute(attention_tc_kernel<4, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, T1));
-    DVT_CUDA_OK(cudaFuncSetAttribute(attention_tc_kernel<5, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, T1));
-    DVT_CUDA_OK(cudaFuncSetAttribute(attention_tc_kernel<6, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, T1));
-    const char* v = getenv("DVT_ATTN_MODE");
-    if (v && v[0] >= '0' && v[0] <= '6') mode = v[0] - '0';
-    const char* k = getenv("DVT_ATTN_KSTAGES");
-    if (k && (k[0] == '1' || k[0] == '2')) kst = k[0] - '0';
-    if (kst == 2) {  // the second K stage must not cost the second resident CTA
-      int per_sm = 0;
-      DVT_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, attention_tc_kernel<1, 2>, ATT_THREADS, (size_t)T2));
-      if (per_sm < 2) kst = 1;
-    }
+    DVT_CUDA_OK(cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
     attr_set = true;
   }
-  DVT_REQUIRE(lse == nullptr || mode == 1 || mode >= 4, "attention: the log-sum-exp output is implemented by DVT_ATTN_MODE=1, 4, 5");
   CUtensorMap tm;
   int rc = make_tmap_3d(&tm, qkv, TMAP_BF16, (uint64_t)3 * C, (uint64_t)N, (uint64_t)B, (uint64_t)3 * C * 2,
                         (uint64_t)N * 3 * C * 2, ATT_D, ATT_BK);
   if (rc) return rc;
   dim3 grid((N + ATT_BQ - 1) / ATT_BQ, heads, B);
   const float sl2 = scale * 1.4426950408889634f;
-  const dim3 blk(ATT_THREADS);
-  if (mode == 6) DVT_CUDA_OK(launch_k(g_vit_pdl, attention_tc_kernel<6, 1>, grid, blk, (size_t)T1, stream, tm, out, N, C, sl2, lse));
-  else if (mode == 5) DVT_CUDA_OK(launch_k(g_vit_pdl, attention_tc_kernel<5, 1>, grid, blk, (size_t)T1, stream, tm, out, N, C, sl2, lse));
-  else if (mode == 4) DVT_CUDA_OK(launch_k(g_vit_pdl, attention_tc_kernel<4, 1>, grid, blk, (size_t)T1, stream, tm, out, N, C, sl2, lse));
-  else if (mode == 3 && kst == 2) DVT_CUDA_OK(launch_k(g_vit_pdl, attention_tc_kernel<3, 2>, grid, blk, (size_t)T2, stream, tm, out, N, C, sl2, lse));
-  else if (mode == 3) DVT_CUDA_OK(launch_k(g_vit_pdl, attention_tc_kernel<3, 1>, grid, blk, (size_t)T1, stream, tm, out, N, C, sl2, lse));
-  else if (mode == 2) DVT_CUDA_OK(launch_k(g_vit_pdl, attention_tc_kernel<2, 1>, grid, dim3(320), (size_t)T1P, stream, tm, out, N, C, sl2, lse));
-  else if (mode == 1 && kst == 2) DVT_CUDA_OK(launch_k(g_vit_pdl, attention_tc_kernel<1, 2>, grid, blk, (size_t)T2, stream, tm, out, N, C, sl2, lse));
-  else if (mode == 1) DVT_CUDA_OK(launch_k(g_vit_pdl, attention_tc_kernel<1, 1>, grid, blk, (size_t)T1, stream, tm, out, N, C, sl2, lse));
-  else DVT_CUDA_OK(launch_k(g_vit_pdl, attention_tc_kernel<0, 1>, grid, blk, (size_t)T1, stream, tm, out, N, C, sl2, lse));
+  DVT_CUDA_OK(launch_k(g_vit_pdl, attention_tc_kernel, grid, dim3(ATT_THREADS), (size_t)ATT_SMEM, stream, tm, out, N, C, sl2, lse));
   DVT_CUDA_OK(cudaGetLastError());
   count_launch();
   return DVT_OK;
 }
-
-void attention_set_debug_buffer(unsigned long long* p) { cudaMemcpyToSymbol(d_att_dbg, &p, sizeof(p)); }
 
 }  // namespace dvt

@@ -1,4 +1,4 @@
-// Multi-head self-attention BACKWARD for head_dim 64 on tcgen05 tensor cores (flash-style: S and P are recomputed per
+// Multi-head self-attention BACKWARD for head_dim 64 on Hopper tensor cores (flash-style: S and P are recomputed per
 // tile from Q, K and the log-sum-exp the forward kernel saved; nothing of size N x N touches HBM).
 // Used by the stage-2 training step (reference: loss.backward() through timm Attention inside the `Denoiser` block,
 // dvt/models/online_denoiser.py:25-36,90; main_denoiser.py:216-220).
@@ -7,17 +7,16 @@
 //   dout  : bf16 [B, N, C]    gradient of the attention output
 //   lse   : f32  [B, H, N]    log2-domain log-sum-exp of the scaled scores, written by attention_tc_kernel
 //   delta : f32  [B, H, N]    rowsum(dout * out)  (attn_delta_kernel)
-//   dqkv  : bf16 [B, N, 3C]   dk, dv written here; dq accumulates in dq_acc f32 [B, N, C] (one atomic per key tile)
+//   dqkv  : bf16 [B, N, 3C]   dk, dv written here; dq accumulates in dq_acc f32 [B, N, C] (fp32 reductions)
 //
-// One CTA per (key tile of 128 keys, head, image), 6 warps; it loops over the query tiles i:
-//   warp 0     TMA producer: K_j, V_j once; Q_i and dO_i through a two-stage ring
-//   warp 1     MMA issuer:   S = Q_i K_j^T and dP = dO_i V_j^T (M128 N128, K-major operands) into TMEM;
-//                            dV_j += P^T dO_i, dK_j += dS^T Q_i (P / dS read as MN-major A, dO / Q as MN-major B straight
-//                            from their TMA tiles), dQ_i = dS K_j (dS K-major A, K_j MN-major B)
-//   warps 2-5  one thread per query row (= TMEM lane): P = exp2(S * scale*log2e - lse), dS = P * (dP - delta) * scale,
-//              both -> bf16 into 128B-swizzled smem (the layout of the forward's P buffer, which serves the K-major and the
-//              MN-major reading alike); dQ_i: TMEM -> red.global.add.v4.f32; at the end dK_j, dV_j: TMEM -> bf16 -> HBM.
-// TMEM columns: S [0,128) dP [128,256) dV [256,320) dK [320,384) dQ [384,448).
+// One CTA per (key tile of 128 keys, head, image), 9 warps; it loops over the query tiles i of 64 queries:
+//   warps 0-7  two consumer warpgroups, 64 keys each, all in registers (wgmma accumulator layout, row = key):
+//              S^T = K_j Q_i^T and dP^T = V_j dO_i^T (m64n64k16, K-major operands from the TMA tiles);
+//              P^T = exp2(S^T * scale*log2e - lse), dS^T = P^T * (dP^T - delta) * scale;
+//              dV_j += P^T dO_i and dK_j += dS^T Q_i (A from registers, dO / Q as MN-major B operands);
+//              dQ_i += dS K_j over this warpgroup's 64 keys (dS^T staged in swizzled smem as an MN-major A operand,
+//              K_j as an MN-major B operand) -> fp32 reductions into dq_acc.
+//   warp 8     TMA producer: K_j, V_j once; Q_i and dO_i through a two-stage ring.
 #include "common.cuh"
 
 namespace dvt {
@@ -25,21 +24,18 @@ namespace dvt {
 namespace {
 
 constexpr int AB_D = 64;
-constexpr int AB_T = 128;                      // tile edge (queries and keys)
-constexpr int AB_THREADS = 192;
-constexpr int AB_TILE = 128 * 128;             // bytes of a [128 x 64] bf16 tile
+constexpr int AB_T = 128;                      // keys per CTA
+constexpr int AB_TQ = 64;                      // queries per iteration
+constexpr int AB_THREADS = 288;
+constexpr int AB_KV_TILE = 128 * 128;          // bytes of a [128 x 64] bf16 tile
+constexpr int AB_Q_TILE = 64 * 128;            // bytes of a [64 x 64] bf16 tile
 constexpr int AB_OFF_K = 0;
-constexpr int AB_OFF_V = AB_OFF_K + AB_TILE;
-constexpr int AB_OFF_Q = AB_OFF_V + AB_TILE;       // 2 stages
-constexpr int AB_OFF_DO = AB_OFF_Q + 2 * AB_TILE;  // 2 stages
-constexpr int AB_OFF_P = AB_OFF_DO + 2 * AB_TILE;  // 2 key atoms x 16 KB
-constexpr int AB_OFF_DS = AB_OFF_P + 2 * AB_TILE;
-constexpr int AB_OFF_BAR = AB_OFF_DS + 2 * AB_TILE;
-constexpr int AB_NUM_BARS = 1 + 2 + 2 + 1 + 1 + 1 + 1 + 1;
-constexpr int AB_OFF_TMEM = AB_OFF_BAR + AB_NUM_BARS * 8;
-constexpr int AB_SMEM_TOTAL = AB_OFF_TMEM + 16 + 1024;
-constexpr uint32_t AB_TMEM_COLS = 512;
-constexpr uint32_t AB_TM_S = 0, AB_TM_DP = 128, AB_TM_DV = 256, AB_TM_DK = 320, AB_TM_DQ = 384;
+constexpr int AB_OFF_V = AB_OFF_K + AB_KV_TILE;
+constexpr int AB_OFF_Q = AB_OFF_V + AB_KV_TILE;     // 2 stages
+constexpr int AB_OFF_DO = AB_OFF_Q + 2 * AB_Q_TILE; // 2 stages
+constexpr int AB_OFF_DS = AB_OFF_DO + 2 * AB_Q_TILE; // one [64 keys x 64 queries] tile per warpgroup
+constexpr int AB_OFF_BAR = AB_OFF_DS + 2 * AB_Q_TILE;
+constexpr int AB_SMEM_TOTAL = AB_OFF_BAR + 5 * 8 + 1024;
 
 __device__ __forceinline__ float ab_ex2(float x) {
   float y;
@@ -48,236 +44,176 @@ __device__ __forceinline__ float ab_ex2(float x) {
 }
 
 __global__ void __launch_bounds__(AB_THREADS, 1)
-attention_bwd_tc_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do,
-                        const float* __restrict__ lse, const float* __restrict__ delta, __nv_bfloat16* __restrict__ dqkv,
-                        float* __restrict__ dq_acc, int N, int C, int H, float scale, float scale_log2e) {
+attention_bwd_tc_kernel(const __grid_constant__ CUtensorMap tm_kv, const __grid_constant__ CUtensorMap tm_q,
+                        const __grid_constant__ CUtensorMap tm_do, const float* __restrict__ lse,
+                        const float* __restrict__ delta, __nv_bfloat16* __restrict__ dqkv, float* __restrict__ dq_acc, int N,
+                        int C, int H, float scale, float scale_log2e) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sK = smem + AB_OFF_K;
   uint8_t* sV = smem + AB_OFF_V;
   uint8_t* sQ = smem + AB_OFF_Q;
   uint8_t* sDO = smem + AB_OFF_DO;
-  uint8_t* sP = smem + AB_OFF_P;
-  uint8_t* sDS = smem + AB_OFF_DS;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + AB_OFF_BAR);
   uint64_t* kv_full = bars;
   uint64_t* qd_full = bars + 1;    // [2]
   uint64_t* qd_empty = bars + 3;   // [2]
-  uint64_t* s_full = bars + 5;     // S and dP of the current query tile are in TMEM
-  uint64_t* s_empty = bars + 6;    // ... and have been read by all 128 row threads
-  uint64_t* p_full = bars + 7;     // P and dS are in shared memory
-  uint64_t* mma2_done = bars + 8;  // dV / dK / dQ MMAs of a query tile complete: P / dS smem free, dQ readable
-  uint64_t* dq_empty = bars + 9;   // dQ has been read out of TMEM
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + AB_OFF_TMEM);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int j = blockIdx.x;                 // key tile
   const int head = blockIdx.y;
   const int b = blockIdx.z;
-  const int T = (N + AB_T - 1) / AB_T;      // query tiles
+  const int T = (N + AB_TQ - 1) / AB_TQ;    // query tiles
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tm_qkv);
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&tm_kv);
+    tma_prefetch_desc(&tm_q);
     tma_prefetch_desc(&tm_do);
     mbar_init(kv_full, 1);
     for (int i = 0; i < 2; ++i) {
       mbar_init(&qd_full[i], 1);
-      mbar_init(&qd_empty[i], 1);
+      mbar_init(&qd_empty[i], 8);
     }
-    mbar_init(s_full, 1);
-    mbar_init(s_empty, 128);
-    mbar_init(p_full, 128);
-    mbar_init(mma2_done, 1);
-    mbar_init(dq_empty, 128);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, AB_TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===================== TMA producer =====================
     if (lane == 0) {
-      mbar_expect_tx(kv_full, 2 * AB_TILE);
-      tma_load_3d(sK, &tm_qkv, kv_full, C + head * AB_D, j * AB_T, b);
-      tma_load_3d(sV, &tm_qkv, kv_full, 2 * C + head * AB_D, j * AB_T, b);
+      mbar_expect_tx(kv_full, 2 * AB_KV_TILE);
+      tma_load_3d(sK, &tm_kv, kv_full, C + head * AB_D, j * AB_T, b);
+      tma_load_3d(sV, &tm_kv, kv_full, 2 * C + head * AB_D, j * AB_T, b);
       for (int i = 0; i < T; ++i) {
         const int st = i & 1;
         mbar_wait_relaxed(&qd_empty[st], ((i >> 1) & 1) ^ 1, 0x60);
-        mbar_expect_tx(&qd_full[st], 2 * AB_TILE);
-        tma_load_3d(sQ + st * AB_TILE, &tm_qkv, &qd_full[st], head * AB_D, i * AB_T, b);
-        tma_load_3d(sDO + st * AB_TILE, &tm_do, &qd_full[st], head * AB_D, i * AB_T, b);
+        mbar_expect_tx(&qd_full[st], 2 * AB_Q_TILE);
+        tma_load_3d(sQ + st * AB_Q_TILE, &tm_q, &qd_full[st], head * AB_D, i * AB_TQ, b);
+        tma_load_3d(sDO + st * AB_Q_TILE, &tm_do, &qd_full[st], head * AB_D, i * AB_TQ, b);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = make_idesc(1, 128, 128, 0, 0);   // K-major x K-major
-      constexpr uint32_t idesc_t = make_idesc(1, 128, 64, 1, 1);    // MN-major A (P / dS transposed) x MN-major B
-      constexpr uint32_t idesc_q = make_idesc(1, 128, 64, 0, 1);    // K-major A (dS) x MN-major B (K_j)
-      const uint32_t k_base = smem_u32(sK), v_base = smem_u32(sV), p_base = smem_u32(sP), ds_base = smem_u32(sDS);
-      auto issue_sdp = [&](int i) {
-        const int st = i & 1;
-        mbar_wait(&qd_full[st], (i >> 1) & 1, 0x61);
-        mbar_wait(s_empty, (i & 1) ^ 1, 0x62);
-        tc_fence_after();
-        const uint64_t dq_ = make_smem_desc(smem_u32(sQ + st * AB_TILE), 0, 1024, 2);
-        const uint64_t dk_ = make_smem_desc(k_base, 0, 1024, 2);
-        const uint64_t do_ = make_smem_desc(smem_u32(sDO + st * AB_TILE), 0, 1024, 2);
-        const uint64_t dv_ = make_smem_desc(v_base, 0, 1024, 2);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) umma_f16(tmem_base + AB_TM_S, dq_ + (uint64_t)(k * 2), dk_ + (uint64_t)(k * 2), idesc_s, k > 0);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) umma_f16(tmem_base + AB_TM_DP, do_ + (uint64_t)(k * 2), dv_ + (uint64_t)(k * 2), idesc_s, k > 0);
-        umma_commit(s_full);
-      };
-      mbar_wait(kv_full, 0, 0x63);
-      issue_sdp(0);
-      for (int i = 0; i < T; ++i) {
-        if (i + 1 < T) issue_sdp(i + 1);
-        const int st = i & 1;
-        mbar_wait(p_full, i & 1, 0x64);
-        mbar_wait(dq_empty, (i & 1) ^ 1, 0x65);
-        tc_fence_after();
-        const uint32_t q_base = smem_u32(sQ + st * AB_TILE), do_base = smem_u32(sDO + st * AB_TILE);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {  // K = 128 queries, 16 per MMA = 16 rows x 128 B = 2048 B
-          // A = P^T: P stored [query rows][key columns] in two 64-key atoms 16 KB apart -> MN-major A with LBO 16 KB
-          const uint64_t da = make_smem_desc(p_base + k * 2048, 2 * AB_TILE / 2, 1024, 2);
-          const uint64_t db = make_smem_desc(do_base + k * 2048, 0, 1024, 2);
-          umma_f16(tmem_base + AB_TM_DV, da, db, idesc_t, (i > 0) || (k > 0));
-        }
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const uint64_t da = make_smem_desc(ds_base + k * 2048, 2 * AB_TILE / 2, 1024, 2);
-          const uint64_t db = make_smem_desc(q_base + k * 2048, 0, 1024, 2);
-          umma_f16(tmem_base + AB_TM_DK, da, db, idesc_t, (i > 0) || (k > 0));
-        }
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {  // K = 128 keys: dS K-major (two key atoms), K_j rows are the K dimension
-          const uint64_t da = make_smem_desc(ds_base + (k >> 2) * AB_TILE + (k & 3) * 32, 0, 1024, 2);
-          const uint64_t db = make_smem_desc(k_base + k * 2048, 0, 1024, 2);
-          umma_f16(tmem_base + AB_TM_DQ, da, db, idesc_q, k > 0);
-        }
-        umma_commit(&qd_empty[st]);
-        umma_commit(mma2_done);
-      }
-    }
-  } else {
-    // ===================== row threads =====================
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;        // query row within the tile (S / dP / dQ) or key row (dK / dV) == TMEM lane
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(quad * 32) << 16);
-    const int kv_valid = min(AB_T, N - j * AB_T);                  // keys of this tile that exist
-    const size_t stat_base = ((size_t)b * H + head) * N;
-    auto dump_dq = [&](int i) {                                    // dQ of query tile i: TMEM -> fp32 atomics
-      uint32_t o[2][32];
-      tmem_ld_32x32(lane_addr + AB_TM_DQ, o[0]);
-      tmem_ld_32x32(lane_addr + AB_TM_DQ + 32, o[1]);
-      tmem_ld_wait();
-      tc_fence_before();
-      mbar_arrive(dq_empty);
-      const int q = i * AB_T + row;
-      if (q < N) {
-        float* dst = dq_acc + ((size_t)b * N + q) * C + head * AB_D;
-#pragma unroll
-        for (int d4 = 0; d4 < 16; ++d4) {
-          const int d = d4 * 4;
-          asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + d), "f"(__uint_as_float(o[d >> 5][d & 31])),
-                       "f"(__uint_as_float(o[d >> 5][(d & 31) + 1])), "f"(__uint_as_float(o[d >> 5][(d & 31) + 2])),
-                       "f"(__uint_as_float(o[d >> 5][(d & 31) + 3]))
-                       : "memory");
-        }
-      }
-    };
-    for (int i = 0; i < T; ++i) {
-      const int q = i * AB_T + row;
-      // rows past N: lse = +inf makes P (and with it dS) exactly zero
-      const float L = q < N ? __ldg(lse + stat_base + q) : INFINITY;
-      const float Dl = q < N ? __ldg(delta + stat_base + q) : 0.f;
-      mbar_wait(s_full, i & 1, 0x66);
-      if (i > 0) mbar_wait(mma2_done, (i - 1) & 1, 0x67);   // P / dS buffers free again, dQ_{i-1} complete
-      tc_fence_after();
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t sreg[32], dreg[32];
-        tmem_ld_32x32(lane_addr + AB_TM_S + c * 32, sreg);
-        tmem_ld_32x32(lane_addr + AB_TM_DP + c * 32, dreg);
-        tmem_ld_wait();
-        if (c == 3) {
-          tc_fence_before();
-          mbar_arrive(s_empty);    // S / dP of this tile live in registers / smem now
-        }
-        const int nval = kv_valid - c * 32;      // valid keys in this chunk (warp-uniform)
-        uint32_t pp[16], dd[16];
-#pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          float p0 = ab_ex2(fmaf(__uint_as_float(sreg[2 * e]), scale_log2e, -L));
-          float p1 = ab_ex2(fmaf(__uint_as_float(sreg[2 * e + 1]), scale_log2e, -L));
-          if (nval < 32) {
-            if (2 * e >= nval) p0 = 0.f;
-            if (2 * e + 1 >= nval) p1 = 0.f;
-          }
-          const float g0 = p0 * (__uint_as_float(dreg[2 * e]) - Dl) * scale;
-          const float g1 = p1 * (__uint_as_float(dreg[2 * e + 1]) - Dl) * scale;
-          pp[e] = pack_bf16x2(p0, p1);
-          dd[e] = pack_bf16x2(g0, g1);
-        }
-        // keys [c*32, c*32+32) -> key atom (c >> 1), 16-byte chunks ((c & 1) * 4 + w), w = 0..3, of row `row`
-        uint8_t* pa = sP + (c >> 1) * AB_TILE + row * 128;
-        uint8_t* da = sDS + (c >> 1) * AB_TILE + row * 128;
-#pragma unroll
-        for (int w = 0; w < 4; ++w) {
-          const int chunk = ((c & 1) * 4 + w) ^ (row & 7);
-          *reinterpret_cast<uint4*>(pa + chunk * 16) = make_uint4(pp[4 * w], pp[4 * w + 1], pp[4 * w + 2], pp[4 * w + 3]);
-          *reinterpret_cast<uint4*>(da + chunk * 16) = make_uint4(dd[4 * w], dd[4 * w + 1], dd[4 * w + 2], dd[4 * w + 3]);
-        }
-      }
-      fence_async_smem();   // generic-proxy writes of P / dS -> visible to tcgen05.mma
-      tc_fence_before();
-      mbar_arrive(p_full);
-      if (i > 0) dump_dq(i - 1);   // overlaps the S / dP MMAs of the next query tile
-    }
-    mbar_wait(mma2_done, (T - 1) & 1, 0x68);
-    tc_fence_after();
-    dump_dq(T - 1);
-    // dK_j, dV_j (TMEM lane = key row)
-    uint32_t o[2][32];
-    const int key = j * AB_T + row;
-#pragma unroll
-    for (int which = 0; which < 2; ++which) {   // 0: dK -> columns [C, 2C), 1: dV -> columns [2C, 3C)
-      const uint32_t col = which == 0 ? AB_TM_DK : AB_TM_DV;
-      tmem_ld_32x32(lane_addr + col, o[0]);
-      tmem_ld_32x32(lane_addr + col + 32, o[1]);
-      tmem_ld_wait();
-      if (key < N) {
-        __nv_bfloat16* dst = dqkv + ((size_t)b * N + key) * 3 * C + (which + 1) * C + head * AB_D;
-#pragma unroll
-        for (int d8 = 0; d8 < 8; ++d8) {
-          uint32_t w[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const int d = d8 * 8 + 2 * e;
-            w[e] = pack_bf16x2(__uint_as_float(o[d >> 5][d & 31]), __uint_as_float(o[(d + 1) >> 5][(d + 1) & 31]));
-          }
-          *reinterpret_cast<uint4*>(dst + d8 * 8) = make_uint4(w[0], w[1], w[2], w[3]);
-        }
-      }
-    }
-    tc_fence_before();
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, AB_TMEM_COLS);
+  // ===================== consumer warpgroups =====================
+  const int wg = warp >> 2;
+  const int g = lane >> 2, t4 = lane & 3;
+  const int krow = (warp & 3) * 16 + g;     // this thread's key rows krow, krow + 8 within the warpgroup's 64 keys
+  uint8_t* sDS = smem + AB_OFF_DS + wg * AB_Q_TILE;
+  const size_t stat_base = ((size_t)b * H + head) * N;
+  bool key_ok[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) key_ok[i] = j * AB_T + wg * 64 + krow + 8 * i < N;
+  const uint64_t dk_a = make_wgmma_desc(smem_u32(sK) + wg * 64 * 128, 0, 1024);     // K rows of this warpgroup, K-major
+  const uint64_t dv_a = make_wgmma_desc(smem_u32(sV) + wg * 64 * 128, 0, 1024);
+  const uint64_t dk_b = make_wgmma_desc(smem_u32(sK) + wg * 64 * 128, 8192, 1024);  // same rows as an MN-major B (dQ)
+  const uint64_t ds_a = make_wgmma_desc(smem_u32(sDS), 8192, 1024);                // dS^T as an MN-major A (dQ)
+  float dk[32], dv[32];
+#pragma unroll
+  for (int e = 0; e < 32; ++e) dk[e] = dv[e] = 0.f;
+  mbar_wait(kv_full, 0, 0x63);
+  for (int i = 0; i < T; ++i) {
+    const int st = i & 1;
+    mbar_wait(&qd_full[st], (i >> 1) & 1, 0x61);
+    const uint32_t q_addr = smem_u32(sQ + st * AB_Q_TILE), do_addr = smem_u32(sDO + st * AB_Q_TILE);
+    float sT[32], dpT[32];
+#pragma unroll
+    for (int e = 0; e < 32; ++e) sT[e] = dpT[e] = 0.f;
+    {
+      const uint64_t dq_b = make_wgmma_desc(q_addr, 0, 1024), ddo_b = make_wgmma_desc(do_addr, 0, 1024);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_64_bf16<0, 0>(sT, dk_a + (uint64_t)(2 * k), dq_b + (uint64_t)(2 * k));
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_64_bf16<0, 0>(dpT, dv_a + (uint64_t)(2 * k), ddo_b + (uint64_t)(2 * k));
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(sT);
+      reg_fence(dpT);
+    }
+    // columns of this thread: queries i * 64 + 8 jj + 2 t4 + c; queries past N: lse = +inf makes P (and dS) zero
+    uint32_t pa[4][4], da[4][4];
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      float L[2], Dl[2];
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        const int q = i * AB_TQ + 8 * jj + 2 * t4 + c;
+        L[c] = q < N ? __ldg(lse + stat_base + q) : INFINITY;
+        Dl[c] = q < N ? __ldg(delta + stat_base + q) : 0.f;
+      }
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        float p[2], d[2];
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          p[c] = key_ok[r] ? ab_ex2(fmaf(sT[4 * jj + 2 * r + c], scale_log2e, -L[c])) : 0.f;
+          d[c] = p[c] * (dpT[4 * jj + 2 * r + c] - Dl[c]) * scale;
+        }
+        pa[jj >> 1][(jj & 1) * 2 + r] = pack_bf16x2(p[0], p[1]);
+        da[jj >> 1][(jj & 1) * 2 + r] = pack_bf16x2(d[0], d[1]);
+      }
+    }
+    // dS^T -> smem: row = key (128 B = 64 queries, 16-byte chunks swizzled by the row), as the wgmma layouts expect
+    named_bar(1 + wg, 128);  // the previous dQ MMA of this warpgroup has finished reading the buffer
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int row = krow + 8 * r;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+        *reinterpret_cast<uint32_t*>(sDS + row * 128 + ((jj ^ (row & 7)) << 4) + 4 * t4) = da[jj >> 1][(jj & 1) * 2 + r];
+    }
+    fence_async_smem();      // generic-proxy writes of dS^T -> visible to wgmma
+    named_bar(1 + wg, 128);
+    float dq[32];
+#pragma unroll
+    for (int e = 0; e < 32; ++e) dq[e] = 0.f;
+    {
+      const uint64_t q_b = make_wgmma_desc(q_addr, 8192, 1024), do_b = make_wgmma_desc(do_addr, 8192, 1024);
+      reg_fence(dv);
+      reg_fence(dk);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) wgmma_64_bf16_rs<1>(dv, pa[kk], do_b + (uint64_t)(kk * 128));  // 16 query rows = 2048 B
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) wgmma_64_bf16_rs<1>(dk, da[kk], q_b + (uint64_t)(kk * 128));
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) wgmma_64_bf16<1, 1>(dq, ds_a + (uint64_t)(kk * 128), dk_b + (uint64_t)(kk * 128));  // 16 keys
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(dv);
+      reg_fence(dk);
+      reg_fence(dq);
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&qd_empty[st]);  // Q_i / dO_i are no longer read
+    // dQ_i partial (this warpgroup's keys): rows = queries 16 (warp & 3) + g + 8 r, columns = d
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int q = i * AB_TQ + krow + 8 * r;
+      if (q < N) {
+        float* dst = dq_acc + ((size_t)b * N + q) * C + head * AB_D + 2 * t4;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+          asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst + 8 * jj), "f"(dq[4 * jj + 2 * r]),
+                       "f"(dq[4 * jj + 2 * r + 1])
+                       : "memory");
+      }
+    }
+  }
+  // dK_j, dV_j (row = key)
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int key = j * AB_T + wg * 64 + krow + 8 * r;
+    if (key < N) {
+      __nv_bfloat16* dst = dqkv + ((size_t)b * N + key) * 3 * C + head * AB_D + 2 * t4;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        *reinterpret_cast<uint32_t*>(dst + C + 8 * jj) = pack_bf16x2(dk[4 * jj + 2 * r], dk[4 * jj + 2 * r + 1]);
+        *reinterpret_cast<uint32_t*>(dst + 2 * C + 8 * jj) = pack_bf16x2(dv[4 * jj + 2 * r], dv[4 * jj + 2 * r + 1]);
+      }
+    }
   }
 }
 
@@ -341,17 +277,20 @@ int launch_attention_bwd(const __nv_bfloat16* qkv, const __nv_bfloat16* out, con
     DVT_CUDA_OK(cudaGetLastError());
     count_launch();
   }
-  CUtensorMap tq, td;
-  int rc = make_tmap_3d(&tq, qkv, TMAP_BF16, (uint64_t)3 * C, (uint64_t)N, (uint64_t)B, (uint64_t)3 * C * 2,
+  CUtensorMap tkv, tq, td;
+  int rc = make_tmap_3d(&tkv, qkv, TMAP_BF16, (uint64_t)3 * C, (uint64_t)N, (uint64_t)B, (uint64_t)3 * C * 2,
                         (uint64_t)N * 3 * C * 2, AB_D, AB_T);
   if (rc) return rc;
+  rc = make_tmap_3d(&tq, qkv, TMAP_BF16, (uint64_t)3 * C, (uint64_t)N, (uint64_t)B, (uint64_t)3 * C * 2,
+                    (uint64_t)N * 3 * C * 2, AB_D, AB_TQ);
+  if (rc) return rc;
   rc = make_tmap_3d(&td, dout, TMAP_BF16, (uint64_t)C, (uint64_t)N, (uint64_t)B, (uint64_t)C * 2, (uint64_t)N * C * 2, AB_D,
-                    AB_T);
+                    AB_TQ);
   if (rc) return rc;
   const float scale = 0.125f;  // 64^-0.5
   dim3 grid((N + AB_T - 1) / AB_T, heads, B);
-  attention_bwd_tc_kernel<<<grid, AB_THREADS, AB_SMEM_TOTAL, stream>>>(tq, td, lse, delta, dqkv, dq_acc, N, C, heads, scale,
-                                                                        scale * 1.4426950408889634f);
+  attention_bwd_tc_kernel<<<grid, AB_THREADS, AB_SMEM_TOTAL, stream>>>(tkv, tq, td, lse, delta, dqkv, dq_acc, N, C, heads,
+                                                                        scale, scale * 1.4426950408889634f);
   DVT_CUDA_OK(cudaGetLastError());
   count_launch();
   attn_dq_cast_kernel<<<num_sms() * 4, 256, 0, stream>>>(dq_acc, dqkv, (size_t)B * N, C);

@@ -12,7 +12,7 @@
 //           encode of the NEXT step (hash-grid gather / interpolation with the pending Adam steps applied on the fly)
 //   sides : gather of the sampled bank rows, residual MLP forward (3 GEMM) / backward (5 GEMM), weight-gradient GEMMs,
 //           Adam(small params), and the dense Adam sweep of the hash table (software-pipelined two steps deep)
-// All GEMMs run on tcgen05 (gemm.cu) as 3xTF32 products of fp32 hi/lo planes (fp32-accurate: bf16 operands cannot
+// All GEMMs run on the tensor cores (gemm.cu) as 3xTF32 products of fp32 hi/lo planes (fp32-accurate: bf16 operands cannot
 // hold the cosine >= 0.999 parity bar, see DESIGN.md); weight-gradient GEMMs read the activations as MN-major
 // operands, so no transposed copies exist; bias gradients come from a ones column appended to the activation buffers.
 //
@@ -245,41 +245,98 @@ __global__ void fit_corners_kernel(GridLevels g, const float* __restrict__ coord
   }
 }
 
-// backward of the encoding: dense-table gradient accumulation with vector atomics
+// backward of the encoding: dense-table gradient accumulation, in a fixed order (the result does not depend on thread
+// scheduling: float atomics would add the contributions of colliding samples in whatever order they arrive, and 2000 Adam
+// steps turn that last-bit noise into visibly different fits).  CTA (level, part) owns the level's entries with
+// entry % GB_PARTS == part; samples in chunks of GB_ROWS: the chunk's (entry, contribution) keys of this part are collected
+// in shared memory and sorted (bitonic; the keys are unique, so the order is canonical), then the first thread of every run
+// of equal entries sums the run in contribution order and adds it to the entry.
 // `stamp` (optional): stamp[entry] = step + 1 marks the entries that received a gradient this step, so that the dense
 // Adam sweep reads (and re-zeroes) the gradient of touched entries only: 24 B/param of traffic instead of 32.
 // The gradient / stamp buffers form a ring of three (TableBufs): the backward of step t writes ring slot t % 3 while the
 // sweeps of steps t-1 / t-2 may still be reading theirs.  tb.stamp[0] == nullptr: plain accumulation into tb.g[0]
 // (unit-test entry point).
-__global__ void fit_grid_bwd_kernel(GridLevels g, const float* __restrict__ coords, StepRows sr, int n,
-                                    const float* __restrict__ denc, int ld_denc, TableBufs tb) {
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= n * g.n_levels) return;
+constexpr int GB_ROWS = 2048;
+constexpr int GB_N = 4 * GB_ROWS;                  // contributions per chunk (a power of two)
+constexpr int GB_THREADS = 512;
+constexpr int GB_PARTS = 8;                        // CTAs per level
+constexpr int GB_SMEM = GB_N * (8 + 4);            // sort keys + corner weights
+__global__ void __launch_bounds__(GB_THREADS, 1)
+fit_grid_bwd_kernel(GridLevels g, const float* __restrict__ coords, StepRows sr, int n, const float* __restrict__ denc,
+                    int ld_denc, TableBufs tb) {
+  extern __shared__ unsigned long long gb_key[];   // [GB_N]: (entry within the level) << 32 | contribution
+  float* gb_w = reinterpret_cast<float*>(gb_key + GB_N);  // [GB_N]: corner weight of each contribution
+  __shared__ int gb_cnt;
+  const int l = blockIdx.x;
+  const uint32_t part = blockIdx.y;
   pdl_wait();     // (no-ops unless launched with programmatic stream serialisation)
   pdl_trigger();
-  const int i = t % n, l = t / n;
   const int* rows = sr.rows(n);
-  const int r = rows ? rows[i] : i;
-  const float2 xy = *reinterpret_cast<const float2*>(sr.coords(coords) + 2 * (size_t)r);
-  const CornerSet c = grid_corners(g, l, xy.x, xy.y);
-  const float4 a = *reinterpret_cast<const float4*>(denc + (size_t)i * ld_denc + l * FIT_F);
-  const float4 b = *reinterpret_cast<const float4*>(denc + (size_t)i * ld_denc + l * FIT_F + 4);
+  const float* xy_all = sr.coords(coords);
   const bool stamped = tb.stamp[0] != nullptr;
   const int slot = stamped ? mod3(sr.step()) : 0;
   float* gtable = DVT_SEL3(tb.g, slot);
   uint32_t* stamp = DVT_SEL3(tb.stamp, slot);
   const uint32_t mark = stamped ? (uint32_t)sr.step() + 1u : 0u;
+  const uint32_t base = g.offset[l];
+  constexpr unsigned long long PAD = ~0ull;
+  for (int r0 = 0; r0 < n; r0 += GB_ROWS) {
+    const int cnt = min(GB_ROWS, n - r0);
+    if (threadIdx.x == 0) gb_cnt = 0;
+    __syncthreads();
+    for (int i = threadIdx.x; i < cnt; i += GB_THREADS) {
+      const int r = rows ? rows[r0 + i] : r0 + i;
+      const float2 xy = *reinterpret_cast<const float2*>(xy_all + 2 * (size_t)r);
+      const CornerSet c = grid_corners(g, l, xy.x, xy.y);
 #pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    if (stamped) stamp[c.idx[k]] = mark;
-    float* dst = gtable + (size_t)c.idx[k] * FIT_F;
-    const float w = c.w[k];
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(w * a.x), "f"(w * a.y), "f"(w * a.z),
-                 "f"(w * a.w)
-                 : "memory");
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + 4), "f"(w * b.x), "f"(w * b.y),
-                 "f"(w * b.z), "f"(w * b.w)
-                 : "memory");
+      for (int k = 0; k < 4; ++k) {
+        const uint32_t e = c.idx[k] - base;
+        if (e % GB_PARTS != part) continue;
+        gb_key[atomicAdd(&gb_cnt, 1)] = ((unsigned long long)e << 32) | (unsigned)(4 * i + k);
+        gb_w[4 * i + k] = c.w[k];
+      }
+    }
+    __syncthreads();
+    const int m = gb_cnt;
+    int np = 2;
+    while (np < m) np <<= 1;
+    for (int p = m + threadIdx.x; p < np; p += GB_THREADS) gb_key[p] = PAD;
+    __syncthreads();
+    for (int k = 2; k <= np; k <<= 1) {
+      for (int j = k >> 1; j > 0; j >>= 1) {
+        for (int t = threadIdx.x; t < np / 2; t += GB_THREADS) {
+          const int lo = 2 * t - (t & (j - 1)), hi = lo + j;  // pair t: index with a 0 inserted at bit log2(j), and its partner
+          const unsigned long long x = gb_key[lo], y = gb_key[hi];
+          if ((x > y) == ((lo & k) == 0)) {
+            gb_key[lo] = y;
+            gb_key[hi] = x;
+          }
+        }
+        __syncthreads();
+      }
+    }
+    for (int p = threadIdx.x; p < m; p += GB_THREADS) {
+      const uint32_t e = (uint32_t)(gb_key[p] >> 32);
+      if (p > 0 && (uint32_t)(gb_key[p - 1] >> 32) == e) continue;  // not the first of its run
+      float4 sa = make_float4(0.f, 0.f, 0.f, 0.f), sb = sa;
+      for (int q = p; q < m && (uint32_t)(gb_key[q] >> 32) == e; ++q) {
+        const uint32_t ci = (uint32_t)gb_key[q];
+        const float w = gb_w[ci];
+        const float* src = denc + (size_t)(r0 + (ci >> 2)) * ld_denc + l * FIT_F;
+        const float4 a = *reinterpret_cast<const float4*>(src), b = *reinterpret_cast<const float4*>(src + 4);
+        sa.x += w * a.x; sa.y += w * a.y; sa.z += w * a.z; sa.w += w * a.w;
+        sb.x += w * b.x; sb.y += w * b.y; sb.z += w * b.z; sb.w += w * b.w;
+      }
+      const uint32_t entry = base + e;
+      if (stamped) stamp[entry] = mark;
+      float4* dst = reinterpret_cast<float4*>(gtable + (size_t)entry * FIT_F);
+      float4 x = dst[0], y = dst[1];
+      x.x += sa.x; x.y += sa.y; x.z += sa.z; x.w += sa.w;
+      y.x += sb.x; y.y += sb.y; y.z += sb.z; y.w += sb.w;
+      dst[0] = x;
+      dst[1] = y;
+    }
+    __syncthreads();  // the next chunk reuses the keys and the counter
   }
 }
 
@@ -473,7 +530,8 @@ __global__ void __launch_bounds__(256, 2) fit_loss_kernel(LossArgs a) {
 // dG of phase 1, off the critical path: the loss kernel stores d pred (hi / lo planes); this kernel, on a side stream,
 // adds every row's d pred to the cells of G that F.grid_sample reads for the row's node (normally one cell with weight 1,
 // for 9 of 37 nodes per axis also a neighbour with a weight of ~1e-6: see LossArgs).  Only Adam(small) at the end of the
-// step consumes gG, so nothing on the main stream waits for these atomics.
+// step consumes gG, so nothing on the main stream waits for it.  One warp per cell GATHERS the rows that touch it, in
+// ascending row order: the sum does not depend on thread scheduling (with atomics it would, and Adam amplifies that).
 struct ScatterArgs {
   const float* dpred;       // [2 planes][n, C]
   size_t plane;
@@ -484,41 +542,61 @@ struct ScatterArgs {
   const float* ax_w0;
   const float* ax_w1;
 };
+constexpr int GS_MAXV = 1536 / 4 / 32;  // float4 columns per lane (C <= 1536)
 __global__ void __launch_bounds__(256) fit_g_scatter_kernel(ScatterArgs a) {
   pdl_wait();
   pdl_trigger();
-  const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int cell = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
-  if (row >= a.n) return;
-  const int cell = a.sr.rows(a.n)[row] % a.hw;
-  int cidx[4] = {cell, cell, cell, cell};
-  float cw[4] = {1.f, 0.f, 0.f, 0.f};
-  if (a.ax_i0) {
-    const int cy = cell / a.gw, cx = cell - cy * a.gw;
-    const int x0 = a.ax_i0[cx], y0 = a.ax_i0[a.gw + cy];
-    const float wx0 = a.ax_w0[cx], wx1 = a.ax_w1[cx], wy0 = a.ax_w0[a.gw + cy], wy1 = a.ax_w1[a.gw + cy];
+  if (cell >= a.hw) return;
+  const int* rows = a.sr.rows(a.n);
+  const int ty = cell / a.gw, tx = cell - ty * a.gw;
+  const int nv = a.C >> 2;
+  float4 acc[GS_MAXV];
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const int xx = x0 + (k & 1), yy = y0 + (k >> 1);
-      const bool inside = xx >= 0 && xx < a.gw && yy >= 0 && yy < a.gh;
-      cidx[k] = inside ? yy * a.gw + xx : cell;
-      cw[k] = inside ? ((k & 1) ? wx1 : wx0) * ((k >> 1) ? wy1 : wy0) : 0.f;
+  for (int j = 0; j < GS_MAXV; ++j) acc[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int r0 = 0; r0 < a.n; r0 += 32) {
+    // weight with which row r0 + lane reaches this cell (0: it does not)
+    float w = 0.f;
+    const int row = r0 + lane;
+    if (row < a.n) {
+      const int rc = rows[row] % a.hw;
+      if (!a.ax_i0) {
+        w = rc == cell ? 1.f : 0.f;
+      } else {
+        const int cy = rc / a.gw, cx = rc - cy * a.gw;
+        const int x0 = a.ax_i0[cx], y0 = a.ax_i0[a.gw + cy];
+        const int dx = tx - x0, dy = ty - y0;
+        if (dx >= 0 && dx <= 1 && dy >= 0 && dy <= 1)
+          w = (dx ? a.ax_w1[cx] : a.ax_w0[cx]) * (dy ? a.ax_w1[a.gw + cy] : a.ax_w0[a.gw + cy]);
+      }
+    }
+    unsigned hit = __ballot_sync(0xffffffffu, w != 0.f);
+    while (hit) {
+      const int src = __ffs(hit) - 1;
+      hit &= hit - 1;
+      const float wk = __shfl_sync(0xffffffffu, w, src);
+      const float4* hi = reinterpret_cast<const float4*>(a.dpred + (size_t)(r0 + src) * a.C);
+      const float4* lo = reinterpret_cast<const float4*>(a.dpred + a.plane + (size_t)(r0 + src) * a.C);
+#pragma unroll
+      for (int j = 0; j < GS_MAXV; ++j) {
+        const int v = lane + 32 * j;
+        if (v < nv) {
+          const float4 h = hi[v], l = lo[v];
+          const float4 d = make_float4(h.x + l.x, h.y + l.y, h.z + l.z, h.w + l.w);  // hi + lo == d pred exactly
+          acc[j].x += d.x * wk; acc[j].y += d.y * wk; acc[j].z += d.z * wk; acc[j].w += d.w * wk;
+        }
+      }
     }
   }
-  const float4* hi = reinterpret_cast<const float4*>(a.dpred + (size_t)row * a.C);
-  const float4* lo = reinterpret_cast<const float4*>(a.dpred + a.plane + (size_t)row * a.C);
-  for (int v = lane; v < (a.C >> 2); v += 32) {
-    const float4 h = hi[v], l = lo[v];
-    const float4 d = make_float4(h.x + l.x, h.y + l.y, h.z + l.z, h.w + l.w);  // hi + lo == d pred exactly
+  float4* dst = reinterpret_cast<float4*>(a.gG + (size_t)cell * a.C);
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      if (cw[k] != 0.f) {
-        float* dst = a.gG + (size_t)cidx[k] * a.C + v * 4;
-        const float wk = cw[k];
-        asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(d.x * wk), "f"(d.y * wk), "f"(d.z * wk),
-                     "f"(d.w * wk)
-                     : "memory");
-      }
+  for (int j = 0; j < GS_MAXV; ++j) {
+    const int v = lane + 32 * j;
+    if (v < nv) {
+      float4 x = dst[v];
+      x.x += acc[j].x; x.y += acc[j].y; x.z += acc[j].z; x.w += acc[j].w;
+      dst[v] = x;
     }
   }
 }
@@ -558,7 +636,6 @@ static int launch_loss(const LossArgs& la, cudaStream_t st, bool pdl) {
 // few persistent 1024-thread CTAs that fill one SM each and leave the other SMs to the GEMM chain of the next steps.
 // (Measured and rejected: one contiguous slice per CTA -- 133 us, HBM channel imbalance; maximum shared-memory
 // carve-out -- 137 us.)
-// (Measured and rejected, r2r: ld.global.cs / st.global.cs streaming hints for p, m, v -- the step got 1-4 us slower.)
 constexpr int ADAM_UNROLL = 2;
 __global__ void __launch_bounds__(1024, 1)
 fit_adam_table_kernel(TableBufs tb, size_t nvec, const AdamScalars* __restrict__ sc, const int* __restrict__ step_base,
@@ -630,10 +707,8 @@ fit_adam_table_kernel(TableBufs tb, size_t nvec, const AdamScalars* __restrict__
 // (TMA, cp.async.bulk).  ONE thread per CTA keeps three 52 KB chunks (p, m, v and the two stamp arrays of 512 table
 // entries) in flight per SM through an mbarrier ring of four stages while 512 threads run the Adam arithmetic out of
 // shared memory and write the results back with coalesced 16-byte stores.  Idea: memory-level parallelism independent of
-// the thread count, so that a few dozen SMs could saturate HBM.  Measured (profiles/r2b_sweep_tma_experiment.txt): beside
-// the GEMM chain it moves ~55 GB/s per SM against ~79 GB/s of the plain-load kernel -- either way ~100-150 KB in flight
-// per SM and ~1.5-2.5 us of loaded latency, i.e. Little's law caps a 40-SM sweep near half of the HBM rate; only the whole
-// GPU (148 SMs x ~90 KB) holds the ~13 MB in flight that 6.5 TB/s needs.  Same adam1() arithmetic, same stamp rules:
+// the thread count, so that a few dozen SMs could saturate HBM (Little's law: the bytes in flight per SM times the SMs
+// the sweep runs on, over the loaded latency, bound its rate).  Same adam1() arithmetic, same stamp rules:
 // bit-identical results (tests/test_fit_gpu.py::test_sweep_kernels_agree).
 // Chunks are dealt round-robin (chunk c -> CTA c % grid), i.e. all CTAs advance one contiguous front together.
 // ----------------------------------------------------------------------------------------------------
@@ -802,6 +877,8 @@ struct Seg {
   int off = 0, rows = 0, cols = 0;  // floats; weights are [rows, cols] row-major, biases rows x 1
 };
 
+constexpr int FIT_SEM_TILES = 1024;
+
 struct Fit {
   // config
   int C, gh, gw, hw, bsz, Lf;
@@ -858,6 +935,7 @@ struct Fit {
   double sched_key[6] = {-1, -1, -1, -1, -1, -1};  // (num_iters, warmup, lr, min_lr, freeze_step) of the uploaded tables
   AdamScalars *sc_main = nullptr, *sc_res = nullptr;
   float* losses = nullptr;    // [num_iters, 5]
+  unsigned* wg_sem = nullptr; // [5][FIT_SEM_TILES] split-K counters of the five weight-gradient call sites (self-resetting)
   int* step_base = nullptr;
   float wd = 1e-5f, loss_scale = 1024.f;
   // bank (borrowed)
@@ -882,18 +960,16 @@ struct Fit {
   std::vector<void*> owned;
 };
 
-// EXPERIMENT (DVT_FIT_CARVEOUT=<percent> for the small kernels, DVT_FIT_CARVEOUT_SWEEP=<percent> for the sweep; off by default).  Every 3xTF32 GEMM CTA of the chain needs 181-212 KB of shared memory, and
-// an SM changes its L1 / shared-memory split only when it is idle: a GEMM CTA cannot join an SM on which one of the fit's
-// small kernels (no shared memory, so by default the largest L1) got first -- it waits until those CTAs have drained.  Seen
-// in the CUPTI timeline (r2u): with one 512-thread sweep CTA on EVERY SM (DVT_FIT_SWEEP_THREADS=512, DVT_FIT_SWEEP_CTAS=148)
-// no GEMM CTA started before the sweep had finished.  Asking for the maximum shared-memory carve-out on the fit's own
-// kernels does make the GEMM CTAs resident beside them, but the loads in flight of the sweep / encode / loss kernels live
-// in L1: with 28 KB of it the 48-CTA sweep takes 286 us instead of 145 and the step 218 us instead of 156; the co-resident
-// geometry reaches 185 us (r2v).  Rejected: the sweep keeps its own SMs and the driver's default split.
+// EXPERIMENT (DVT_FIT_CARVEOUT=<percent> for the small kernels, DVT_FIT_CARVEOUT_SWEEP=<percent> for the sweep; off by
+// default).  The 3xTF32 GEMM CTAs of the chain need up to ~200 KB of shared memory, and an SM changes its L1 / shared-memory
+// split only when it is idle: a GEMM CTA cannot join an SM on which one of the fit's small kernels (no shared memory, so by
+// default the largest L1) got first.  Asking for a shared-memory carve-out on the fit's own kernels makes the GEMM CTAs
+// resident beside them, at the cost of the L1 the sweep / encode / loss kernels keep their loads in flight in.
 static int fit_prepare_kernels() {
   static bool done = false;
   if (done) return DVT_OK;
   done = true;
+  DVT_CUDA_OK(cudaFuncSetAttribute(fit_grid_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GB_SMEM));
   const char* e = getenv("DVT_FIT_CARVEOUT");            // percent of the unified L1 / shared array, small kernels
   const char* es = getenv("DVT_FIT_CARVEOUT_SWEEP");     // ... the sweep
   const int pct = e ? atoi(e) : 0, pct_sweep = es ? atoi(es) : 0;
@@ -954,7 +1030,7 @@ int fit_create(Fit** out, int C, int gh, int gw, int bsz, int n_levels, const fl
   DVT_CUDA_OK(cudaEventCreateWithFlags(&f->ev_in, cudaEventDisableTiming));
   DVT_CUDA_OK(cudaEventCreateWithFlags(&f->ev_out, cudaEventDisableTiming));
   {
-    // Schedule knobs (defaults = the fastest measured at the headline size, profiles/r1w_fit_schedules.txt, r2_fit_step_ab.txt):
+    // Schedule knobs (defaults chosen at the headline size; not yet re-tuned for the 132 SMs of an H100):
     //   DVT_FIT_SWEEP_CTAS="a[,b]"  per phase (1 [, 2]): n > 0 pipelined sweep on n persistent CTAs (1024 threads, one
     //                               per SM); 0 pipelined sweep on 8 x #SM CTAs of 256 threads; -1 sequential schedule
     //   DVT_FIT_PIPELINE=0          sequential schedule in both phases
@@ -966,20 +1042,19 @@ int fit_create(Fit** out, int C, int gh, int gw, int bsz, int n_levels, const fl
     }
     //   DVT_FIT_PDL=0               plain stream-ordered launches (no programmatic dependent launch)
     //   DVT_FIT_RES_TF32=1          residual-MLP GEMMs in plain TF32 instead of 3xTF32 (experiment; not the default)
-    //   DVT_FIT_SWEEP_TMA=1         persistent sweep CTAs use the TMA-staged kernel instead of plain loads (measured slower
-    //                               beside the chain: profiles/r2b_sweep_tma_experiment.txt; kept as a tested experiment)
+    //   DVT_FIT_SWEEP_TMA=1         persistent sweep CTAs use the TMA-staged kernel instead of plain loads (bit-identical;
+    //                               kept as a tested experiment)
     const char* tm = getenv("DVT_FIT_SWEEP_TMA");
     f->sweep_tma = tm && tm[0] == '1';
     //   DVT_FIT_WGRAD_TF32=1        weight-gradient GEMMs of the field MLP in plain TF32 (experiment; not the default)
     const char* wt = getenv("DVT_FIT_WGRAD_TF32");
     f->wgrad_x3 = (wt && wt[0] == '1') ? 2 : 1;
-    //   DVT_FIT_SWEEP_PDL=0         sweep t+1 is launched only when sweep t has completed (no waiting resident CTAs); neutral
+    //   DVT_FIT_SWEEP_PDL=0         sweep t+1 is launched only when sweep t has completed (no waiting resident CTAs)
     //   DVT_FIT_X3_WIDE_MIN_N="a[,b]" per phase: 3xTF32 GEMMs with N >= this use 128 x 128 tiles (0: always 128 x 64)
     //   DVT_FIT_WGRAD_SMS=n         split-K of the weight-gradient GEMMs fills at most n SMs (they share the GPU with the
-    //                               data-gradient GEMMs of the critical path; 96: -9 us/step in phase 1, r2p)
+    //                               data-gradient GEMMs of the critical path)
     //   DVT_FIT_OFFPATH_PRIO=n      launch priority of the kernels that only feed Adam(small), n levels below the chain.
-    //                               The graphs keep the attribute (checked with DVT_FIT_DEBUG_GRAPH=1) but the step time
-    //                               does not move (r2o): an SM is handed to whichever queued CTA fits first.  Default 0.
+    //                               The graphs keep the attribute (DVT_FIT_DEBUG_GRAPH=1 shows it).  Default 0.
     if (const char* sp_ = getenv("DVT_FIT_SWEEP_PDL")) f->sweep_pdl = sp_[0] != '0';
     if (const char* wm = getenv("DVT_FIT_X3_WIDE_MIN_N")) {
       int a = 0, b = 0;
@@ -1035,6 +1110,7 @@ int fit_create(Fit** out, int C, int gh, int gw, int bsz, int n_levels, const fl
   A((void**)&f->Rout, n * C * 4); A((void**)&f->step_base, sizeof(int));
   A((void**)&f->inputs_dev, sizeof(FitInputs));
   A((void**)&f->flags_dev, sizeof(int));
+  A((void**)&f->wg_sem, 5 * FIT_SEM_TILES * sizeof(unsigned));
   if (!rc && cudaHostAlloc((void**)&f->flags_pinned, sizeof(int), cudaHostAllocDefault) != cudaSuccess) rc = DVT_ERR_CUDA;
   if (rc) { for (void* p : f->owned) cudaFree(p); delete f; return rc; }
   // ones columns (bias gradients through the weight-gradient GEMMs)
@@ -1437,14 +1513,17 @@ static int fit_dgrad(Op dY, int M, int Nout, Op W, int Kin, const float* Hmask, 
 }
 
 // dW[Nout, Kin] (+ db[Nout]) += dY^T . [X | 1]:  dY stored [n, Nout] (MN-major A), X stored [n, Kin + ones] (MN-major B)
-static int fit_wgrad(Op dY, int n, int Nout, Op X, int Kin, float* gW, float* gb, cudaStream_t st, int impl,
+// sem: FIT_SEM_TILES zeroed per-tile counters of this call site: the splits of a tile add their partial sums in split
+// order, so the gradient does not depend on which split finishes first.
+static int fit_wgrad(Op dY, int n, int Nout, Op X, int Kin, float* gW, float* gb, unsigned* sem, cudaStream_t st, int impl,
                      bool pdl = false, int x3 = 1, int prio_drop = 0, int wide = 0, int sm_cap = 1 << 20) {
   GemmEpi e;
-  e.out = gW; e.ldo = Kin; e.out_mode = OUT_F32_ATOMIC; e.last_col_out = gb;
+  e.out = gW; e.ldo = Kin; e.out_mode = OUT_F32_ATOMIC; e.last_col_out = gb; e.splitk_sem = sem;
   // split-K so that (output tiles x splits) fills the SMs once: tiles are 128 x 64 or 128 x 128, k-blocks 32 samples
   const int kb = (n + 31) / 32;
   const int bn = gemm_x3_tile_n(Kin + 1, wide);
   const int tiles = ((Nout + 127) / 128) * ((Kin + bn) / bn);
+  DVT_REQUIRE(tiles <= FIT_SEM_TILES, "fit: %d weight-gradient tiles exceed the split-K counters", tiles);
   int splits = std::max(1, std::min(std::min(num_sms(), sm_cap) / std::max(tiles, 1), kb / 4));
   GemmShape s{Nout, Kin + 1, n, splits};
   s.a_mn = 1; s.b_mn = 1; s.x3 = x3; s.plane_a = dY.plane; s.plane_b = X.plane; s.pdl = pdl; s.prio_drop = prio_drop;
@@ -1571,19 +1650,19 @@ static int fit_enqueue_step(Fit* f, int step_off, bool phase2, cudaStream_t st, 
     FIT_RC(fork(sC, f->ev[3]));
     FIT_RC(fork(sE, f->ev[11]));
   }
-  FIT_RC(fit_wgrad(dpred, n, C, h1, H1, sg + f->W2.off, sg + f->b2.off, sB, impl, pdl, f->wgrad_x3, off, wide, wcap));   // side B
+  FIT_RC(fit_wgrad(dpred, n, C, h1, H1, sg + f->W2.off, sg + f->b2.off, f->wg_sem + 0 * FIT_SEM_TILES, sB, impl, pdl, f->wgrad_x3, off, wide, wcap));   // side B
   FIT_RC(fit_dgrad(dpred, n, C, W(f->W2), H1, f->h1, f->ld_h1, f->dh1, H1, p_nh, true, st, impl, pdl, 1, 0, wide));  // main
   FIT_RC(fork(sB, f->ev[4]));  // dh1 ready
-  FIT_RC(fit_wgrad(dh1, n, H1, enc, Lf, sg + f->W1.off, sg + f->b1.off, sB, impl, pdl, f->wgrad_x3, off, wide, wcap));  // side B (reads enc)
+  FIT_RC(fit_wgrad(dh1, n, H1, enc, Lf, sg + f->W1.off, sg + f->b1.off, f->wg_sem + 1 * FIT_SEM_TILES, sB, impl, pdl, f->wgrad_x3, off, wide, wcap));  // side B (reads enc)
   FIT_RC(fit_dgrad(dh1, n, H1, W(f->W1), Lf, nullptr, 0, f->denc, Lf, 0, false, st, impl, pdl, 1, 0, wide));
   if (!phase2) {
     // dG (+ grid_sample's neighbour shares) on side C, enqueued BEHIND the two data-gradient GEMMs: launched beside them, its
-    // 256 small CTAs take the registers the GEMM CTAs need and delay the critical path by ~10 us (measured, r2i)
+    // 256 small CTAs take the registers the GEMM CTAs need and delay the critical path.
     FIT_RC(fork(sC, f->ev[3]));
     ScatterArgs sa;
     sa.dpred = f->dpred; sa.plane = p_nc; sa.sr = sr; sa.gG = sg + f->G.off; sa.n = n; sa.C = C; sa.hw = f->hw;
     sa.gw = f->gw; sa.gh = f->gh; sa.ax_i0 = f->ax_i0; sa.ax_w0 = f->ax_w0; sa.ax_w1 = f->ax_w1;
-    DVT_CUDA_OK(launch_kx(LaunchOpt{pdl, off}, fit_g_scatter_kernel, dim3((n * 32 + tb - 1) / tb), dim3(tb), 0, sC, sa));
+    DVT_CUDA_OK(launch_kx(LaunchOpt{pdl, off}, fit_g_scatter_kernel, dim3((f->hw * 32 + tb - 1) / tb), dim3(tb), 0, sC, sa));
     DVT_CUDA_OK(cudaGetLastError());
     count_launch();
   }
@@ -1591,8 +1670,8 @@ static int fit_enqueue_step(Fit* f, int step_off, bool phase2, cudaStream_t st, 
   // next encode reads
   if (pipe && f->epoch_steps >= 2)
     DVT_CUDA_OK(cudaStreamWaitEvent(st, f->ev_sweep[(f->epoch_steps - 2) % 3], 0));
-  DVT_CUDA_OK(launch_k(pdl, fit_grid_bwd_kernel, dim3(enc_blocks), dim3(tb), 0, st, f->grid, f->coords, sr, n, f->denc, Lf,
-                       f->tb));
+  DVT_CUDA_OK(launch_k(pdl, fit_grid_bwd_kernel, dim3(f->grid.n_levels, GB_PARTS), dim3(GB_THREADS), (size_t)GB_SMEM, st, f->grid,
+                       f->coords, sr, n, f->denc, Lf, f->tb));
   DVT_CUDA_OK(cudaGetLastError());
   count_launch();
   if (phase2) {
@@ -1601,10 +1680,10 @@ static int fit_enqueue_step(Fit* f, int step_off, bool phase2, cudaStream_t st, 
     FIT_RC(fit_dgrad(dR, n, C, W(f->R3), Hr, f->r2, f->ld_r, f->dr2, Hr, p_nr, true, sC, impl, pdl, f->res_x3, off, wide));
     DVT_CUDA_OK(cudaEventRecord(f->ev[12], sC));                                              // dr2 ready
     FIT_RC(fit_dgrad(dr2, n, Hr, W(f->R2), Hr, f->r1, f->ld_r, f->dr1, Hr, p_nr, true, sC, impl, pdl, f->res_x3, off, wide));
-    FIT_RC(fit_wgrad(dr1, n, Hr, rawb, C, sg + f->R1.off, sg + f->rb1.off, sC, impl, pdl, f->res_x3, off, wide, wcap));
-    FIT_RC(fit_wgrad(dR, n, C, r2, Hr, sg + f->R3.off, sg + f->rb3.off, sE, impl, pdl, f->res_x3, off, wide, wcap));
+    FIT_RC(fit_wgrad(dr1, n, Hr, rawb, C, sg + f->R1.off, sg + f->rb1.off, f->wg_sem + 2 * FIT_SEM_TILES, sC, impl, pdl, f->res_x3, off, wide, wcap));
+    FIT_RC(fit_wgrad(dR, n, C, r2, Hr, sg + f->R3.off, sg + f->rb3.off, f->wg_sem + 3 * FIT_SEM_TILES, sE, impl, pdl, f->res_x3, off, wide, wcap));
     DVT_CUDA_OK(cudaStreamWaitEvent(sE, f->ev[12], 0));
-    FIT_RC(fit_wgrad(dr2, n, Hr, r1, Hr, sg + f->R2.off, sg + f->rb2.off, sE, impl, pdl, f->res_x3, off, wide, wcap));
+    FIT_RC(fit_wgrad(dr2, n, Hr, r1, Hr, sg + f->R2.off, sg + f->rb2.off, f->wg_sem + 4 * FIT_SEM_TILES, sE, impl, pdl, f->res_x3, off, wide, wcap));
     FIT_RC(join(sE, f->ev[13]));
   }
   FIT_RC(join(sC, f->ev[5]));
@@ -1870,7 +1949,8 @@ int hashgrid_bwd(int n_levels, const float* scale, const uint32_t* res, const ui
   const StepRows sr{nullptr, nullptr, 0};
   TableBufs tb = {};
   tb.g[0] = gtable;  // no stamps: plain accumulation
-  fit_grid_bwd_kernel<<<(n * n_levels + 255) / 256, 256, 0, st>>>(g, coords, sr, n, dout, n_levels * FIT_F, tb);
+  FIT_RC(fit_prepare_kernels());
+  fit_grid_bwd_kernel<<<dim3(n_levels, GB_PARTS), GB_THREADS, GB_SMEM, st>>>(g, coords, sr, n, dout, n_levels * FIT_F, tb);
   DVT_CUDA_OK(cudaGetLastError());
   return DVT_OK;
 }

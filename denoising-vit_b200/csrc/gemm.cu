@@ -1,10 +1,15 @@
-// TN GEMM on 5th-gen tensor cores: C[M,N] = A[M,K] * B[N,K]^T with fused epilogues.
+// TN GEMM on Hopper tensor cores: C[M,N] = A[M,K] * B[N,K]^T with fused epilogues.
 //
-// One persistent CTA per SM, 10 warps:
-//   warp 0      TMA producer   (A: 128 x 128B box, B: BN x 128B box, SWIZZLE_128B, 3-5 stage mbarrier ring)
-//   warp 1      MMA issuer     (lane 0 issues tcgen05.mma M=128 N=BN K=16/8; accumulators in TMEM, 2 stages)
-//   warps 2..9  epilogue       (tcgen05.ld 32x32b -> registers -> per-warp smem transpose -> coalesced stores;
-//               two warps per TMEM lane quadrant take alternating 32-column chunks; 4 warps in the x3 kernels)
+// bf16 and TF32 products (gemm_wgmma_kernel): one 128 x 128 output tile per CTA, 9 warps:
+//   warps 0-7   two consumer warpgroups, 64 rows each: wgmma m64n128 (k16 bf16 / k8 tf32) straight from the swizzled TMA
+//               tiles (bf16 operands K-major or MN-major, TF32 K-major), fp32 accumulators in registers
+//   warp 8      TMA producer (A: 128 x 128B, B: 128 x 128B per stage, SWIZZLE_128B, 3-stage mbarrier ring)
+//   The accumulators are then staged through shared memory (the drained operand ring) and the eight consumer warps run
+//   the fused epilogue on 32 x 32 chunks in a coalesced layout.  Three stages (96 KB) keep two CTAs resident per SM, so
+//   one CTA's epilogue overlaps the other's main loop.
+// 3xTF32 products of the stage-1 fit (gemm_x3_kernel, fp32 hi/lo operand planes): 128 x 64 or 128 x 128 tiles, 8 warps
+//   of mma.sync m16n8k8 TF32 with fragments read from the swizzled TMA tiles -- the fit's backward products read
+//   MN-major fp32 operands, which wgmma's TF32 form does not accept (K-major only).
 // K tails, M tails and N tails are handled by TMA zero-fill plus masking in the epilogue.
 //
 // Used for: patch-embed, QKV, attention out-proj, MLP fc1/fc2 (reference: timm VisionTransformer reached from
@@ -21,36 +26,43 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int KB_BYTES = 128;  // bytes of K per pipeline stage row (= one 128B swizzle atom)
-// 8 epilogue warps per CTA (two per TMEM lane quadrant, alternating 32-column chunks: twice the ALU throughput and
-// memory-level parallelism of one warp per scheduler).  The x3 (fit) kernels use 128x64 tiles: their problems are small
-// (M = 2048), so narrower tiles mean more CTAs, half the MMA time per k-block and a one-chunk-per-warp epilogue.
-// The 128x256 bf16 tiles (HP-1) get 12 epilogue warps: their GELU / residual epilogues are ALU- and latency-bound.
-// The 128x128 x3 tiles keep three 64 KB stages: only four epilogue warps' transpose scratch fits beside them.
-// (so does the experimental four-stage variant of the 128x64 x3 tile: DVT_GEMM_X3_STAGES=4)
-constexpr int epi_warps(int bn, bool x3, int stages) { return (bn == 256 && !x3) ? 12 : (x3 && (bn == 128 || stages == 4)) ? 4 : 8; }
-constexpr int SCR_PITCH = 36;  // floats; 16B-aligned rows, conflict-free for the access pattern below
 
-template <int BN, int STAGES, bool X3 = false>
-struct GemmSmem {
-  static constexpr int EW = epi_warps(BN, X3, STAGES);
-  static constexpr int THREADS = 32 * (2 + EW);
-  static constexpr int A_BYTES = BM * KB_BYTES * (X3 ? 2 : 1);  // x3: hi plane then lo plane
-  static constexpr int B_BYTES = BN * KB_BYTES * (X3 ? 2 : 1);
-  static constexpr int SCR_BYTES = EW * 32 * SCR_PITCH * 4;
-  static constexpr int OFF_A = 0;
-  static constexpr int OFF_B = OFF_A + STAGES * A_BYTES;
-  static constexpr int OFF_SCR = OFF_B + STAGES * B_BYTES;
-  static constexpr int OFF_BAR = OFF_SCR + SCR_BYTES;
-  static constexpr int NUM_BARS = 2 * STAGES + 4;
-  static constexpr int OFF_TMEM = OFF_BAR + NUM_BARS * 8;
-  static constexpr int TOTAL = OFF_TMEM + 16 + 1024;  // + alignment slack
+// wgmma kernel
+constexpr int WG_BN = 128;
+constexpr int WG_STAGES = 3;
+constexpr int WG_THREADS = 288;                      // 2 consumer warpgroups + 1 producer warp
+constexpr int WG_STAGE_BYTES = (BM + WG_BN) * KB_BYTES;
+constexpr int WG_OFF_BAR = WG_STAGES * WG_STAGE_BYTES;
+constexpr int WG_SMEM = WG_OFF_BAR + 2 * WG_STAGES * 8 + 1024;  // + alignment slack
+constexpr int EPI_PITCH = WG_BN + 8;                 // floats per staged accumulator row (16B aligned, conflict-free)
+static_assert(BM * EPI_PITCH * 4 <= WG_OFF_BAR, "staged accumulators must fit in the operand ring");
+static_assert(2 * WG_SMEM <= 227 * 1024, "two CTAs per SM");
+
+// 3xTF32 kernel
+constexpr int X3_STAGES = 3;
+constexpr int X3_THREADS = 256;
+template <int BN>
+struct X3Smem {
+  static constexpr int A_BYTES = 2 * BM * KB_BYTES;  // hi plane then lo plane (K-major) / 32-column atoms (MN-major)
+  static constexpr int B_BYTES = 2 * BN * KB_BYTES;
+  static constexpr int STAGE = A_BYTES + B_BYTES;
+  static constexpr int OFF_BAR = X3_STAGES * STAGE;
+  static constexpr int PITCH = BN + 8;
+  static constexpr int TOTAL = OFF_BAR + X3_STAGES * 8 + 1024;
+  static_assert(BM * PITCH * 4 <= OFF_BAR, "staged accumulators must fit in the operand ring");
 };
 
-// Ragged-N tail of one 32x32 chunk (last chunk of N = 385, 129, ...): rare, so its loops stay rolled (unrolled it
-// made every kernel 130 KB; an out-of-line call was tried too and cost 30 % on the big GEMMs through ABI spills).
+__device__ __forceinline__ void stamp_ts(const GemmEpi& e, int slot) {
+  if (e.debug_ts && blockIdx.x == 0) {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    e.debug_ts[slot] = t;
+  }
+}
+
 template <bool FIT>
-__device__ __forceinline__ void epi_scalar_tail(const GemmEpi& e, const GemmShape& s, const float* scr, int lane, int m0,
-                                             int n, bool has_k) {
+__device__ __forceinline__ void epi_scalar_tail(const GemmEpi& e, const GemmShape& s, const float* scr, int pitch, int lane,
+                                                int m0, int n, bool has_k) {
 #pragma unroll 1
   for (int jj = 0; jj < 8; ++jj) {
     const int i = (lane >> 3) + 4 * jj;
@@ -59,26 +71,19 @@ __device__ __forceinline__ void epi_scalar_tail(const GemmEpi& e, const GemmShap
 #pragma unroll 1
     for (int q = 0; q < 4; ++q) {
       if (n + q >= s.N) break;
-      const float x = scr[i * SCR_PITCH + (lane & 7) * 4 + q];
+      const float x = scr[i * pitch + (lane & 7) * 4 + q];
       epi_post1<FIT>(e, m, n + q, epi_pre<FIT>(e, m, n + q, has_k ? x : 0.0f));
     }
   }
 }
 
-// One 32-row x 32-column chunk of an accumulator tile, as read by tcgen05.ld 32x32b (thread = row): transpose through the
-// warp's shared-memory scratch, then the fused epilogue in the coalesced layout (each lane: 4 consecutive columns of 8
-// rows).  m0: global row of this lane's first row (tile row base + quadrant * 32 + lane / 8); n_base: global column of the
-// chunk.  Shared by the single-CTA and the CTA-pair kernels.
+// One 32-row x 32-column chunk of an accumulator tile staged in shared memory (`scr`: the chunk's first element, rows
+// `pitch` floats apart), with the fused epilogue in the coalesced layout (each lane: 4 consecutive columns of 8 rows).
+// m0: global row of this lane's first row (chunk row base + lane / 8); n_base: global column of the chunk.  Everything
+// that depends on the column (bias, LayerScale, ...) is loaded once per chunk as a float4.
 template <bool FIT = false>
-__device__ __forceinline__ void epi_chunk(const GemmEpi& e, const GemmShape& s, float* scr, int lane, const uint32_t (&r)[32],
+__device__ __forceinline__ void epi_chunk(const GemmEpi& e, const GemmShape& s, const float* scr, int pitch, int lane,
                                           int n_base, int m0, bool has_k) {
-  // ---- transpose through smem: afterwards each lane holds 4 consecutive columns of 8 rows.  No math on the
-  // thread-per-row registers: everything that depends on the column (bias, LayerScale, ...) is loaded once per
-  // chunk as a float4 in the coalesced layout below.
-#pragma unroll
-  for (int j = 0; j < 8; ++j)
-    *reinterpret_cast<uint4*>(scr + lane * SCR_PITCH + 4 * j) = make_uint4(r[4 * j], r[4 * j + 1], r[4 * j + 2], r[4 * j + 3]);
-  __syncwarp();
   const int col4 = (lane & 7) * 4;
   const int n = n_base + col4;
   if (n + 3 < s.N) {
@@ -104,7 +109,7 @@ __device__ __forceinline__ void epi_chunk(const GemmEpi& e, const GemmShape& s, 
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
           const int m = m0 + 4 * jj;
-          float4 x = *reinterpret_cast<const float4*>(scr + ((lane >> 3) + 4 * jj) * SCR_PITCH + col4);
+          float4 x = *reinterpret_cast<const float4*>(scr + ((lane >> 3) + 4 * jj) * pitch + col4);
           uint2 pk;
           const float2 g01 = gelu_erf2(fadd2(make_float2(x.x, x.y), make_float2(b4.x, b4.y)));
           const float2 g23 = gelu_erf2(fadd2(make_float2(x.z, x.w), make_float2(b4.z, b4.w)));
@@ -116,7 +121,7 @@ __device__ __forceinline__ void epi_chunk(const GemmEpi& e, const GemmShape& s, 
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
           const int m = m0 + 4 * jj;
-          float4 x = *reinterpret_cast<const float4*>(scr + ((lane >> 3) + 4 * jj) * SCR_PITCH + col4);
+          float4 x = *reinterpret_cast<const float4*>(scr + ((lane >> 3) + 4 * jj) * pitch + col4);
           uint2 pk;
           pk.x = pack_bf16x2(fmaxf(x.x + b4.x, 0.0f), fmaxf(x.y + b4.y, 0.0f));
           pk.y = pack_bf16x2(fmaxf(x.z + b4.z, 0.0f), fmaxf(x.w + b4.w, 0.0f));
@@ -126,7 +131,7 @@ __device__ __forceinline__ void epi_chunk(const GemmEpi& e, const GemmShape& s, 
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
           const int m = m0 + 4 * jj;
-          float4 x = *reinterpret_cast<const float4*>(scr + ((lane >> 3) + 4 * jj) * SCR_PITCH + col4);
+          float4 x = *reinterpret_cast<const float4*>(scr + ((lane >> 3) + 4 * jj) * pitch + col4);
           const float2 v01 = fadd2(make_float2(x.x, x.y), make_float2(b4.x, b4.y));
           const float2 v23 = fadd2(make_float2(x.z, x.w), make_float2(b4.z, b4.w));
           uint2 pk;
@@ -141,7 +146,7 @@ __device__ __forceinline__ void epi_chunk(const GemmEpi& e, const GemmShape& s, 
 #pragma unroll
       for (int jj = 0; jj < 8; ++jj) {
         const int m = m0 + 4 * jj;
-        const float4 x = *reinterpret_cast<const float4*>(scr + ((lane >> 3) + 4 * jj) * SCR_PITCH + col4);
+        const float4 x = *reinterpret_cast<const float4*>(scr + ((lane >> 3) + 4 * jj) * pitch + col4);
         const float2 o01 = ffma2(make_float2(g4.x, g4.y), fadd2(make_float2(x.x, x.y), make_float2(b4.x, b4.y)),
                                  make_float2(xin[jj].x, xin[jj].y));
         const float2 o23 = ffma2(make_float2(g4.z, g4.w), fadd2(make_float2(x.z, x.w), make_float2(b4.z, b4.w)),
@@ -154,7 +159,7 @@ __device__ __forceinline__ void epi_chunk(const GemmEpi& e, const GemmShape& s, 
       for (int jj = 0; jj < 8; ++jj) {
       const int i = (lane >> 3) + 4 * jj;
       const int m = m0 + 4 * jj;
-      float4 x = *reinterpret_cast<const float4*>(scr + i * SCR_PITCH + col4);
+      float4 x = *reinterpret_cast<const float4*>(scr + i * pitch + col4);
       if (m >= s.M) continue;
       if (!has_k) x = make_float4(0.f, 0.f, 0.f, 0.f);
       x.x += b4.x; x.y += b4.y; x.z += b4.z; x.w += b4.w;
@@ -190,283 +195,296 @@ __device__ __forceinline__ void epi_chunk(const GemmEpi& e, const GemmShape& s, 
     }
   } else {
     // ---------------- ragged N tail: scalar path ----------------
-    epi_scalar_tail<FIT>(e, s, scr, lane, m0, n, has_k);
+    epi_scalar_tail<FIT>(e, s, scr, pitch, lane, m0, n, has_k);
   }
   }
 
-template <int BN, int STAGES, bool TF32, bool A_MN, bool B_MN, bool X3 = false>
-__global__ void __launch_bounds__(GemmSmem<BN, STAGES, X3>::THREADS, 1)
-gemm_tn_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmShape s,
-                  GemmEpi e) {
-  static_assert(!X3 || TF32, "x3 is a TF32 mode");
-  static_assert(X3 || !(TF32 && (A_MN || B_MN)), "plain TF32 is K-major only");
-  using L = GemmSmem<BN, STAGES, X3>;
-  constexpr int ELEM = TF32 ? 4 : 2;
-  constexpr int BK = KB_BYTES / ELEM;         // elements of K per stage
-  constexpr int UMMA_K_BYTES = 32;            // K=16 bf16 or K=8 tf32 per instruction
-  constexpr int MMAS_PER_STAGE = KB_BYTES / UMMA_K_BYTES;
-  // x3 with a K-major B: the hi and lo planes of a B tile are adjacent [BN x 128 B] blocks, i.e. ONE K-major tile of 2 BN
-  // rows.  A_hi . [B_hi | B_lo] is therefore a single MMA of width 2 BN whose accumulator holds hi.hi in columns [0, BN) and
-  // hi.lo in [BN, 2 BN); A_lo . B_hi accumulates into the first half and the epilogue adds the halves.  Two instructions
-  // per k-step instead of three: a 128 x N x 8 TF32 MMA costs ~78 clk for any N <= 128 (tools/gemm_timeline.py), so the
-  // k-block gets a quarter cheaper.  An MN-major B tile is made of 32-column atoms ([32 k-rows][32 mn] = 4 KB each); for the
-  // same trick its atoms are loaded plane by plane -- [plane][atom] instead of [atom][plane] -- so that the lo atoms
-  // continue the hi atoms at the same 4 KB stride (one more TMA instruction per atom, same bytes).
-  constexpr bool CAT = X3 && 4 * BN <= 512;
-  constexpr int ACC_W = CAT ? 2 * BN : BN;  // TMEM columns of one accumulator stage
-  constexpr uint32_t TMEM_COLS = (2 * ACC_W <= 32) ? 32 : (2 * ACC_W <= 64) ? 64 : (2 * ACC_W <= 128) ? 128
-                                 : (2 * ACC_W <= 256) ? 256 : 512;
-  static_assert(2 * ACC_W <= 512, "two accumulator stages must fit TMEM");
 
+// Tile t of a launch: (split, tile_n, tile_m), split fastest.
+struct TileIdx {
+  int tm, tn, kb0, kb1, kb_total;
+};
+__device__ __forceinline__ TileIdx tile_of(const GemmShape& s, int bn, int bk) {
+  TileIdx r;
+  const int tiles_n = (s.N + bn - 1) / bn;
+  const int t = blockIdx.x;
+  const int split = t % s.splits;
+  const int mn = t / s.splits;
+  r.tn = mn % tiles_n;
+  r.tm = mn / tiles_n;
+  r.kb_total = (s.K + bk - 1) / bk;
+  const int per = (r.kb_total + s.splits - 1) / s.splits;
+  r.kb0 = split * per;
+  r.kb1 = min(r.kb_total, r.kb0 + per);
+  return r;
+}
+
+// Epilogue of a tile whose fp32 accumulators sit in shared memory ([BM][pitch]): warp w of `nwarps` takes the 32 x 32
+// chunks w, w + nwarps, ...
+template <bool FIT, int BN>
+__device__ __forceinline__ void epi_tile(const GemmEpi& e, const GemmShape& s, const float* tile, int pitch, int warp,
+                                         int nwarps, int lane, int tm, int tn, bool has_k) {
+#pragma unroll 1
+  for (int c = warp; c < (BM / 32) * (BN / 32); c += nwarps) {
+    const int rb = c / (BN / 32), cb = c % (BN / 32);
+    const int n_base = tn * BN + cb * 32;
+    if (n_base >= s.N || tm * BM + rb * 32 >= s.M) continue;  // whole chunk out of range (warp-uniform)
+    epi_chunk<FIT>(e, s, tile + rb * 32 * pitch + cb * 32, pitch, lane, n_base, tm * BM + rb * 32 + (lane >> 3), has_k);
+  }
+}
+
+template <bool TF32, bool A_MN, bool B_MN>
+__global__ void __launch_bounds__(WG_THREADS, 2)
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmShape s, GemmEpi e) {
+  static_assert(!(TF32 && (A_MN || B_MN)), "TF32 wgmma operands are K-major only");
+  constexpr int BK = KB_BYTES / (TF32 ? 4 : 2);  // elements of K per stage
+  constexpr int A_BYTES = BM * KB_BYTES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sA = smem + L::OFF_A;
-  uint8_t* sB = smem + L::OFF_B;
-  float* scr_all = reinterpret_cast<float*>(smem + L::OFF_SCR);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::OFF_BAR);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + STAGES;
-  uint64_t* tfull = bars + 2 * STAGES;
-  uint64_t* tempty = bars + 2 * STAGES + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + L::OFF_TMEM);
-
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + WG_OFF_BAR);
+  uint64_t* empty = full + WG_STAGES;
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  auto stampt = [&](int slot) {
-    if (e.debug_ts && blockIdx.x == 0) {
-      unsigned long long t;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-      e.debug_ts[slot] = t;
-    }
-  };
-  if (threadIdx.x == 0) stampt(0);  // kernel entry
-  if (threadIdx.x == 0 && e.debug_ts && blockIdx.x == 0) e.debug_ts[14] = (unsigned long long)clock64();
+  if (threadIdx.x == 0) stamp_ts(e, 0);
+  const TileIdx ti = tile_of(s, WG_BN, BK);
 
-  const int tiles_m = (s.M + BM - 1) / BM;
-  const int tiles_n = (s.N + BN - 1) / BN;
-  const int num_tiles = tiles_m * tiles_n * s.splits;
-  const int kb_total = (s.K + BK - 1) / BK;
-  const int kb_per_split = (kb_total + s.splits - 1) / s.splits;
-
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int i = 0; i < STAGES; ++i) {
+    for (int i = 0; i < WG_STAGES; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      mbar_init(&tempty[i], L::EW * 32);
+      mbar_init(&empty[i], 8);
     }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (threadIdx.x == 0) stampt(1);  // setup done (barriers, TMEM)
   // PDL: everything above overlapped the tail of the previous kernel; its results are needed from here on
   pdl_wait();
   pdl_trigger();
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===================== TMA producer =====================
     if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        const int split = t % s.splits;
-        const int mn = t / s.splits;
-        const int tn = mn % tiles_n;
-        const int tm = mn / tiles_n;
-        const int kb0 = split * kb_per_split;
-        const int kb1 = min(kb_total, kb0 + kb_per_split);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&empty[stage], phase ^ 1, 1);
-          mbar_expect_tx(&full[stage], L::A_BYTES + L::B_BYTES);
-          if (X3) {
-            // fp32 hi/lo planes: 3-D maps (inner, rows, plane); one box brings both planes of a tile / atom
-            if (A_MN) {
+      for (int kb = ti.kb0, it = 0; kb < ti.kb1; ++kb, ++it) {
+        const int st = it % WG_STAGES;
+        mbar_wait_relaxed(&empty[st], ((it / WG_STAGES) & 1) ^ 1, 1);
+        uint8_t* sA = smem + st * WG_STAGE_BYTES;
+        uint8_t* sB = sA + A_BYTES;
+        mbar_expect_tx(&full[st], WG_STAGE_BYTES);
+        if (A_MN) {  // stored [K, M]: boxes of 64 (M, contiguous) x BK (K rows) = one MN-major swizzle-atom column each
 #pragma unroll
-              for (int a = 0; a < BM / 32; ++a)
-                tma_load_3d(sA + stage * L::A_BYTES + a * 8192, &tmA, &full[stage], tm * BM + a * 32, kb * BK, 0);
-            } else {
-              tma_load_3d(sA + stage * L::A_BYTES, &tmA, &full[stage], kb * BK, tm * BM, 0);
-            }
-            if (B_MN) {
-              // (tensor map box = ONE plane of an atom: launch_gemm_tn)
-#pragma unroll
-              for (int pl = 0; pl < 2; ++pl)
-#pragma unroll
-                for (int a = 0; a < BN / 32; ++a)
-                  tma_load_3d(sB + stage * L::B_BYTES + (pl * (BN / 32) + a) * 4096, &tmB, &full[stage], tn * BN + a * 32, kb * BK, pl);
-            } else {
-              tma_load_3d(sB + stage * L::B_BYTES, &tmB, &full[stage], kb * BK, tn * BN, 0);
-            }
-          } else {
-            if (A_MN) {
-              // stored [K, M]: boxes of 64 (M, contiguous) x BK (K rows) = one MN-major swizzle-atom column each
-#pragma unroll
-              for (int a = 0; a < BM / 64; ++a)
-                tma_load_2d(sA + stage * L::A_BYTES + a * (BK * 128), &tmA, &full[stage], tm * BM + a * 64, kb * BK);
-            } else {
-              tma_load_2d(sA + stage * L::A_BYTES, &tmA, &full[stage], kb * BK, tm * BM);
-            }
-            if (B_MN) {
-#pragma unroll
-              for (int a = 0; a < BN / 64; ++a)
-                tma_load_2d(sB + stage * L::B_BYTES + a * (BK * 128), &tmB, &full[stage], tn * BN + a * 64, kb * BK);
-            } else {
-              tma_load_2d(sB + stage * L::B_BYTES, &tmB, &full[stage], kb * BK, tn * BN);
-            }
-          }
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(TF32 ? 2u : 1u, BM, BN, A_MN ? 1u : 0u, B_MN ? 1u : 0u);
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        const int split = t % s.splits;
-        const int kb0 = split * kb_per_split;
-        const int kb1 = min(kb_total, kb0 + kb_per_split);
-        mbar_wait(&tempty[as], aphase ^ 1, 2);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * ACC_W;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full[stage], phase, 3);
-          tc_fence_after();
-          if (kb == kb0) stampt(2);  // first operands landed
-          // K-major: rows of 128 B (one swizzle atom of K), 8-row groups 1024 B apart; K advances 32 B per MMA.
-          // MN-major (bf16): tile = [MN/64 atoms][BK k-rows][64 mn]; atoms BK*128 B apart (LBO), 8-k groups 1024 B
-          // apart (SBO); K advances 16 rows = 2048 B per MMA.
-          // x3 (fp32 hi/lo planes): K-major tile = [plane][rows][128 B]; MN-major A tile = [MN/32 atoms][plane][32 k-rows]
-          // [32 mn] (atoms 8192 B apart, lo plane +4096 B), MN-major B tile = [plane][MN/32 atoms][32 k-rows][32 mn] (atoms
-          // 4096 B apart, lo plane after the hi atoms); K advances 8 rows = 1024 B per MMA.  MN-major TF32 operands
-          // must use the "128B swizzle with 32B atoms" layout (descriptor layout type 1, TMA SWIZZLE_128B_ATOM_32B):
-          // the swizzle pattern repeats every 4 K-rows, so the stride between K groups (SBO) is 512 B.
-          const uint32_t a_base = smem_u32(sA + stage * L::A_BYTES), b_base = smem_u32(sB + stage * L::B_BYTES);
-          if (X3) {
-            const uint32_t a_lo = a_base + (A_MN ? 4096 : BM * KB_BYTES), b_lo = b_base + (B_MN ? (BN / 32) * 4096 : BN * KB_BYTES);
-            const uint32_t lbo_a = A_MN ? 8192 : 0, lbo_b = B_MN ? 4096 : 0;
-#pragma unroll
-            for (int k = 0; k < MMAS_PER_STAGE; ++k) {
-              const uint32_t ka = A_MN ? k * 1024 : k * UMMA_K_BYTES, kbb = B_MN ? k * 1024 : k * UMMA_K_BYTES;
-              constexpr uint32_t sbo_a = A_MN ? 512 : 1024, sbo_b = B_MN ? 512 : 1024;
-              constexpr uint32_t lt_a = A_MN ? 1 : 2, lt_b = B_MN ? 1 : 2;
-              const uint64_t dah = make_smem_desc(a_base + ka, lbo_a, sbo_a, lt_a), dal = make_smem_desc(a_lo + ka, lbo_a, sbo_a, lt_a);
-              const uint64_t dbh = make_smem_desc(b_base + kbb, lbo_b, sbo_b, lt_b), dbl = make_smem_desc(b_lo + kbb, lbo_b, sbo_b, lt_b);
-              const uint32_t acc0 = (kb > kb0 || k > 0) ? 1u : 0u;
-              if (CAT && s.x3 == 1) {
-                constexpr uint32_t idesc_cat = make_idesc(2u, BM, 2 * BN, A_MN ? 1u : 0u, B_MN ? 1u : 0u);
-                umma_tf32(d_tmem, dah, dbh, idesc_cat, acc0);  // [hi.hi | hi.lo]: the descriptor at B_hi spans both planes
-                umma_tf32(d_tmem, dal, dbh, idesc, 1u);        // + lo.hi
-              } else if (s.x3 == 1) {
-                umma_tf32(d_tmem, dal, dbh, idesc, acc0);  // small terms first
-                umma_tf32(d_tmem, dah, dbl, idesc, 1u);
-                umma_tf32(d_tmem, dah, dbh, idesc, 1u);
-              } else {  // x3 == 2: plain TF32 product of the hi parts (same operand layout, a third of the MMA work)
-                umma_tf32(d_tmem, dah, dbh, idesc, acc0);
-              }
-            }
-          } else {
-            const uint64_t da = make_smem_desc(a_base, A_MN ? BK * 128 : 0, 1024, 2);
-            const uint64_t db = make_smem_desc(b_base, B_MN ? BK * 128 : 0, 1024, 2);
-#pragma unroll
-            for (int k = 0; k < MMAS_PER_STAGE; ++k) {
-              const uint64_t adv_a = (uint64_t)((A_MN ? k * 2048 : k * UMMA_K_BYTES) >> 4);
-              const uint64_t adv_b = (uint64_t)((B_MN ? k * 2048 : k * UMMA_K_BYTES) >> 4);
-              if (TF32) umma_tf32(d_tmem, da + adv_a, db + adv_b, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-              else umma_f16(d_tmem, da + adv_a, db + adv_b, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-            }
-          }
-          umma_commit(&empty[stage]);  // frees the smem slot once these MMAs have read it
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(&tfull[as]);  // accumulator complete
-        stampt(3);                // all MMAs issued
-        if (++as == 2) {
-          as = 0;
-          aphase ^= 1;
-        }
-      }
-    }
-  } else {
-    // ===================== epilogue warps =====================
-    const int ew = warp - 2;
-    const int quad = warp & 3;  // TMEM lane quadrant this warp may access
-    constexpr int CSTEP = L::EW / 4;       // warps sharing a quadrant
-    const int c_first = ew >> 2;           // ... take alternating 32-column chunks
-    float* scr = scr_all + ew * 32 * SCR_PITCH;
-    int as = 0;
-    uint32_t aphase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      const int split = t % s.splits;
-      const int mn = t / s.splits;
-      const int tn = mn % tiles_n;
-      const int tm = mn / tiles_n;
-      const int kb0 = split * kb_per_split;
-      const bool has_k = kb0 < kb_total;
-      mbar_wait(&tfull[as], aphase, 4);
-      tc_fence_after();
-      if (ew == 0 && lane == 0) stampt(4);  // accumulator ready, epilogue starts
-      const uint32_t taddr_row = tmem_base + ((uint32_t)(quad * 32) << 16) + as * ACC_W;
-#pragma unroll 1
-      for (int c = c_first; c < BN / 32; c += CSTEP) {
-        uint32_t r[32];
-        tmem_ld_32x32(taddr_row + c * 32, r);
-        if (CAT && s.x3 == 1) {
-          uint32_t r2[32];
-          tmem_ld_32x32(taddr_row + BN + c * 32, r2);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) + __uint_as_float(r2[i]));
+          for (int a = 0; a < BM / 64; ++a) tma_load_2d(sA + a * (BK * 128), &tmA, &full[st], ti.tm * BM + a * 64, kb * BK);
         } else {
-          tmem_ld_wait();
+          tma_load_2d(sA, &tmA, &full[st], kb * BK, ti.tm * BM);
         }
-        if (c + CSTEP >= BN / 32) {  // this warp's last read of the accumulator stage
-          tc_fence_before();
-          mbar_arrive(&tempty[as]);
+        if (B_MN) {
+#pragma unroll
+          for (int a = 0; a < WG_BN / 64; ++a) tma_load_2d(sB + a * (BK * 128), &tmB, &full[st], ti.tn * WG_BN + a * 64, kb * BK);
+        } else {
+          tma_load_2d(sB, &tmB, &full[st], kb * BK, ti.tn * WG_BN);
         }
-        const int n_base = tn * BN + c * 32;
-        if (n_base >= s.N) continue;  // whole chunk out of range (warp-uniform)
-        epi_chunk<X3>(e, s, scr, lane, r, n_base, tm * BM + quad * 32 + (lane >> 3), has_k);
-        __syncwarp();
-        if (ew == 0 && lane == 0) stampt(8 + (c & 7));  // chunk done (profiling aid)
-      }
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1;
       }
     }
+    return;
   }
 
-  if (warp == 2 && lane == 0) stampt(5);  // first epilogue warp done
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
+  // ===================== consumer warpgroups =====================
+  const int wg = warp >> 2;  // rows [64 wg, 64 wg + 64) of the tile
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  reg_fence(acc);
+  for (int kb = ti.kb0, it = 0; kb < ti.kb1; ++kb, ++it) {
+    const int st = it % WG_STAGES;
+    mbar_wait(&full[st], (it / WG_STAGES) & 1, 3);
+    const uint32_t a_base = smem_u32(smem + st * WG_STAGE_BYTES), b_base = a_base + A_BYTES;
+    // K-major: rows of 128 B, K advances 32 B per MMA.  MN-major: [64-wide atoms, BK * 128 B apart][BK k-rows of 128 B];
+    // K advances 16 rows = 2048 B per MMA.
+    const uint64_t da = A_MN ? make_wgmma_desc(a_base + wg * (BK * 128), BK * 128, 1024) : make_wgmma_desc(a_base + wg * 64 * 128, 0, 1024);
+    const uint64_t db = make_wgmma_desc(b_base, B_MN ? BK * 128 : 0, 1024);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const uint64_t adv_a = (uint64_t)((A_MN ? k * 2048 : k * 32) >> 4);
+      const uint64_t adv_b = (uint64_t)((B_MN ? k * 2048 : k * 32) >> 4);
+      if constexpr (TF32) wgmma_128_tf32(acc, da + adv_a, db + adv_b);
+      else wgmma_128_bf16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da + adv_a, db + adv_b);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();  // the MMAs of the previous stage have completed: release its slot
+    reg_fence(acc);
+    if (it > 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[(it - 1) % WG_STAGES]);
+    }
   }
-  if (threadIdx.x == 0) stampt(6);  // kernel exit
-  if (threadIdx.x == 0 && e.debug_ts && blockIdx.x == 0) e.debug_ts[15] = (unsigned long long)clock64();
+  wgmma_wait<0>();
+  reg_fence(acc);
+
+  // ---- stage the accumulators in the drained operand ring, then the fused epilogue ----
+  named_bar(1, 256);  // both warpgroups are done reading operands
+  float* tile = reinterpret_cast<float*>(smem);
+  {
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int c0 = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      *reinterpret_cast<float2*>(tile + r0 * EPI_PITCH + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(tile + (r0 + 8) * EPI_PITCH + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    }
+  }
+  named_bar(1, 256);
+  epi_tile<false, WG_BN>(e, s, tile, EPI_PITCH, warp, 8, lane, ti.tm, ti.tn, ti.kb0 < ti.kb_total);
+  if (threadIdx.x == 0) stamp_ts(e, 6);
+}
+
+// ----------------------------------------------------------------------------------------------------
+// 3xTF32 ("x3"): fp32-accurate products of fp32 operands stored as hi / lo planes.  Per stage a 128 x 32 slab of A and a
+// BN x 32 slab of B, both planes, through TMA with 128-byte swizzle:
+//   K-major operand   [plane][rows][32 fp32]                    (one 3-D box)
+//   MN-major operand  [32-wide atoms][plane][32 k-rows][32 fp32] (one 3-D box per atom)
+// 8 warps in a 4 (M) x 2 (N) grid, each 32 x BN/2 of the tile.
+// ----------------------------------------------------------------------------------------------------
+template <int ROWS, bool MN>
+__device__ __forceinline__ uint32_t x3_ld(const uint8_t* base, int r, int k, int plane) {
+  uint32_t off;
+  if (MN) off = (r >> 5) * 8192 + plane * 4096 + k * 128 + ((((r & 31) >> 2) ^ (k & 7)) << 4) + (r & 3) * 4;
+  else off = plane * (ROWS * 128) + r * 128 + (((k >> 2) ^ (r & 7)) << 4) + (k & 3) * 4;
+  return *reinterpret_cast<const uint32_t*>(base + off);
+}
+
+__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+}
+
+template <int BN, bool A_MN, bool B_MN>
+__global__ void __launch_bounds__(X3_THREADS, 1)
+gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmShape s, GemmEpi e) {
+  using L = X3Smem<BN>;
+  constexpr int BK = 32;
+  constexpr int WN = BN / 2;   // columns per warp
+  constexpr int NT = WN / 8;   // n8 sub-tiles per warp
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + L::OFF_BAR);
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int g = lane >> 2, t = lane & 3;
+  const int wm = warp & 3, wn = warp >> 2;
+  if (threadIdx.x == 0) stamp_ts(e, 0);
+  const TileIdx ti = tile_of(s, BN, BK);
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    for (int i = 0; i < X3_STAGES; ++i) mbar_init(&full[i], 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_wait();
+  pdl_trigger();
+
+  auto issue = [&](int kb, int st) {
+    uint8_t* sA = smem + st * L::STAGE;
+    uint8_t* sB = sA + L::A_BYTES;
+    mbar_expect_tx(&full[st], L::STAGE);
+    if (A_MN) {
+#pragma unroll
+      for (int a = 0; a < BM / 32; ++a) tma_load_3d(sA + a * 8192, &tmA, &full[st], ti.tm * BM + a * 32, kb * BK, 0);
+    } else {
+      tma_load_3d(sA, &tmA, &full[st], kb * BK, ti.tm * BM, 0);
+    }
+    if (B_MN) {
+#pragma unroll
+      for (int a = 0; a < BN / 32; ++a) tma_load_3d(sB + a * 8192, &tmB, &full[st], ti.tn * BN + a * 32, kb * BK, 0);
+    } else {
+      tma_load_3d(sB, &tmB, &full[st], kb * BK, ti.tn * BN, 0);
+    }
+  };
+  if (threadIdx.x == 0)
+    for (int i = 0; i < X3_STAGES && ti.kb0 + i < ti.kb1; ++i) issue(ti.kb0 + i, i);
+
+  float acc[2][NT][4];
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int ni = 0; ni < NT; ++ni)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) acc[mi][ni][q] = 0.f;
+
+  for (int kb = ti.kb0, it = 0; kb < ti.kb1; ++kb, ++it) {
+    const int st = it % X3_STAGES;
+    mbar_wait(&full[st], (it / X3_STAGES) & 1, 3);
+    const uint8_t* sA = smem + st * L::STAGE;
+    const uint8_t* sB = sA + L::A_BYTES;
+#pragma unroll
+    for (int kk = 0; kk < BK; kk += 8) {
+      uint32_t ah[2][4], al[2][4];
+#pragma unroll
+      for (int mi = 0; mi < 2; ++mi) {
+        const int r = wm * 32 + mi * 16 + g;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int rr = r + (q & 1) * 8, k = kk + t + (q >> 1) * 4;
+          ah[mi][q] = x3_ld<BM, A_MN>(sA, rr, k, 0);
+          al[mi][q] = x3_ld<BM, A_MN>(sA, rr, k, 1);
+        }
+      }
+#pragma unroll
+      for (int ni = 0; ni < NT; ++ni) {
+        const int n = wn * WN + ni * 8 + g;
+        uint32_t bh[2], bl[2];
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+          bh[q] = x3_ld<BN, B_MN>(sB, n, kk + t + 4 * q, 0);
+          bl[q] = x3_ld<BN, B_MN>(sB, n, kk + t + 4 * q, 1);
+        }
+#pragma unroll
+        for (int mi = 0; mi < 2; ++mi) {
+          if (s.x3 == 1) {
+            mma_tf32(acc[mi][ni], al[mi], bh);  // small terms first
+            mma_tf32(acc[mi][ni], ah[mi], bl);
+          }
+          mma_tf32(acc[mi][ni], ah[mi], bh);  // (x3 == 2: the hi parts only, plain TF32 accuracy)
+        }
+      }
+    }
+    __syncthreads();  // every warp is done with this slot
+    if (threadIdx.x == 0 && kb + X3_STAGES < ti.kb1) issue(kb + X3_STAGES, st);
+  }
+
+  // ---- stage the accumulators in the drained operand ring, then the fused epilogue ----
+  float* tile = reinterpret_cast<float*>(smem);
+#pragma unroll
+  for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+    for (int ni = 0; ni < NT; ++ni) {
+      const int r = wm * 32 + mi * 16 + g, c = wn * WN + ni * 8 + 2 * t;
+      *reinterpret_cast<float2*>(tile + r * L::PITCH + c) = make_float2(acc[mi][ni][0], acc[mi][ni][1]);
+      *reinterpret_cast<float2*>(tile + (r + 8) * L::PITCH + c) = make_float2(acc[mi][ni][2], acc[mi][ni][3]);
+    }
+  __syncthreads();
+  // split-K with counters: split k of a tile adds its partial sums once splits 0 .. k-1 have added theirs (lower block
+  // indices, scheduled first), so every element is summed in split order
+  const bool serial = e.splitk_sem != nullptr && s.splits > 1;
+  unsigned* sem = e.splitk_sem + blockIdx.x / s.splits;
+  const unsigned split = blockIdx.x % s.splits;
+  if (serial) {
+    if (threadIdx.x == 0) {
+      const long long t0 = clock64();
+      while (ld_acquire_u32(sem) != split)
+        if (clock64() - t0 > DVT_WATCHDOG_CYCLES) dev_fail(0x5E3u, split);
+    }
+    __syncthreads();
+  }
+  epi_tile<true, BN>(e, s, tile, L::PITCH, warp, 8, lane, ti.tm, ti.tn, ti.kb0 < ti.kb_total);
+  if (serial) {
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) st_release_u32(sem, split + 1 == (unsigned)s.splits ? 0u : split + 1);
+  }
+  if (threadIdx.x == 0) stamp_ts(e, 6);
 }
 
 // ----------------------------------------------------------------------------------------------------
@@ -511,32 +529,29 @@ __global__ void gemm_tn_simt_kernel(const T* __restrict__ A, int lda, const T* _
   }
 }
 
-template <int BN, int STAGES, bool TF32, bool A_MN, bool B_MN, bool X3 = false>
-int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& s, const GemmEpi& e,
-              cudaStream_t stream) {
-  using L = GemmSmem<BN, STAGES, X3>;
-  auto kern = gemm_tn_tc_kernel<BN, STAGES, TF32, A_MN, B_MN, X3>;
-  const int tiles = ((s.M + BM - 1) / BM) * ((s.N + BN - 1) / BN) * s.splits;
-  int grid = tiles < num_sms() ? tiles : num_sms();
-  // DVT_GEMM_TILES_PER_CTA=n (n > 0) bounds the tiles one CTA works through, i.e. launches more, shorter-lived CTAs than
-  // SMs: a persistent CTA keeps its SM for the whole kernel, which starves concurrent high-priority streams (the fit
-  // running beside the next image's ViT forwards); short-lived CTAs hand SMs over every few microseconds instead.
-  static int tiles_per_cta = -1;
-  if (tiles_per_cta < 0) {
-    const char* v = getenv("DVT_GEMM_TILES_PER_CTA");
-    tiles_per_cta = v ? atoi(v) : 0;
-  }
-  if (!X3 && tiles_per_cta > 0) grid = std::max(grid, (tiles + tiles_per_cta - 1) / tiles_per_cta);
-  DVT_CUDA_OK(launch_kx(LaunchOpt{s.pdl != 0, s.prio_drop}, kern, dim3(grid), dim3(L::THREADS), (size_t)L::TOTAL, stream, tmA, tmB, s, e));
+template <bool TF32, bool A_MN, bool B_MN>
+int launch_wgmma(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& s, const GemmEpi& e, cudaStream_t stream) {
+  const int tiles = ((s.M + BM - 1) / BM) * ((s.N + WG_BN - 1) / WG_BN) * s.splits;
+  DVT_CUDA_OK(launch_kx(LaunchOpt{s.pdl != 0, s.prio_drop}, gemm_wgmma_kernel<TF32, A_MN, B_MN>, dim3(tiles),
+                        dim3(WG_THREADS), (size_t)WG_SMEM, stream, tmA, tmB, s, e));
   count_launch();
   DVT_CUDA_OK(cudaGetLastError());
   return DVT_OK;
 }
 
-template <int BN, int STAGES, bool TF32, bool A_MN, bool B_MN, bool X3 = false>
-int prep_one() {
-  DVT_CUDA_OK(cudaFuncSetAttribute(gemm_tn_tc_kernel<BN, STAGES, TF32, A_MN, B_MN, X3>,
-                                   cudaFuncAttributeMaxDynamicSharedMemorySize, GemmSmem<BN, STAGES, X3>::TOTAL));
+template <int BN, bool A_MN, bool B_MN>
+int launch_x3(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& s, const GemmEpi& e, cudaStream_t stream) {
+  const int tiles = ((s.M + BM - 1) / BM) * ((s.N + BN - 1) / BN) * s.splits;
+  DVT_CUDA_OK(launch_kx(LaunchOpt{s.pdl != 0, s.prio_drop}, gemm_x3_kernel<BN, A_MN, B_MN>, dim3(tiles), dim3(X3_THREADS),
+                        (size_t)X3Smem<BN>::TOTAL, stream, tmA, tmB, s, e));
+  count_launch();
+  DVT_CUDA_OK(cudaGetLastError());
+  return DVT_OK;
+}
+
+template <typename K>
+int set_smem(K kern, int bytes) {
+  DVT_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
   return DVT_OK;
 }
 
@@ -547,38 +562,29 @@ int gemm_prepare() {
   static bool done = false;
   if (done) return DVT_OK;
   int rc;
-  if ((rc = prep_one<256, 3, true, false, false>())) return rc;
-  if ((rc = prep_one<128, 5, true, false, false>())) return rc;
-  if ((rc = prep_one<256, 3, false, true, true>())) return rc;
-  if ((rc = prep_one<128, 5, false, true, true>())) return rc;
-  if ((rc = prep_one<256, 3, false, false, true>())) return rc;
-  if ((rc = prep_one<128, 5, false, false, true>())) return rc;
-  if ((rc = prep_one<256, 3, false, false, false>())) return rc;
-  if ((rc = prep_one<128, 5, false, false, false>())) return rc;
-  if ((rc = prep_one<64, 3, true, false, false, true>())) return rc;
-  if ((rc = prep_one<64, 3, true, false, true, true>())) return rc;
-  if ((rc = prep_one<64, 3, true, true, true, true>())) return rc;
-  if ((rc = prep_one<64, 4, true, false, false, true>())) return rc;
-  if ((rc = prep_one<64, 4, true, false, true, true>())) return rc;
-  if ((rc = prep_one<64, 4, true, true, true, true>())) return rc;
-  if ((rc = prep_one<128, 3, true, false, false, true>())) return rc;
-  if ((rc = prep_one<128, 3, true, false, true, true>())) return rc;
-  if ((rc = prep_one<128, 3, true, true, true, true>())) return rc;
+  if ((rc = set_smem(gemm_wgmma_kernel<true, false, false>, WG_SMEM))) return rc;
+  if ((rc = set_smem(gemm_wgmma_kernel<false, false, false>, WG_SMEM))) return rc;
+  if ((rc = set_smem(gemm_wgmma_kernel<false, false, true>, WG_SMEM))) return rc;
+  if ((rc = set_smem(gemm_wgmma_kernel<false, true, true>, WG_SMEM))) return rc;
+  if ((rc = set_smem(gemm_x3_kernel<64, false, false>, X3Smem<64>::TOTAL))) return rc;
+  if ((rc = set_smem(gemm_x3_kernel<64, false, true>, X3Smem<64>::TOTAL))) return rc;
+  if ((rc = set_smem(gemm_x3_kernel<64, true, true>, X3Smem<64>::TOTAL))) return rc;
+  if ((rc = set_smem(gemm_x3_kernel<128, false, false>, X3Smem<128>::TOTAL))) return rc;
+  if ((rc = set_smem(gemm_x3_kernel<128, false, true>, X3Smem<128>::TOTAL))) return rc;
+  if ((rc = set_smem(gemm_x3_kernel<128, true, true>, X3Smem<128>::TOTAL))) return rc;
   done = true;
   return DVT_OK;
 }
 
-// Tile width of the 3xTF32 kernels.  Measured on the fit's shapes (tools/gemm_timeline.py): a k-block costs ~0.66 us with
-// 12 MMAs whether the tile is 128 x 64 or 128 x 128 (each 128 x N x 8 TF32 instruction takes ~78 clk for N <= 128), so the
-// wide tile halves the tensor time and moves a third less operand data through L2 per flop; the narrow tile gives twice
-// the CTAs and the shorter epilogue.  The caller chooses per call (GemmShape::x3_wide_min_n; 0 = always 128 x 64).
+// Tile width of the 3xTF32 kernels: 128 x 128 halves the operand traffic per flop, 128 x 64 gives twice the CTAs and the
+// shorter epilogue.  The caller chooses per call (GemmShape::x3_wide_min_n; 0 = always 128 x 64).
 int gemm_x3_tile_n(int N, int wide_min_n) { return (wide_min_n > 0 && N >= wide_min_n) ? 128 : 64; }
 
 int default_gemm_impl() {
   static int impl = -1;
   if (impl < 0) {
     const char* v = getenv("DVT_GEMM_IMPL");
-    impl = (v && v[0] == 's') ? GEMM_SIMT_DEBUG : GEMM_TCGEN05;
+    impl = (v && v[0] == 's') ? GEMM_SIMT_DEBUG : GEMM_TC;
   }
   return impl;
 }
@@ -624,26 +630,20 @@ int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dty
     CUtensorMap tA, tB;
     int rc3;
     const int bn3 = gemm_x3_tile_n(s.N, s.x3_wide_min_n);
-    if (s.a_mn) rc3 = make_tmap_3d(&tA, A, TMAP_F32, (uint64_t)s.M, (uint64_t)s.K, 2, (uint64_t)lda * 4, s.plane_a * 4, 32, 32, 2, true);
+    if (s.a_mn) rc3 = make_tmap_3d(&tA, A, TMAP_F32, (uint64_t)s.M, (uint64_t)s.K, 2, (uint64_t)lda * 4, s.plane_a * 4, 32, 32, 2);
     else rc3 = make_tmap_3d(&tA, A, TMAP_F32, (uint64_t)s.K, (uint64_t)s.M, 2, (uint64_t)lda * 4, s.plane_a * 4, 32, BM, 2);
     if (rc3) return rc3;
-    if (s.b_mn) rc3 = make_tmap_3d(&tB, B, TMAP_F32, (uint64_t)s.N, (uint64_t)s.K, 2, (uint64_t)ldb * 4, s.plane_b * 4, 32, 32, 1, true);
+    if (s.b_mn) rc3 = make_tmap_3d(&tB, B, TMAP_F32, (uint64_t)s.N, (uint64_t)s.K, 2, (uint64_t)ldb * 4, s.plane_b * 4, 32, 32, 2);
     else rc3 = make_tmap_3d(&tB, B, TMAP_F32, (uint64_t)s.K, (uint64_t)s.N, 2, (uint64_t)ldb * 4, s.plane_b * 4, 32, bn3, 2);
     if (rc3) return rc3;
     if (bn3 == 128) {
-      if (s.a_mn) return launch_tc<128, 3, true, true, true, true>(tA, tB, s, epi, stream);
-      if (s.b_mn) return launch_tc<128, 3, true, false, true, true>(tA, tB, s, epi, stream);
-      return launch_tc<128, 3, true, false, false, true>(tA, tB, s, epi, stream);
+      if (s.a_mn) return launch_x3<128, true, true>(tA, tB, s, epi, stream);
+      if (s.b_mn) return launch_x3<128, false, true>(tA, tB, s, epi, stream);
+      return launch_x3<128, false, false>(tA, tB, s, epi, stream);
     }
-    static const bool four = [] { const char* e = getenv("DVT_GEMM_X3_STAGES"); return e && e[0] == '4'; }();
-    if (four) {  // experiment: a fourth 48 KB stage (and four epilogue warps) for the 128 x 64 tile
-      if (s.a_mn) return launch_tc<64, 4, true, true, true, true>(tA, tB, s, epi, stream);
-      if (s.b_mn) return launch_tc<64, 4, true, false, true, true>(tA, tB, s, epi, stream);
-      return launch_tc<64, 4, true, false, false, true>(tA, tB, s, epi, stream);
-    }
-    if (s.a_mn) return launch_tc<64, 3, true, true, true, true>(tA, tB, s, epi, stream);
-    if (s.b_mn) return launch_tc<64, 3, true, false, true, true>(tA, tB, s, epi, stream);
-    return launch_tc<64, 3, true, false, false, true>(tA, tB, s, epi, stream);
+    if (s.a_mn) return launch_x3<64, true, true>(tA, tB, s, epi, stream);
+    if (s.b_mn) return launch_x3<64, false, true>(tA, tB, s, epi, stream);
+    return launch_x3<64, false, false>(tA, tB, s, epi, stream);
   }
   DVT_REQUIRE(dtype == TMAP_BF16 || (!s.a_mn && !s.b_mn), "gemm: MN-major operands are implemented for bf16 only");
   DVT_REQUIRE(!(s.a_mn && !s.b_mn), "gemm: A MN-major with B K-major is not instantiated");
@@ -651,30 +651,18 @@ int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dty
               "gemm: row pitch must be a multiple of 16 bytes (lda=%d ldb=%d elem=%d)", lda, ldb, elem);
   DVT_REQUIRE((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(B) & 15) == 0,
               "gemm: operands must be 16-byte aligned");
-  // wide tiles when N is large enough to fill them; narrow ones for the small fit GEMMs
-  const bool wide = s.N >= 256 && (s.N % 256 == 0 || s.N > 1024);
-  if (dtype == TMAP_BF16 && !s.a_mn && !s.b_mn && wide && s.splits == 1 && s.M >= 256 && epi.out_mode != OUT_F32_ATOMIC &&
-      impl != GEMM_TCGEN05_1CTA && gemm_cg2_enabled())
-    return launch_gemm_cg2(A, lda, B, ldb, s, epi, stream);  // 256 x 256 tiles on CTA pairs (tcgen05 cta_group::2)
   CUtensorMap tmA, tmB;
   int rc;
   if (s.a_mn) rc = make_tmap_2d(&tmA, A, dtype, (uint64_t)s.K, (uint64_t)s.M, (uint64_t)lda * elem, bk, 64);
   else rc = make_tmap_2d(&tmA, A, dtype, (uint64_t)s.M, (uint64_t)s.K, (uint64_t)lda * elem, BM, bk);
   if (rc) return rc;
   if (s.b_mn) rc = make_tmap_2d(&tmB, B, dtype, (uint64_t)s.K, (uint64_t)s.N, (uint64_t)ldb * elem, bk, 64);
-  else rc = make_tmap_2d(&tmB, B, dtype, (uint64_t)s.N, (uint64_t)s.K, (uint64_t)ldb * elem, wide ? 256 : 128, bk);
+  else rc = make_tmap_2d(&tmB, B, dtype, (uint64_t)s.N, (uint64_t)s.K, (uint64_t)ldb * elem, WG_BN, bk);
   if (rc) return rc;
-  if (dtype == TMAP_F32)
-    return wide ? launch_tc<256, 3, true, false, false>(tmA, tmB, s, epi, stream)
-                : launch_tc<128, 5, true, false, false>(tmA, tmB, s, epi, stream);
-  if (s.a_mn)
-    return wide ? launch_tc<256, 3, false, true, true>(tmA, tmB, s, epi, stream)
-                : launch_tc<128, 5, false, true, true>(tmA, tmB, s, epi, stream);
-  if (s.b_mn)
-    return wide ? launch_tc<256, 3, false, false, true>(tmA, tmB, s, epi, stream)
-                : launch_tc<128, 5, false, false, true>(tmA, tmB, s, epi, stream);
-  return wide ? launch_tc<256, 3, false, false, false>(tmA, tmB, s, epi, stream)
-              : launch_tc<128, 5, false, false, false>(tmA, tmB, s, epi, stream);
+  if (dtype == TMAP_F32) return launch_wgmma<true, false, false>(tmA, tmB, s, epi, stream);
+  if (s.a_mn) return launch_wgmma<false, true, true>(tmA, tmB, s, epi, stream);
+  if (s.b_mn) return launch_wgmma<false, false, true>(tmA, tmB, s, epi, stream);
+  return launch_wgmma<false, false, false>(tmA, tmB, s, epi, stream);
 }
 
 }  // namespace dvt

@@ -42,6 +42,8 @@ struct GemmEpi {
   int rows_per_group = 0;             // patches per image
   int group_stride = 0;               // tokens per image
   int row_offset = 0;                 // prefix tokens
+  unsigned* splitk_sem = nullptr;     // OUT_F32_ATOMIC with split-K, 3xTF32 kernel: one zeroed counter per output tile; the
+                                      // splits of a tile then add in split order (a deterministic sum), resetting it to 0
 };
 
 struct GemmShape {
@@ -60,8 +62,7 @@ struct GemmShape {
 };
 
 // FIT = true (the 3xTF32 kernels of the stage-1 fit): epilogue features only other callers use -- GELU, the bf16 mask with
-// GELU', bf16 / residual / remapped outputs -- are compiled out.  The fit's GEMMs are small and latency bound; every
-// instruction the generic epilogue carries along was measured in their run time (profiles/r2_fit_step_ab.txt).
+// GELU', bf16 / residual / remapped outputs -- are compiled out: the fit's GEMMs are small and latency bound.
 template <bool FIT = false>
 __device__ __forceinline__ float epi_pre(const GemmEpi& e, int m, int n, float acc) {
   float v = acc;
@@ -186,17 +187,12 @@ __device__ __forceinline__ void epi_post4(const GemmEpi& e, int m, int n, float4
   }
 }
 
-enum GemmImpl { GEMM_TCGEN05 = 0, GEMM_SIMT_DEBUG = 1, GEMM_TCGEN05_1CTA = 2 /* tcgen05, never the CTA-pair kernel */ };
+enum GemmImpl { GEMM_TC = 0 /* tensor cores: wgmma, mma.sync for 3xTF32 */, GEMM_SIMT_DEBUG = 1 };
 
-// dtype: TMAP_BF16 (kind::f16, bf16 operands) or TMAP_F32 (kind::tf32, fp32 operands; K-major only).
+// dtype: TMAP_BF16 (bf16 operands) or TMAP_F32 (TF32 products of fp32 operands; K-major only unless x3).
 // lda / ldb: row pitch in elements of the stored matrix ([M,K] / [N,K], or [K,M] / [K,N] for MN-major operands).
 int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dtype, const GemmShape& shape,
                    const GemmEpi& epi, cudaStream_t stream, int impl = -1 /* -1: process default */);
-
-// CTA-pair kernel (gemm2.cu): bf16, K-major operands, no split-K; launch_gemm_tn routes the large GEMMs there
-// (DVT_GEMM_CG2=0 keeps everything on the single-CTA kernels).
-int launch_gemm_cg2(const void* A, int lda, const void* B, int ldb, const GemmShape& s, const GemmEpi& e, cudaStream_t stream);
-bool gemm_cg2_enabled();
 
 int default_gemm_impl();
 int gemm_prepare();

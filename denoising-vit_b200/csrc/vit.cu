@@ -3,7 +3,7 @@
 // (dvt/models/vit_wrapper.py:122-143) for the standard pre-LN ViT family (DINOv2 S/B/L/g, +reg4).
 //
 // Data flow per call (M = B * tokens, C = embed dim), all activations resident in HBM workspaces owned by the
-// handle; the residual stream is fp32, GEMM operands bf16 with fp32 accumulation in TMEM:
+// handle; the residual stream is fp32, GEMM operands bf16 with fp32 accumulation in registers (wgmma):
 //   im2col -> [GEMM patch-embed + bias + pos-embed -> x] -> prefix rows
 //   per block: LN1 -> [GEMM qkv + bias] -> attention -> [GEMM proj + bias, x += ls1 * .] ->
 //              LN2 -> [GEMM fc1 + bias + GELU] -> [GEMM fc2 + bias, x += ls2 * .]
@@ -213,9 +213,9 @@ int vit_forward(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int 
 
   const int Mi = (int)M;
   // Programmatic dependent launch along the block stack is available (DVT_VIT_PDL=1) but OFF by default: these kernels
-  // run for 25-200 us each, so the hidden launch latency is worth < 1 %, and CTAs that are resident early but blocked in
-  // griddepcontrol.wait take SM slots from the fit running beside the forwards (measured: 803.7 vs 784.5 ms / image,
-  // profiles/r1x_validate.txt).  The fit's 10-20 us kernels are where PDL pays (fit.cu).
+  // are long, so the hidden launch latency is worth little, and CTAs that are resident early but blocked in
+  // griddepcontrol.wait take SM slots from the fit running beside the forwards.  The fit's short kernels are where PDL
+  // pays (fit.cu).
   static int vit_pdl = -1;
   if (vit_pdl < 0) {
     const char* pv = getenv("DVT_VIT_PDL");

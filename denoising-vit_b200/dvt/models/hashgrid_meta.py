@@ -42,7 +42,7 @@ class HashGridMeta:
 def make_meta(n_levels: int, base_resolution: int = 16, max_resolution: int = 1024, n_features_per_level: int = 8,
               log2_hashmap_size: int = 20) -> HashGridMeta:
     if n_features_per_level != 8:
-        raise NotImplementedError("the B200 hash grid implements n_features_per_level == 8 (the value DVT uses)")
+        raise NotImplementedError("the H100 hash grid implements n_features_per_level == 8 (the value DVT uses)")
     if not 1 <= n_levels <= 16:
         raise NotImplementedError("n_levels must be in [1, 16]")
     pls64 = float(np.exp((np.log(max_resolution) - np.log(base_resolution)) / (n_levels - 1))) if n_levels > 1 else 1.0

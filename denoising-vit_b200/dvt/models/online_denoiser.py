@@ -1,6 +1,6 @@
 """Drop-in for dvt/models/online_denoiser.py of the reference (SURVEY.md section 8(f-4), denoised-backbone inference):
 same `Denoiser` constructor, parameters and state-dict names (`denoiser.*` with timm `Block` names, `pos_embed`, `vit.*`),
-same `forward` flags and return values (online_denoiser.py:13-104).  The forward runs on the hand-written sm_100a kernels
+same `forward` flags and return values (online_denoiser.py:13-104).  The forward runs on the hand-written sm_90a kernels
 of libdvt_b200.so: the frozen ViT through `PretrainedViTWrapper`, the learnable position embedding (resampled like
 timm's `resample_abs_pos_embed` when the grid differs), then the denoiser block(s) as
 LayerNorm -> QKV GEMM -> flash attention -> out-proj GEMM (+ residual) -> LayerNorm -> fc1 GEMM + GELU -> fc2 GEMM
@@ -8,7 +8,7 @@ LayerNorm -> QKV GEMM -> flash attention -> out-proj GEMM (+ residual) -> LayerN
 
 TRAINING (SURVEY 8(f-2), reference main_denoiser.py:213-220): when gradients are enabled and the denoiser's parameters
 require them, every block runs as ONE autograd node (`dvt.train_ops.block_forward`) whose backward is hand-written too:
-flash-attention backward on tcgen05, LayerNorm / GELU / bias gradients, bf16 data- and weight-gradient GEMMs that read
+flash-attention backward on wgmma, LayerNorm / GELU / bias gradients, bf16 data- and weight-gradient GEMMs that read
 weights and activations in place as MN-major operands.  The position embedding (and its resampling, when the grid
 differs) stays an ordinary torch op in the graph, so `pos_embed.grad` comes out of autograd."""
 from __future__ import annotations

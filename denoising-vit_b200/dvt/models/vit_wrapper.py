@@ -1,6 +1,6 @@
 """Drop-in for dvt/models/vit_wrapper.py of the reference: same `MODEL_LIST`, same `PretrainedViTWrapper`
 constructor, attributes and `get_intermediate_layers` contract (reference vit_wrapper.py:15-146), with the forward
-executed by libdvt_b200.so (hand-written sm_100a kernels) instead of timm.
+executed by libdvt_b200.so (hand-written sm_90a kernels) instead of timm.
 
 `self.model` is a parameter container whose state-dict keys are timm's, so checkpoints of the wrapper
 (`model.<timm key>`, reference make_video_demo.py:31-34) load unchanged.  There is no network in this build:
@@ -299,7 +299,7 @@ class PretrainedViTWrapper(nn.Module):
         self.patch_size = int(re.search(r"patch(\d+)", model_identifier).group(1))
         self.dynamic_img_size = dynamic_img_size
         self.dynamic_img_pad = dynamic_img_pad
-        assert dynamic_img_size and not dynamic_img_pad, "the B200 path implements dynamic_img_size=True, no padding"
+        assert dynamic_img_size and not dynamic_img_pad, "the H100 path implements dynamic_img_size=True, no padding"
         self.model, self.transformation = self.create_model(model_identifier, **kwargs)
         # overwrite the stride size (reference vit_wrapper.py:78-79)
         if stride != self.model.patch_embed.proj.stride[0]:
@@ -322,7 +322,7 @@ class PretrainedViTWrapper(nn.Module):
         if model_identifier not in ARCHS:
             raise NotImplementedError(
                 f"{model_identifier}: architecture outside the plain pre-LN / head_dim-64 ViT family is not "
-                "implemented by the B200 path (see DESIGN.md, out of scope)")
+                "implemented by the H100 path (see DESIGN.md, out of scope)")
         a = dict(ARCHS[model_identifier])
         patch = int(kwargs.pop("patch_size", self.patch_size))
         if "img_size" in kwargs:
@@ -359,7 +359,7 @@ class PretrainedViTWrapper(nn.Module):
         return model, transformation
 
     def extract_into(self, x: torch.Tensor, layer_index: int, out_nhwc: torch.Tensor, norm: bool = True) -> torch.Tensor:
-        """B200-only convenience used by the stage-1 pipeline: writes the [B, h, w, C] map of `layer_index` straight into
+        """library-only convenience used by the stage-1 pipeline: writes the [B, h, w, C] map of `layer_index` straight into
         `out_nhwc` (a slice of the feature bank) instead of returning a fresh tensor."""
         return self.model._run(x, layer_index, norm, all_tokens=False, out=out_nhwc)
 

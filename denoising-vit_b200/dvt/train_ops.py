@@ -1,6 +1,6 @@
 """Stage-2 training operators over torch CUDA tensors (SURVEY.md section 8(f-2)): thin wrappers around the C ABI plus the
 two autograd functions the training step is made of -- the denoiser block (`block_forward`) and the distillation loss
-(`denoise_loss`).  Every kernel behind them is hand-written sm_100a code of libdvt_b200.so; torch only owns the tensors.
+(`denoise_loss`).  Every kernel behind them is hand-written sm_90a code of libdvt_b200.so; torch only owns the tensors.
 
 Reference step (main_denoiser.py:213-220): pred = model(original_feats); loss = mse(pred, denoised) + 1 - mean cosine;
 loss.backward(); AdamW.step() -- through timm `Block` (pre-LN attention + GELU MLP, no LayerScale)."""

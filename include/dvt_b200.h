@@ -1,5 +1,5 @@
 /*
- * dvt_b200 -- C ABI of the B200-native (sm_100a) hot paths of Denoising-ViT (DVT).
+ * dvt_b200 -- C ABI of the H100-native (sm_90a) hot paths of Denoising-ViT (DVT).
  *
  * The reference (Jiawei-Yang/Denoising-ViT) has no FFI layer of its own: its hot paths are reached through the
  * Python API of `dvt.models`, which in turn calls timm (ViT forward), tiny-cuda-nn (hash-grid encoding) and
@@ -43,11 +43,10 @@ int dvt_device_error(unsigned int* code_out);
 /* Number of kernels this library has launched in the calling process (CUDA-graph replays count their nodes). */
 long long dvt_launch_count(void);
 /* Profiling aid: when set (device pointer to 16 x u64, or NULL to disable), dvt_gemm_f32x3 launches record %globaltimer
- * milestones of CTA 0: entry, setup done, first operands landed, MMAs issued, epilogue start, epilogue end, exit. */
+ * milestones of CTA 0: slot 0 at entry, slot 6 at exit. */
 int dvt_debug_set_timestamp_buffer(unsigned long long* dev_buf16);
-/* Process-wide kernel implementation switch for debugging: 0 = tcgen05 tensor-core kernels (default),
- * 1 = plain SIMT reference kernels (same semantics, slow; also settable with DVT_GEMM_IMPL=simt), 2 = tcgen05 without the
- * CTA-pair GEMM (cta_group::2; DVT_GEMM_CG2=0 does the same for a whole process), -1 = back to the default. */
+/* Process-wide kernel implementation switch for debugging: 0 = tensor-core kernels (wgmma / mma.sync; default),
+ * 1 = plain SIMT reference kernels (same semantics, slow; also settable with DVT_GEMM_IMPL=simt), -1 = back to the default. */
 int dvt_set_debug_impl(int impl);
 
 /* ---------------------------------------------------------------------------------------------------------

@@ -1,4 +1,4 @@
-"""DVT stage 2 (training the generalizable denoiser) on B200 -- drop-in for the reference's main_denoiser.py.
+"""DVT stage 2 (training the generalizable denoiser) on H100 -- drop-in for the reference's main_denoiser.py.
 
 Same flags (reference main_denoiser.py:25-78 incl. `--auto_stride` and the 518 -> 512 rule for stride 16 / 8), same model
 (`dvt.models.Denoiser(vit=None, num_blocks)`, :129-135), same objective (MSE + 1 - mean cosine, :214-217), AdamW with
@@ -6,11 +6,11 @@ betas (0.9, 0.999) and weight decay on every parameter (:176-180), sqrt-scaled l
 schedule (:174,181-188), same checkpoint layout `{"denoiser", "optimizer", "step"}` + `latest.pth` symlink (:239-264).
 
 What runs where: forward and backward of the transformer block, the loss with its gradient and the AdamW update are
-hand-written sm_100a kernels (dvt/train_ops.py, dvt/optim.py); data parallelism is ONE NCCL all-reduce of the flat
+hand-written sm_90a kernels (dvt/train_ops.py, dvt/optim.py); data parallelism is ONE NCCL all-reduce of the flat
 gradient buffer per step (the reference wraps the model in DistributedDataParallel, :137-140).  Launch with torchrun
 (RANK / WORLD_SIZE / LOCAL_RANK from the environment), one process per GPU.
 
-B200 extension: `--collated <file.pt>` trains straight from the tensors stage 1 gathered with its all-gather
+H100 extension: `--collated <file.pt>` trains straight from the tensors stage 1 gathered with its all-gather
 (`main_img_denoising.py --collate_out`), held in HBM, instead of re-reading the `.npy` store.
 The PCA visualisation (reference :266-275) is outside the hot path and not produced."""
 import argparse
@@ -71,7 +71,7 @@ def get_args(argv=None):
     parser.add_argument("--dist_url", default="env://")
     parser.add_argument("--distributed", action="store_true")
     parser.add_argument("--device", default="cuda", help="device to use for training / testing")
-    # B200 extensions (not reference flags)
+    # H100 extensions (not reference flags)
     parser.add_argument("--collated", type=str, default=None,
                         help="train from the in-memory stacks written by main_img_denoising.py --collate_out")
     parser.add_argument("--resume", type=str, default=None, help="checkpoint to continue from (e.g. .../latest.pth)")
@@ -113,7 +113,7 @@ def main(args):
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
-    assert torch.cuda.is_available(), "the B200 stage-2 trainer needs a CUDA device (no CPU fallback)"
+    assert torch.cuda.is_available(), "the H100 stage-2 trainer needs a CUDA device (no CPU fallback)"
     torch.cuda.set_device(local)
     device = torch.device("cuda", local)
     if world > 1:

@@ -1,4 +1,4 @@
-"""DVT stage 1 (per-image denoising) on B200 -- drop-in for the reference's main_img_denoising.py.
+"""DVT stage 1 (per-image denoising) on H100 -- drop-in for the reference's main_img_denoising.py.
 
 Same command line (reference main_img_denoising.py:152-217), same outputs
 (`{save_root}/raw_features/{model}/<rel>.npy` (h, w, C) float32 and `{save_root}/denoised_features/{model}/<rel>.npy`
@@ -87,7 +87,7 @@ def get_args(argv=None):
     p.add_argument("--num_vis_samples", type=int, default=5)
     p.add_argument("--vis_freq", type=int, default=100)
     p.add_argument("--seed", type=int, default=0)
-    # B200 extensions (not reference flags)
+    # H100 extensions (not reference flags)
     p.add_argument("--collate_out", type=str, default=None,
                    help="rank 0 saves the all-gathered stacks of raw and denoised maps [N, h, w, C] (+ the image list) here "
                         "(.pt); main_denoiser.py --collated trains from it")
@@ -112,7 +112,7 @@ def main(args):
     misc.fix_random_seeds(args.seed)
     if rank == 0:
         print(f"Arguments:\n{json.dumps(vars(args), indent=4)}")
-    assert torch.cuda.is_available(), "the B200 stage-1 driver needs a CUDA device (no CPU fallback)"
+    assert torch.cuda.is_available(), "the H100 stage-1 driver needs a CUDA device (no CPU fallback)"
     torch.cuda.set_device(local)
     device = torch.device("cuda", local)
     if world > 1:

@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "denoising-vit_b200")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA GPU (H100)")
 
 
 def pytest_collection_modifyitems(config, items):

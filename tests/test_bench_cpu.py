@@ -1,6 +1,5 @@
 """bench.py contract on the CPU: the reference arm (`--impl reference`) prints ONE JSON line with the keys the driver reads,
-the same `config` as the B200 arm, and ranks other than 0 exit without work.  (The B200 arm needs a GPU: it is run by the
-driver and by tools/r2*_gpu.sh; its line is committed under profiles/.)"""
+the same `config` as the H100 arm, and ranks other than 0 exit without work.  (The H100 arm needs a GPU.)"""
 import json
 import os
 import subprocess
@@ -32,8 +31,8 @@ def test_reference_arm_prints_the_contract_line():
     assert d["e2e"]["h2d_bytes_per_step"] == 0 and d["e2e"]["d2h_bytes_per_step"] == 0
     assert abs(d["ms_per_step"] * d["value"] - 1000.0) < 1e-6
 
-    # the config both arms print is one function of the flags: the committed B200 line carries the same dict
-    with open(os.path.join(ROOT, "profiles", "r2z11_bench.json")) as fh:
+    # the config both arms print is one function of the flags: the GPU arm's line (tests/golden) carries the same dict
+    with open(os.path.join(ROOT, "tests", "golden", "bench_gpu_line.json")) as fh:
         ours = json.load(fh)
     same = {k: v for k, v in ours["config"].items() if k != "images_per_gpu"}
     assert same == {k: v for k, v in d["config"].items() if k != "images_per_gpu"}

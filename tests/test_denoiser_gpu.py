@@ -86,7 +86,7 @@ def test_denoised_backbone_at_stride4_with_center_padding():
     """What SURVEY.md row f-4 is for: a video-sized frame (480 x 850) centre-padded to patch multiples (490 x 854), the
     frozen ViT at stride 4 -> 120 x 211 = 25 320 patch tokens, the learnable 37 x 37 position embedding resampled to that
     grid, one denoiser block over the 25 320-token sequence.  Checker: the oracle (ViT + Denoiser restatement) evaluated in
-    fp32 on the same GPU (its explicit attention matrix needs ~30 GB: fine on a B200, not on a CPU box)."""
+    fp32 on the same GPU (its explicit attention matrix needs ~30 GB: fine on a H100, not on a CPU box)."""
     import dvt.models as DVT
     from dvt import _lib
     from oracle import denoiser as OD

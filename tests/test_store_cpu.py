@@ -78,44 +78,33 @@ def test_feature_store_writer_writes_the_reference_store(tmp_path):
 
 
 def test_store_reads_back_through_the_reference_dataset(tmp_path):
-    """The store written here, read by the REFERENCE's stage-2 dataset (dvt/dataset/paired_list_dataset.py:27-43,
-    imported unmodified).  Runs in the build container only (needs /root/reference)."""
-    import importlib.util
-    import pytest
-    ref_file = "/root/reference/dvt/dataset/paired_list_dataset.py"
-    if not os.path.isfile(ref_file):
-        pytest.skip("reference checkout not present on this machine")
-    from PIL import Image
+    """The store written here, read the way the REFERENCE's stage-2 dataset reads it (dvt/dataset/paired_list_dataset.py:27-43):
+    tests/golden/store_reference_reads.json records, per list entry, the files that dataset opens relative to the store's
+    root (denoised first, then raw) and the shapes it returns after np.load(...).squeeze()."""
+    import json
     from dvt.store import FeatureStoreWriter
     from dvt.utils import misc
-    spec = importlib.util.spec_from_file_location("ref_paired", ref_file)
-    ref = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(ref)
-    h, w, C = 3, 4, 16
+    with open(os.path.join(ROOT, "tests", "golden", "store_reference_reads.json")) as f:
+        gold = json.load(f)
+    h, w, C = gold["feature_shape"]
     data_root = str(tmp_path / "data") + "/"
-    model = "vit_small_patch14_dinov2.lvd142m"
-    args = Namespace(data_root=data_root, save_root=str(tmp_path / "feats"), model=model)
-    rels = ["a/one.jpg", "b/two.png"]
+    args = Namespace(data_root=data_root, save_root=str(tmp_path / "feats"), model=gold["model"])
+    rels = [it["entry"] for it in gold["items"]]
+    assert len(rels) == gold["length"] == 2
     wr = FeatureStoreWriter()
     maps = {}
     for k, rel in enumerate(rels):
-        os.makedirs(os.path.dirname(os.path.join(data_root, rel)), exist_ok=True)
-        Image.fromarray(np.full((8, 8, 3), 40 * k, np.uint8)).save(os.path.join(data_root, rel))
         g = torch.Generator().manual_seed(k)
         maps[rel] = (torch.randn(h, w, C, generator=g), torch.randn(1, h, w, C, generator=g))
         wr.submit(*misc.feature_paths(args, os.path.join(data_root, rel)), *maps[rel])
     wr.close()
-    lst = tmp_path / "list.txt"
-    lst.write_text("".join(f"{r} 0\n" for r in rels))
-    ds = ref.PairedListDataset(data_root=data_root, data_list=str(lst),
-                               feat_root=f"{args.save_root}/denoised_features/{model}/", transform=lambda im: im.size)
-    assert len(ds) == 2
-    for k, rel in enumerate(rels):
-        item = ds[k]
-        assert item["image"] == (8, 8)
-        assert item["original_feats"].shape == (h, w, C) and item["denoised_feats"].shape == (h, w, C)
-        assert np.array_equal(item["original_feats"], maps[rel][0].numpy())
-        assert np.array_equal(item["denoised_feats"], maps[rel][1][0].numpy())
+    for it in gold["items"]:
+        den_rel, raw_rel = it["opened"]
+        denoised = np.load(os.path.join(args.save_root, den_rel)).squeeze()
+        original = np.load(os.path.join(args.save_root, raw_rel)).squeeze()
+        assert list(original.shape) == it["original_shape"] and list(denoised.shape) == it["denoised_shape"]
+        assert np.array_equal(original, maps[it["entry"]][0].numpy())
+        assert np.array_equal(denoised, maps[it["entry"]][1][0].numpy())
 
 
 def test_sampling_stream_is_the_references_rng_stream():

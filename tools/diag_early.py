@@ -31,8 +31,8 @@ if __name__ == "__main__":
                  weight_decay=cfg["weight_decay"], warmup_iters=cfg["warmup_iters"], freeze_after=cfg["freeze_after"],
                  loss_scale=cfg["loss_scale"], log_every=1)
     prev = {}
-    for tag, impl, env in (("tcgen05 3xTF32, sequential", 0, {"DVT_FIT_PIPELINE": "0"}), ("tcgen05 3xTF32, sequential (again)", 0, {"DVT_FIT_PIPELINE": "0"}),
-                           ("SIMT fp32, sequential", 1, {"DVT_FIT_PIPELINE": "0"}), ("tcgen05 3xTF32, pipelined", 0, {})):
+    for tag, impl, env in (("tensor-core 3xTF32, sequential", 0, {"DVT_FIT_PIPELINE": "0"}), ("tensor-core 3xTF32, sequential (again)", 0, {"DVT_FIT_PIPELINE": "0"}),
+                           ("SIMT fp32, sequential", 1, {"DVT_FIT_PIPELINE": "0"}), ("tensor-core 3xTF32, pipelined", 0, {})):
         os.environ.pop("DVT_FIT_PIPELINE", None)
         os.environ.update(env)
         feats, coords, init, idx, den, field, _ = T._setup(cfg)

@@ -56,4 +56,4 @@ if __name__ == "__main__":
     print(f"run-to-run min cos {cs(a, b):.6f}; pipelined vs sequential {cs(a, c):.6f}; graphs vs none {cs(c, d):.6f}")
     if len(sys.argv) > 1 and sys.argv[1] == "simt":
         f, lf = run("sequential, SIMT fp32 GEMMs", {"DVT_FIT_PIPELINE": "0"}, impl=1, graph_steps=0)
-        print(f"simt vs tcgen05 sequential {cs(f, c):.6f}")
+        print(f"simt vs tensor-core sequential {cs(f, c):.6f}")

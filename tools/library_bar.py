@@ -1,5 +1,5 @@
 """GPU "library bar" (BASELINE.md section 4.5, SURVEY.md 8(d)): what the reference's own op sequence costs on the SAME
-B200 when every op goes to the vendor libraries -- the number the fused kernels of this repository have to beat.
+H100 when every op goes to the vendor libraries -- the number the fused kernels of this repository have to beat.
 
   * HP-1: a ViT-B/14 forward as the reference reaches it through timm (vit_wrapper.py:136-143): Conv2d patch embedding,
     per block LayerNorm -> Linear(qkv) -> F.scaled_dot_product_attention -> Linear(proj) -> LayerScale + residual ->

@@ -1,7 +1,6 @@
 #!/usr/bin/env python
 """Per-kernel timings at the headline shapes (ViT-B/14, 518^2, batch B views; fit with C=768, 2048 pixels, 16 levels).
-CUDA events around back-to-back launches after warm-up, L2 flushed between timed launches unless --no-flush.
-Also the target of the ncu captures committed under profiles/ (--only NAME --iters 3)."""
+CUDA events around back-to-back launches after warm-up, L2 flushed between timed launches unless --no-flush."""
 import argparse
 import os
 import sys

@@ -52,6 +52,15 @@ int launch_denoise_loss(const float* pred, const float* tgt, float* dpred, float
                         cudaStream_t st);
 int launch_adamw(float* p, const float* g, float* m, float* v, size_t n, double lr, double beta1, double beta2, double eps,
                  double weight_decay, long long step, cudaStream_t st);
+int launch_layerscale_bwd(const float* dx, int ldx, const __nv_bfloat16* branch, const float* gamma, __nv_bfloat16* dbranch,
+                          float* dbias, float* dgamma, float* workspace, int rows, int C, cudaStream_t st);
+int launch_vit_embed_bwd(const float* dx0, int B, int ntok, int prefix, int C, __nv_bfloat16* dpatch, float* dpos,
+                         float* dprefix, float* dbias, float* workspace, cudaStream_t st);
+int launch_layernorm_bwd_grouped(const float* x, const float* gamma, const float* dy, float* dx_accum, float* dgamma,
+                                 float* dbeta, float* workspace, int rows, int C, float eps, int in_group, int skip,
+                                 cudaStream_t st);
+int launch_vit_embed_fwd(const __nv_bfloat16* patches, int Kp, const __nv_bfloat16* w, const float* bias, const float* pos_patch,
+                         const float* prefix_rows, int B, int np, int prefix, int C, float* out, cudaStream_t st, int impl);
 const char* last_error();
 extern int g_debug_impl_override;
 int g_debug_impl_override = -1;
@@ -123,6 +132,26 @@ int dvt_gemm_tn_residual(const void* A, int lda, const void* B, int ldb, int dty
                         reinterpret_cast<cudaStream_t>(stream), eff_impl());
 }
 
+int dvt_gemm_tn_residual_ex(const void* A, int lda, const void* B, int ldb, int dtype, int M, int N, int K,
+                            const float* bias, const float* gamma, float* x_inout, int ldx, void* branch_out_bf16,
+                            int ld_branch, void* stream) {
+  DVT_REQUIRE(dtype == DVT_DTYPE_BF16 || dtype == DVT_DTYPE_F32, "dvt_gemm_tn_residual_ex: bad dtype %d", dtype);
+  DVT_REQUIRE(A && B && x_inout, "dvt_gemm_tn_residual_ex: null pointer");
+  DVT_REQUIRE(!branch_out_bf16 || (ld_branch >= N && ld_branch % 4 == 0),
+              "dvt_gemm_tn_residual_ex: ld_branch=%d must be >= N=%d and a multiple of 4", ld_branch, N);
+  GemmEpi e;
+  e.bias = bias;
+  e.gamma = gamma;
+  e.out = x_inout;
+  e.ldo = ldx;
+  e.out_mode = OUT_F32_RESID;
+  e.branch = reinterpret_cast<__nv_bfloat16*>(branch_out_bf16);
+  e.ld_branch = ld_branch;
+  GemmShape s{M, N, K, 1};
+  return launch_gemm_tn(A, lda, B, ldb, dtype == DVT_DTYPE_BF16 ? TMAP_BF16 : TMAP_F32, s, e,
+                        reinterpret_cast<cudaStream_t>(stream), eff_impl());
+}
+
 int dvt_layernorm(const float* x, int ldx, const float* gamma, const float* beta, void* y, int ldy, int y_dtype,
                   int rows, int C, float eps, int in_group, int skip, void* stream) {
   DVT_REQUIRE(x && gamma && beta && y, "dvt_layernorm: null pointer");
@@ -183,6 +212,29 @@ int dvt_gemm_bf16_bwd(const void* A, int lda, int a_mn, const void* B, int ldb, 
   s.a_mn = a_mn;
   s.b_mn = b_mn;
   return launch_gemm_tn(A, lda, B, ldb, TMAP_BF16, s, e, reinterpret_cast<cudaStream_t>(stream), eff_impl());
+}
+/* ---- stage-3 (distillation) operators ---- */
+int dvt_layerscale_bwd(const float* dx, int ldx, const void* branch_bf16, const float* gamma, void* dbranch_bf16, float* dbias,
+                       float* dgamma, float* workspace, int rows, int C, void* stream) {
+  return launch_layerscale_bwd(dx, ldx, reinterpret_cast<const __nv_bfloat16*>(branch_bf16), gamma,
+                               reinterpret_cast<__nv_bfloat16*>(dbranch_bf16), dbias, dgamma, workspace, rows, C,
+                               reinterpret_cast<cudaStream_t>(stream));
+}
+int dvt_vit_embed_fwd(const void* patches_bf16, int Kp, const void* w_bf16, const float* bias, const float* pos_patch,
+                      const float* prefix_rows, int B, int np, int prefix, int C, float* out, void* stream) {
+  return launch_vit_embed_fwd(reinterpret_cast<const __nv_bfloat16*>(patches_bf16), Kp,
+                              reinterpret_cast<const __nv_bfloat16*>(w_bf16), bias, pos_patch, prefix_rows, B, np, prefix, C,
+                              out, reinterpret_cast<cudaStream_t>(stream), eff_impl());
+}
+int dvt_vit_embed_bwd(const float* dx0, int B, int ntok, int prefix, int C, void* dpatch_bf16, float* dpos, float* dprefix,
+                      float* dbias, float* workspace, void* stream) {
+  return launch_vit_embed_bwd(dx0, B, ntok, prefix, C, reinterpret_cast<__nv_bfloat16*>(dpatch_bf16), dpos, dprefix, dbias,
+                              workspace, reinterpret_cast<cudaStream_t>(stream));
+}
+int dvt_layernorm_bwd_grouped(const float* x, const float* gamma, const float* dy, float* dx_accum, float* dgamma, float* dbeta,
+                              float* workspace, int rows, int C, float eps, int in_group, int skip, void* stream) {
+  return launch_layernorm_bwd_grouped(x, gamma, dy, dx_accum, dgamma, dbeta, workspace, rows, C, eps, in_group, skip,
+                                      reinterpret_cast<cudaStream_t>(stream));
 }
 int dvt_denoise_loss(const float* pred, const float* target, float* dpred, float* losses3, int rows, int C, float grad_scale,
                      void* stream) {

@@ -151,7 +151,14 @@ __device__ __forceinline__ void epi_chunk(const GemmEpi& e, const GemmShape& s, 
                                  make_float2(xin[jj].x, xin[jj].y));
         const float2 o23 = ffma2(make_float2(g4.z, g4.w), fadd2(make_float2(x.z, x.w), make_float2(b4.z, b4.w)),
                                  make_float2(xin[jj].z, xin[jj].w));
-        if (m < s.M) *reinterpret_cast<float4*>(outp + (size_t)m * e.ldo + n) = make_float4(o01.x, o01.y, o23.x, o23.y);
+        if (m < s.M) {
+          *reinterpret_cast<float4*>(outp + (size_t)m * e.ldo + n) = make_float4(o01.x, o01.y, o23.x, o23.y);
+          if (e.branch) {
+            const float2 v01 = fadd2(make_float2(x.x, x.y), make_float2(b4.x, b4.y));
+            const float2 v23 = fadd2(make_float2(x.z, x.w), make_float2(b4.z, b4.w));
+            store_branch4(e, m, n, make_float4(v01.x, v01.y, v23.x, v23.y));
+          }
+        }
       }
     } else {
       // ---- generic path (fit epilogues: masks, split planes, atomics, remap) ----
@@ -188,6 +195,7 @@ __device__ __forceinline__ void epi_chunk(const GemmEpi& e, const GemmShape& s, 
         float4 o = xin[jj];
         o.x = fmaf(g4.x, x.x, o.x); o.y = fmaf(g4.y, x.y, o.y); o.z = fmaf(g4.z, x.z, o.z); o.w = fmaf(g4.w, x.w, o.w);
         *reinterpret_cast<float4*>(reinterpret_cast<float*>(e.out) + (size_t)m * e.ldo + n) = o;
+        if (e.branch) store_branch4(e, m, n, x);
       } else {
         epi_post4<FIT>(e, m, n, x);
       }

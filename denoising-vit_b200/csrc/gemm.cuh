@@ -38,6 +38,8 @@ struct GemmEpi {
   float* last_col_out = nullptr;      // OUT_F32_ATOMIC only: column N-1 is accumulated into last_col_out[m] instead
                                       // (bias gradient through a ones column in the B operand)
   const float* gamma = nullptr;       // LayerScale (OUT_F32_RESID)
+  __nv_bfloat16* branch = nullptr;    // OUT_F32_RESID only, optional [M, ld_branch]: the pre-LayerScale value v (bf16), kept
+  int ld_branch = 0;                  // for the LayerScale gradient (training forward of the ViT)
   const float* addend = nullptr;      // [rows_per_group, N] (OUT_F32_REMAP)
   int rows_per_group = 0;             // patches per image
   int group_stride = 0;               // tokens per image
@@ -88,6 +90,14 @@ __device__ __forceinline__ size_t epi_out_row(const GemmEpi& e, int m) {
   return (size_t)m;
 }
 
+// bf16 copy of 4 consecutive pre-LayerScale values (OUT_F32_RESID with a branch buffer)
+__device__ __forceinline__ void store_branch4(const GemmEpi& e, int m, int n, float4 v) {
+  uint2 p;
+  p.x = pack_bf16x2(v.x, v.y);
+  p.y = pack_bf16x2(v.z, v.w);
+  *reinterpret_cast<uint2*>(e.branch + (size_t)m * e.ld_branch + n) = p;
+}
+
 // scalar post-stage (SIMT debug path and ragged tails)
 template <bool FIT = false>
 __device__ __forceinline__ void epi_post1(const GemmEpi& e, int m, int n, float v) {
@@ -110,6 +120,7 @@ __device__ __forceinline__ void epi_post1(const GemmEpi& e, int m, int n, float 
       float* o = reinterpret_cast<float*>(e.out) + row * e.ldo + n;
       float g = e.gamma ? __ldg(e.gamma + n) : 1.0f;
       *o = fmaf(g, v, *o);
+      if (e.branch) e.branch[(size_t)m * e.ld_branch + n] = __float2bfloat16_rn(v);
     } break;
     case OUT_F32_REMAP: {
       int p = m % e.rows_per_group;
@@ -167,6 +178,7 @@ __device__ __forceinline__ void epi_post4(const GemmEpi& e, int m, int n, float4
       x.z = fmaf(g.z, v.z, x.z);
       x.w = fmaf(g.w, v.w, x.w);
       *o = x;
+      if (e.branch) store_branch4(e, m, n, v);
     } break;
     case OUT_F32_REMAP: {
       int p = m % e.rows_per_group;

@@ -29,6 +29,16 @@ SIGNATURES = {
                             c_int, c_int, c_int, c_void_p]),
     "dvt_gemm_tn_residual": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                      c_void_p, c_int, c_void_p]),
+    "dvt_gemm_tn_residual_ex": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                        c_void_p, c_int, c_void_p, c_int, c_void_p]),
+    "dvt_layerscale_bwd": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                   c_void_p]),
+    "dvt_vit_embed_fwd": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
+                                  c_void_p]),
+    "dvt_vit_embed_bwd": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                  c_void_p]),
+    "dvt_layernorm_bwd_grouped": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                          c_float, c_int, c_int, c_void_p]),
     "dvt_layernorm": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_int,
                               c_int, c_void_p]),
     "dvt_attention_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),

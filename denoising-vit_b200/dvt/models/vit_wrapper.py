@@ -2,6 +2,11 @@
 constructor, attributes and `get_intermediate_layers` contract (reference vit_wrapper.py:15-146), with the forward
 executed by libdvt_b200.so (hand-written sm_90a kernels) instead of timm.
 
+Training (stage 3, reference main_distillation.py): after `set_trainable()`, calls made with gradients enabled return a
+differentiable result whose backward is hand-written CUDA too (dvt.train_ops: patch embedding, pre-LN blocks with
+LayerScale, final norm with the prefix strip); `set_grad_checkpointing(True)` makes every block recompute its forward in
+the backward instead of keeping its activations.  Without `set_trainable()` every call is the inference forward.
+
 `self.model` is a parameter container whose state-dict keys are timm's, so checkpoints of the wrapper
 (`model.<timm key>`, reference make_video_demo.py:31-34) load unchanged.  There is no network in this build:
 `pretrained=True` weights are read from `$DVT_WEIGHTS_DIR/<model_identifier>.pth` when present, otherwise the
@@ -20,7 +25,7 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
-from .. import _lib
+from .. import _lib, train_ops
 from .._lib import check, cur_stream, lib, ptr
 
 logger = logging.getLogger(__name__)
@@ -153,6 +158,9 @@ class B200VisionTransformer(nn.Module):
         self._handle: Optional[c_void_p] = None
         self._dirty = True
         self._pos_cache = {}
+        self._param_sig = None
+        self._trainable = False
+        self._grad_ckpt = False
 
     def _init_weights(self):
         nn.init.normal_(self.cls_token, std=1e-6)
@@ -163,8 +171,9 @@ class B200VisionTransformer(nn.Module):
                 nn.init.trunc_normal_(m.weight, std=0.02)
                 nn.init.zeros_(m.bias)
 
-    def set_grad_checkpointing(self, enable: bool = True):  # API parity with timm; inference-only path
-        return None
+    def set_grad_checkpointing(self, enable: bool = True):
+        """timm API: the blocks of the training path keep only their input and recompute the rest in the backward."""
+        self._grad_ckpt = bool(enable)
 
     # ---- weight plumbing ------------------------------------------------------------------------------
     def _apply(self, fn, *a, **k):
@@ -184,6 +193,12 @@ class B200VisionTransformer(nn.Module):
 
     def _sync(self):
         a = self.arch
+        # parameters changed in place (an optimiser step; FusedAdamW also re-points them into its flat buffer): the
+        # handle's bf16 copies and the cached position tables are stale
+        sig = tuple((p._version, p.data_ptr()) for p in self.parameters())
+        if sig != self._param_sig:
+            self._dirty = True
+            self._pos_cache = {}
         if self._handle is None:
             h = c_void_p()
             check(lib().dvt_vit_create(byref(h), a["embed"], a["depth"], a["heads"], self.patch_embed.patch_size[0],
@@ -199,6 +214,7 @@ class B200VisionTransformer(nn.Module):
             t = v.detach().to(dtype=torch.float32).contiguous()
             check(lib().dvt_vit_load(self._handle, k.encode(), ptr(t), t.numel()), f"dvt_vit_load({k})")
         self._dirty = False
+        self._param_sig = sig
 
     def __del__(self):
         try:
@@ -231,6 +247,52 @@ class B200VisionTransformer(nn.Module):
                 self._pos_cache[key] = (grid[0].contiguous(), torch.cat(rows, 0).contiguous())
         return self._pos_cache[key]
 
+    def _pos_tables_train(self, h: int, w: int) -> Tuple[torch.Tensor, torch.Tensor]:
+        """`_pos_tables` inside the autograd graph: gradients reach pos_embed, cls_token and reg_token."""
+        pos = self.pos_embed.float()
+        npre = 0 if self.no_embed_class else 1
+        pre, grid = pos[:, :npre], pos[:, npre:]
+        gh, gw = self.native_grid
+        if (h, w) != (gh, gw):
+            C = grid.shape[-1]
+            g = grid.reshape(1, gh, gw, C).permute(0, 3, 1, 2)
+            g = F.interpolate(g, size=(h, w), mode="bicubic", antialias=True)
+            grid = g.permute(0, 2, 3, 1).reshape(1, h * w, C)
+        cls = self.cls_token.float()[0]
+        if not self.no_embed_class:
+            cls = cls + pre[0]
+        rows = [cls]
+        if self.num_reg_tokens:
+            rows.append(self.reg_token.float()[0])
+        return grid[0], torch.cat(rows, 0)
+
+    def _training(self) -> bool:
+        return self._trainable and torch.is_grad_enabled()
+
+    def _run_train(self, x: torch.Tensor, layer_index: int, norm: bool) -> torch.Tensor:
+        """Differentiable forward to the [B, h, w, C] map of `layer_index` (prefix tokens stripped)."""
+        if self.arch["swiglu"]:
+            raise NotImplementedError(f"{self.identifier}: the training path has no SwiGLU backward (ViT-g)")
+        if not x.is_cuda:
+            raise _lib.DvtError("dvt_b200 ViT training needs a CUDA tensor (no CPU fallback)")
+        if x.dtype not in (torch.float32, torch.bfloat16):
+            x = x.float()
+        x = x.contiguous()
+        B, _, H, W = x.shape
+        P = self.patch_embed.patch_size[0]
+        stride = int(self.patch_embed.proj.stride[0])
+        h, w = (H - P) // stride + 1, (W - P) // stride + 1
+        prefix, ntok, C = self.num_prefix_tokens, self.num_prefix_tokens + h * w, self.embed_dim
+        pos_patch, prefix_rows = self._pos_tables_train(h, w)
+        t = train_ops.vit_embed(x, self.patch_embed.proj.weight, self.patch_embed.proj.bias, pos_patch, prefix_rows, stride)
+        for i in range(layer_index + 1):
+            t = train_ops.vit_block_forward(t, self.blocks[i], self.arch["heads"], B, checkpoint=self._grad_ckpt)
+        if norm:
+            y = train_ops.vit_norm_strip(t, self.norm.weight, self.norm.bias, ntok, prefix)
+        else:
+            y = t.view(B, ntok, C)[:, prefix:]
+        return y.reshape(B, h, w, C)
+
     # ---- forward --------------------------------------------------------------------------------------
     def _run(self, x: torch.Tensor, layer_index: int, norm: bool, all_tokens: bool,
              out: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -256,7 +318,6 @@ class B200VisionTransformer(nn.Module):
                                     int(all_tokens), cur_stream()), "dvt_vit_forward")
         return out
 
-    @torch.no_grad()
     def forward_intermediates(self, x, indices=None, return_prefix_tokens=False, norm=False, stop_early=False,
                               output_fmt="NCHW", intermediates_only=False):
         assert output_fmt in ("NCHW", "NLC")
@@ -268,6 +329,16 @@ class B200VisionTransformer(nn.Module):
             take = list(range(depth - indices, depth))
         else:
             take = [i if i >= 0 else depth + i for i in indices]
+        if self._training():
+            # what distillation asks for (reference main_distillation.py:236): one layer, patch tokens only
+            if len(take) != 1 or return_prefix_tokens:
+                raise NotImplementedError("the ViT training path returns one layer without prefix tokens")
+            t = self._run_train(x, take[0], norm)  # [B, h, w, C]
+            return [t.permute(0, 3, 1, 2) if output_fmt == "NCHW" else t.reshape(t.shape[0], -1, t.shape[-1])]
+        with torch.no_grad():
+            return self._forward_intermediates_infer(x, take, return_prefix_tokens, norm, output_fmt)
+
+    def _forward_intermediates_infer(self, x, take, return_prefix_tokens, norm, output_fmt):
         outs = []
         for idx in take:  # one pass per requested layer (DVT asks for a single layer)
             if return_prefix_tokens:
@@ -357,6 +428,13 @@ class PretrainedViTWrapper(nn.Module):
             transforms.Normalize(mean=a["mean"], std=a["std"]),
         ])
         return model, transformation
+
+    def set_trainable(self, flag: bool = True):
+        """Opt in to the training path (stage-3 distillation): with gradients enabled, `get_intermediate_layers` returns a
+        differentiable result (one layer, no prefix tokens; not for the SwiGLU ViT-g backbones).  Off by default: the
+        frozen-backbone callers keep the inference forward even when their parameters require grad."""
+        self.model._trainable = bool(flag)
+        return self
 
     def extract_into(self, x: torch.Tensor, layer_index: int, out_nhwc: torch.Tensor, norm: bool = True) -> torch.Tensor:
         """library-only convenience used by the stage-1 pipeline: writes the [B, h, w, C] map of `layer_index` straight into

@@ -64,6 +64,9 @@ class FusedAdamW:
         self.step_count += 1
         train_ops.adamw_(self.flat_p, self.flat_g, self.exp_avg, self.exp_avg_sq, lr=g["lr"], betas=g["betas"], eps=g["eps"],
                          weight_decay=g["weight_decay"], step=self.step_count)
+        # the kernel writes the flat buffer behind autograd's back: bump the parameters' version counters so that caches keyed
+        # on them (the bf16 weight copies of dvt.models) see the update
+        torch.autograd.graph.increment_version(self.params)
 
     def state_dict(self) -> Dict:
         state = {}

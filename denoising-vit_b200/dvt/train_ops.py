@@ -207,3 +207,231 @@ class _LossFn(torch.autograd.Function):
 def denoise_loss(pred: torch.Tensor, target: torch.Tensor):
     """(loss, l2_loss, cosine_similarity_loss) of main_denoiser.py:214-217 in one kernel; differentiable w.r.t. pred."""
     return _LossFn.apply(pred, target)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# stage 3 (distillation, reference main_distillation.py): the whole ViT backbone as autograd nodes -- token assembly,
+# pre-LN blocks with optional LayerScale, final LayerNorm with the prefix strip
+# ---------------------------------------------------------------------------------------------------------------------
+_WS_ROWS = 256     # workspace rows (of C floats) of the fixed-order column sums (include/dvt_b200.h, stage 3)
+
+
+def _workspace(C: int, device) -> torch.Tensor:
+    return torch.empty(_WS_ROWS * C, device=device, dtype=torch.float32)
+
+
+def gemm_tn_residual_ex_(x: torch.Tensor, a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None,
+                         gamma: torch.Tensor | None, branch: torch.Tensor | None) -> torch.Tensor:
+    """x += gamma * (a @ w.T + bias) in place (fp32 x); when `branch` (bf16 [M, N]) is given, it receives a @ w.T + bias."""
+    assert x.is_cuda and x.dtype == torch.float32 and x.stride(1) == 1
+    M, K = a.shape
+    N = w.shape[0]
+    if branch is not None:
+        assert branch.dtype == torch.bfloat16 and branch.shape == (M, N) and branch.is_contiguous()
+    check(lib().dvt_gemm_tn_residual_ex(ptr(a), a.stride(0), ptr(w), w.stride(0), _dt(a), M, N, K, ptr(bias), ptr(gamma), ptr(x),
+                                        x.stride(0), ptr(branch), N, cur_stream()), "dvt_gemm_tn_residual_ex")
+    return x
+
+
+def layerscale_bwd(dx: torch.Tensor, branch: torch.Tensor | None, gamma: torch.Tensor | None, want_dbranch: bool = True):
+    """Backward of x += gamma * branch: (dbranch bf16 = gamma * dx, dbias = sum_rows gamma * dx, dgamma = sum_rows dx *
+    branch or None).  gamma None: no LayerScale (cast + column sum).  Fixed-order sums: bit-identical across calls."""
+    assert dx.is_cuda and dx.dtype == torch.float32 and dx.dim() == 2 and dx.stride(1) == 1
+    rows, C = dx.shape
+    dbranch = torch.empty((rows, C), device=dx.device, dtype=torch.bfloat16) if want_dbranch else None
+    dbias = torch.empty(C, device=dx.device, dtype=torch.float32)
+    dgamma = None
+    if gamma is not None:
+        gamma = gamma.detach().float().contiguous()
+        if branch is not None:
+            assert branch.dtype == torch.bfloat16 and branch.shape == (rows, C) and branch.is_contiguous()
+            dgamma = torch.empty(C, device=dx.device, dtype=torch.float32)
+    check(lib().dvt_layerscale_bwd(ptr(dx), dx.stride(0), ptr(branch if dgamma is not None else None), ptr(gamma), ptr(dbranch),
+                                   ptr(dbias), ptr(dgamma), ptr(_workspace(C, dx.device)), rows, C, cur_stream()),
+          "dvt_layerscale_bwd")
+    return dbranch, dbias, dgamma
+
+
+def vit_embed_bwd(dx0: torch.Tensor, batch: int, prefix: int):
+    """dx0 f32 [batch * ntok, C] -> (dpatch bf16 [batch * np, C], dpos f32 [np, C], dprefix f32 [prefix, C], dbias f32 [C])."""
+    assert dx0.is_cuda and dx0.dtype == torch.float32 and dx0.is_contiguous()
+    M, C = dx0.shape
+    ntok = M // batch
+    np_ = ntok - prefix
+    dev = dx0.device
+    dpatch = torch.empty((batch * np_, C), device=dev, dtype=torch.bfloat16)
+    dpos = torch.empty((np_, C), device=dev, dtype=torch.float32)
+    dprefix = torch.empty((prefix, C), device=dev, dtype=torch.float32)
+    dbias = torch.empty(C, device=dev, dtype=torch.float32)
+    check(lib().dvt_vit_embed_bwd(ptr(dx0), batch, ntok, prefix, C, ptr(dpatch), ptr(dpos), ptr(dprefix), ptr(dbias),
+                                  ptr(_workspace(C, dev)), cur_stream()), "dvt_vit_embed_bwd")
+    return dpatch, dpos, dprefix, dbias
+
+
+def layernorm_bwd_grouped_(dx_accum: torch.Tensor, x: torch.Tensor, gamma: torch.Tensor, dy: torch.Tensor, in_group: int,
+                           skip: int, eps: float = 1e-6):
+    """Backward of ops.layernorm(x, ..., in_group, skip): dy holds the compacted rows; dx_accum += dLN/dx on the kept rows
+    of the full [rows, C] tensor; returns (dgamma, dbeta) (fixed-order sums)."""
+    rows, C = x.shape
+    assert all(t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() for t in (dx_accum, x, dy))
+    assert dx_accum.shape == x.shape and dy.shape == (rows // in_group * (in_group - skip), C)
+    g = gamma.detach().float().contiguous()
+    dgamma = torch.empty(C, device=x.device, dtype=torch.float32)
+    dbeta = torch.empty(C, device=x.device, dtype=torch.float32)
+    check(lib().dvt_layernorm_bwd_grouped(ptr(x), ptr(g), ptr(dy), ptr(dx_accum), ptr(dgamma), ptr(dbeta),
+                                          ptr(_workspace(C, x.device)), rows, C, eps, in_group, skip, cur_stream()),
+          "dvt_layernorm_bwd_grouped")
+    return dgamma, dbeta
+
+
+class _VitEmbedFn(torch.autograd.Function):
+    """Patch embedding (im2col -> GEMM + bias + position) and the prefix rows, as in dvt_vit_forward.  The image gets no
+    gradient; pos_patch [np, C] and prefix_rows [prefix, C] are tensors of the caller's graph (built from pos_embed /
+    cls_token / reg_token), so autograd carries their gradients on to the parameters."""
+
+    @staticmethod
+    def forward(ctx, img, pe_w, pe_b, pos_patch, prefix_rows, stride: int):
+        if not img.is_cuda:
+            raise _lib.DvtError("dvt_b200 ViT training needs CUDA tensors (no CPU fallback)")
+        C, _, P, _ = pe_w.shape
+        K = 3 * P * P
+        Kp = (K + 7) // 8 * 8
+        B, _, H, W = img.shape
+        h, w = (H - P) // stride + 1, (W - P) // stride + 1
+        np_, prefix = h * w, prefix_rows.shape[0]
+        patches = ops.im2col(img.detach().contiguous(), P, stride)
+        wpad = torch.nn.functional.pad(pe_w.detach().float().reshape(C, K), (0, Kp - K)).to(torch.bfloat16).contiguous()
+        out = torch.empty((B * (np_ + prefix), C), device=img.device, dtype=torch.float32)
+        pp = pos_patch.detach().float().contiguous()
+        pr = prefix_rows.detach().float().contiguous()
+        check(lib().dvt_vit_embed_fwd(ptr(patches), Kp, ptr(wpad), ptr(pe_b.detach().float().contiguous()), ptr(pp), ptr(pr), B,
+                                      np_, prefix, C, ptr(out), cur_stream()), "dvt_vit_embed_fwd")
+        ctx.save_for_backward(patches)
+        ctx.meta = (B, prefix, C, P, K)
+        return out
+
+    @staticmethod
+    def backward(ctx, dx0):
+        (patches,) = ctx.saved_tensors
+        B, prefix, C, P, K = ctx.meta
+        dpatch, dpos, dprefix, dbias = vit_embed_bwd(dx0.detach().float().contiguous(), B, prefix)
+        gw = wgrad(dpatch, patches)[:, :K].reshape(C, 3, P, P)
+        return None, gw, dbias, dpos, dprefix, None
+
+
+def vit_embed(img: torch.Tensor, patch_embed_w, patch_embed_b, pos_patch, prefix_rows, stride: int) -> torch.Tensor:
+    """Token rows f32 [B * (prefix + h*w), C] of images [B, 3, H, W] (f32 or bf16)."""
+    return _VitEmbedFn.apply(img, patch_embed_w, patch_embed_b, pos_patch, prefix_rows, stride)
+
+
+def _vit_block_fwd(x0, wts, heads: int, batch: int, keep: bool):
+    """Forward of one pre-LN ViT block on prepared weights; returns (x2, activations for the backward or None)."""
+    n1w, n1b, wq, qkvb, wp, projb, ls1, n2w, n2b, w1, fc1b, w2, fc2b, ls2 = wts
+    M, C = x0.shape
+    N = M // batch
+    xn1 = ops.layernorm(x0, n1w, n1b, 1e-6, out_dtype=torch.bfloat16)
+    qkv = ops.gemm_tn(xn1, wq, qkvb, None, torch.bfloat16)
+    att, lse = attention_fwd_lse(qkv.view(batch, N, 3 * C), heads)
+    att = att.view(M, C)
+    branch = lambda g: torch.empty((M, C), device=x0.device, dtype=torch.bfloat16) if (keep and g is not None) else None  # noqa
+    x1 = x0.clone()
+    br1 = branch(ls1)
+    gemm_tn_residual_ex_(x1, att, wp, projb, ls1, br1)
+    xn2 = ops.layernorm(x1, n2w, n2b, 1e-6, out_dtype=torch.bfloat16)
+    hpre = ops.gemm_tn(xn2, w1, fc1b, None, torch.bfloat16)
+    hid = gelu(hpre)
+    x2 = x1.clone()
+    br2 = branch(ls2)
+    gemm_tn_residual_ex_(x2, hid, w2, fc2b, ls2, br2)
+    return x2, ((x1, xn1, qkv, att, lse, br1, xn2, hpre, hid, br2) if keep else None)
+
+
+class _VitBlockFn(torch.autograd.Function):
+    """timm ViT `Block` (pre-LN attention + GELU MLP, LayerScale ls1 / ls2 when given) forward / backward on the CUDA
+    kernels; bf16 GEMM operands, fp32 residual stream and fp32 master weights, as `_BlockFn`.  Saved for the backward: what
+    `_BlockFn` saves, plus the bf16 pre-LayerScale branch values of the two residual GEMMs (LayerScale blocks only).
+    checkpoint=True saves the block input only and recomputes the forward during the backward."""
+
+    @staticmethod
+    def forward(ctx, x0, n1w, n1b, qkvw, qkvb, projw, projb, ls1, n2w, n2b, fc1w, fc1b, fc2w, fc2b, ls2, heads: int, batch: int,
+                checkpoint: bool):
+        if not x0.is_cuda:
+            raise _lib.DvtError("dvt_b200 ViT training needs CUDA tensors (no CPU fallback)")
+        f32 = lambda t: None if t is None else t.detach().float().contiguous()      # noqa: E731
+        b16 = lambda t: t.detach().to(torch.bfloat16).contiguous()                   # noqa: E731
+        wts = (f32(n1w), f32(n1b), b16(qkvw), f32(qkvb), b16(projw), f32(projb), f32(ls1), f32(n2w), f32(n2b), b16(fc1w),
+               f32(fc1b), b16(fc2w), f32(fc2b), f32(ls2))
+        x0 = x0.detach().float().contiguous()
+        x2, acts = _vit_block_fwd(x0, wts, heads, batch, keep=not checkpoint)
+        ctx.wts, ctx.heads, ctx.batch, ctx.checkpoint = wts, heads, batch, checkpoint
+        ctx.save_for_backward(x0, *(acts if acts is not None else ()))
+        return x2
+
+    @staticmethod
+    def backward(ctx, dx2):
+        x0, *acts = ctx.saved_tensors
+        wts, heads, batch = ctx.wts, ctx.heads, ctx.batch
+        n1w, _, wq, _, wp, _, ls1, n2w, _, w1, _, w2, _, ls2 = wts
+        if ctx.checkpoint:
+            _, acts = _vit_block_fwd(x0, wts, heads, batch, keep=True)
+        x1, xn1, qkv, att, lse, br1, xn2, hpre, hid, br2 = acts
+        M, C = x0.shape
+        N = M // batch
+        dx2 = dx2.detach().float().contiguous()
+        # ---- MLP branch: x2 = x1 + ls2 * (fc2(gelu(fc1(LN2(x1)))) ----
+        d2, g_fc2b, g_ls2 = layerscale_bwd(dx2, br2, ls2)
+        g_fc2w = wgrad(d2, hid)
+        dhpre = dgrad(d2, w2, torch.bfloat16, gelu_preact=hpre)
+        g_fc1w = wgrad(dhpre, xn2)
+        g_fc1b = colsum(dhpre)
+        dxn2 = dgrad(dhpre, w1, torch.float32)
+        dx1 = dx2.clone()
+        g_n2w, g_n2b = layernorm_bwd_(dx1, x1, n2w, dxn2)
+        # ---- attention branch: x1 = x0 + ls1 * proj(attn(qkv(LN1(x0)))) ----
+        d1, g_projb, g_ls1 = layerscale_bwd(dx1, br1, ls1)
+        g_projw = wgrad(d1, att)
+        datt = dgrad(d1, wp, torch.bfloat16)
+        dqkv = attention_bwd(qkv.view(batch, N, 3 * C), att.view(batch, N, C), datt.view(batch, N, C), lse, heads).view(M, 3 * C)
+        g_qkvw = wgrad(dqkv, xn1)
+        g_qkvb = colsum(dqkv)
+        dxn1 = dgrad(dqkv, wq, torch.float32)
+        dx0 = dx1
+        g_n1w, g_n1b = layernorm_bwd_(dx0, x0, n1w, dxn1)
+        return (dx0, g_n1w, g_n1b, g_qkvw, g_qkvb, g_projw, g_projb, g_ls1, g_n2w, g_n2b, g_fc1w, g_fc1b, g_fc2w, g_fc2b, g_ls2,
+                None, None, None)
+
+
+def vit_block_forward(x: torch.Tensor, blk, heads: int, batch: int, checkpoint: bool = False) -> torch.Tensor:
+    """x f32 [batch * tokens, C] through one ViT block (`blk`: module with timm Block parameter names; ls1 / ls2 either
+    LayerScale modules with `gamma` or identities)."""
+    ls1 = getattr(blk.ls1, "gamma", None)
+    ls2 = getattr(blk.ls2, "gamma", None)
+    return _VitBlockFn.apply(x, blk.norm1.weight, blk.norm1.bias, blk.attn.qkv.weight, blk.attn.qkv.bias, blk.attn.proj.weight,
+                             blk.attn.proj.bias, ls1, blk.norm2.weight, blk.norm2.bias, blk.mlp.fc1.weight, blk.mlp.fc1.bias,
+                             blk.mlp.fc2.weight, blk.mlp.fc2.bias, ls2, heads, batch, checkpoint)
+
+
+class _VitNormStripFn(torch.autograd.Function):
+    """Final LayerNorm over the token rows with the prefix tokens dropped (dvt_layernorm in_group / skip form): x f32
+    [B * ntok, C] -> f32 [B * (ntok - prefix), C]; backward through dvt_layernorm_bwd_grouped (prefix rows get zero)."""
+
+    @staticmethod
+    def forward(ctx, x, w, b, ntok: int, prefix: int):
+        x = x.detach().float().contiguous()
+        wf, bf = w.detach().float().contiguous(), b.detach().float().contiguous()
+        y = ops.layernorm(x, wf, bf, 1e-6, out_dtype=torch.float32, in_group=ntok, skip=prefix)
+        ctx.save_for_backward(x, wf)
+        ctx.meta = (ntok, prefix)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, wf = ctx.saved_tensors
+        ntok, prefix = ctx.meta
+        dx = torch.zeros_like(x)
+        dg, db = layernorm_bwd_grouped_(dx, x, wf, dy.detach().float().contiguous(), ntok, prefix)
+        return dx, dg, db, None, None
+
+
+def vit_norm_strip(x: torch.Tensor, w, b, ntok: int, prefix: int) -> torch.Tensor:
+    return _VitNormStripFn.apply(x, w, b, ntok, prefix)

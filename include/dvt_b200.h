@@ -237,6 +237,40 @@ int dvt_adamw(float* p, const float* g, float* m, float* v, size_t n, double lr,
               double weight_decay, long long step, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * Stage 3: distillation of the whole ViT backbone (reference main_distillation.py: the student
+ * PretrainedViTWrapper is trained so that its features match a frozen Denoiser(vit=...) teacher).  Unit operators that
+ * dvt.train_ops composes, with the stage-2 set above, into the autograd graph of the ViT.  The column sums of these
+ * calls are fixed-order two-level reductions through `workspace` (f32, at least 256 * C elements), so repeated calls are
+ * bit-identical.
+ * ------------------------------------------------------------------------------------------------------- */
+/* dvt_gemm_tn_residual that also writes the pre-LayerScale branch value A.B^T + bias as bf16 into branch_out
+ * ([M, ld_branch], optional: NULL behaves exactly like dvt_gemm_tn_residual).  x_inout is updated identically. */
+int dvt_gemm_tn_residual_ex(const void* A, int lda, const void* B, int ldb, int dtype, int M, int N, int K,
+                            const float* bias, const float* gamma, float* x_inout, int ldx, void* branch_out_bf16,
+                            int ld_branch, void* stream);
+/* Backward of x += gamma * branch (branch = A.B^T + bias): one pass over dx (f32 [rows, C], row pitch ldx) that writes
+ * dbranch = gamma * dx (bf16 [rows, C], optional), dbias[C] = sum_rows gamma * dx and, when dgamma is given, dgamma[C] =
+ * sum_rows dx * branch (branch: the bf16 [rows, C] side output of dvt_gemm_tn_residual_ex).  gamma NULL: unit scale (no
+ * LayerScale): the call casts dx to bf16 and sums its columns.  dbias / dgamma are overwritten. */
+int dvt_layerscale_bwd(const float* dx, int ldx, const void* branch_bf16, const float* gamma, void* dbranch_bf16, float* dbias,
+                       float* dgamma, float* workspace, int rows, int C, void* stream);
+/* Token assembly of the ViT forward on caller-owned tensors: out [B, prefix + np, C] f32 = patch rows
+ * patches (bf16 [B*np, Kp], dvt_im2col) . w^T (bf16 [C, Kp], zero-padded conv weight) + bias + pos_patch[p] after
+ * `prefix` rows copied from prefix_rows [prefix, C] (what dvt_vit_forward does before the first block). */
+int dvt_vit_embed_fwd(const void* patches_bf16, int Kp, const void* w_bf16, const float* bias, const float* pos_patch,
+                      const float* prefix_rows, int B, int np, int prefix, int C, float* out, void* stream);
+/* Backward of dvt_vit_embed_fwd w.r.t. everything but the image: from dx0 (f32 [B, ntok, C], ntok = prefix + np) writes
+ * dpatch (bf16 [B*np, C], the patch rows compacted: the dY of the patch-embed weight gradient), dpos (f32 [np, C], summed
+ * over the batch), dprefix (f32 [prefix, C], summed over the batch) and dbias (f32 [C]).  All overwritten. */
+int dvt_vit_embed_bwd(const float* dx0, int B, int ntok, int prefix, int C, void* dpatch_bf16, float* dpos, float* dprefix,
+                      float* dbias, float* workspace, void* stream);
+/* Backward of dvt_layernorm in its in_group / skip form (final norm + prefix strip): dy f32 [rows / in_group * (in_group -
+ * skip), C] holds the compacted rows, x and dx_accum f32 [rows, C] the full ones; dx_accum += d/dx on the kept rows only
+ * (the skipped rows are not touched); dgamma / dbeta [C] are overwritten. */
+int dvt_layernorm_bwd_grouped(const float* x, const float* gamma, const float* dy, float* dx_accum, float* dgamma, float* dbeta,
+                              float* workspace, int rows, int C, float eps, int in_group, int skip, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * view generation (SURVEY.md 8(f-1), the step in front of HP-1)
  * Replaces RandomResizedCropFlip.forward (dvt/dataset/transform.py:39-76) + the 8-worker DataLoader of
  * main_img_denoising.py:277-310.  image: device f32 [3, H, W] (already normalised).  boxes_host: HOST int32 [V, 4] =

@@ -7,7 +7,7 @@
 namespace dvt {
 struct Vit;
 int vit_create(Vit** out, int embed, int depth, int heads, int patch, int mlp_hidden, int swiglu, int layerscale,
-               int prefix, float ln_eps);
+               int prefix, float ln_eps, int pre_norm, int patch_bias);
 void vit_destroy(Vit* v);
 int vit_load(Vit* v, const char* name, const float* src, size_t numel);
 int vit_reserve(Vit* v, size_t tokens, size_t patches);
@@ -43,7 +43,8 @@ int hashgrid_fwd(int n_levels, const float* scale, const uint32_t* res, const ui
 int hashgrid_bwd(int n_levels, const float* scale, const uint32_t* res, const uint32_t* size, const uint32_t* offset,
                  const uint32_t* hashed, const float* coords, int n, const float* dout, float* gtable, cudaStream_t st);
 int launch_attention_bwd(const __nv_bfloat16* qkv, const __nv_bfloat16* out, const __nv_bfloat16* dout, const float* lse,
-                         __nv_bfloat16* dqkv, float* dq_acc, float* delta, int B, int N, int heads, cudaStream_t stream);
+                         __nv_bfloat16* dqkv, float* dq_acc, float* delta, int B, int N, int heads, cudaStream_t stream,
+                         int head_dim);
 int launch_layernorm_bwd(const float* x, const float* gamma, const float* dy, float* dx_accum, float* dgamma, float* dbeta,
                          int rows, int C, float eps, cudaStream_t st);
 int launch_colsum(const void* in, bool bf16, int ld, int rows, int cols, float* out, cudaStream_t st);
@@ -168,6 +169,14 @@ int dvt_attention_fwd(const void* qkv_bf16, void* out_bf16, int B, int N, int he
                           B, N, heads, reinterpret_cast<cudaStream_t>(stream), impl);
 }
 
+int dvt_attention_fwd_hd(const void* qkv_bf16, void* out_bf16, int B, int N, int heads, int head_dim, void* stream) {
+  DVT_REQUIRE(qkv_bf16 && out_bf16, "dvt_attention_fwd_hd: null pointer");
+  int impl = eff_impl();
+  if (impl < 0) impl = default_gemm_impl();
+  return launch_attention(reinterpret_cast<const __nv_bfloat16*>(qkv_bf16), reinterpret_cast<__nv_bfloat16*>(out_bf16),
+                          B, N, heads, reinterpret_cast<cudaStream_t>(stream), impl, nullptr, head_dim);
+}
+
 /* ---- stage-2 training operators (SURVEY.md 8(f-2)) ---- */
 int dvt_attention_fwd_lse(const void* qkv_bf16, void* out_bf16, float* lse, int B, int N, int heads, void* stream) {
   DVT_REQUIRE(qkv_bf16 && out_bf16 && lse, "dvt_attention_fwd_lse: null pointer");
@@ -178,7 +187,20 @@ int dvt_attention_bwd(const void* qkv_bf16, const void* out_bf16, const void* do
                       float* dq_workspace, float* delta_workspace, int B, int N, int heads, void* stream) {
   return launch_attention_bwd(reinterpret_cast<const __nv_bfloat16*>(qkv_bf16), reinterpret_cast<const __nv_bfloat16*>(out_bf16),
                               reinterpret_cast<const __nv_bfloat16*>(dout_bf16), lse, reinterpret_cast<__nv_bfloat16*>(dqkv_bf16),
-                              dq_workspace, delta_workspace, B, N, heads, reinterpret_cast<cudaStream_t>(stream));
+                              dq_workspace, delta_workspace, B, N, heads, reinterpret_cast<cudaStream_t>(stream), 64);
+}
+int dvt_attention_fwd_lse_hd(const void* qkv_bf16, void* out_bf16, float* lse, int B, int N, int heads, int head_dim,
+                             void* stream) {
+  DVT_REQUIRE(qkv_bf16 && out_bf16 && lse, "dvt_attention_fwd_lse_hd: null pointer");
+  return launch_attention(reinterpret_cast<const __nv_bfloat16*>(qkv_bf16), reinterpret_cast<__nv_bfloat16*>(out_bf16),
+                          B, N, heads, reinterpret_cast<cudaStream_t>(stream), 0, lse, head_dim);
+}
+int dvt_attention_bwd_hd(const void* qkv_bf16, const void* out_bf16, const void* dout_bf16, const float* lse,
+                         void* dqkv_bf16, float* dq_workspace, float* delta_workspace, int B, int N, int heads, int head_dim,
+                         void* stream) {
+  return launch_attention_bwd(reinterpret_cast<const __nv_bfloat16*>(qkv_bf16), reinterpret_cast<const __nv_bfloat16*>(out_bf16),
+                              reinterpret_cast<const __nv_bfloat16*>(dout_bf16), lse, reinterpret_cast<__nv_bfloat16*>(dqkv_bf16),
+                              dq_workspace, delta_workspace, B, N, heads, reinterpret_cast<cudaStream_t>(stream), head_dim);
 }
 int dvt_layernorm_bwd(const float* x, const float* gamma, const float* dy, float* dx_accum, float* dgamma, float* dbeta,
                       int rows, int C, float eps, void* stream) {
@@ -256,7 +278,13 @@ int dvt_vit_create(dvt_vit_t** out, int embed, int depth, int heads, int patch, 
                    int layerscale, int prefix_tokens, float ln_eps) {
   DVT_REQUIRE(out, "dvt_vit_create: null out");
   return vit_create(reinterpret_cast<Vit**>(out), embed, depth, heads, patch, mlp_hidden, swiglu, layerscale,
-                    prefix_tokens, ln_eps);
+                    prefix_tokens, ln_eps, 0, 1);
+}
+int dvt_vit_create_ex(dvt_vit_t** out, int embed, int depth, int heads, int patch, int mlp_hidden, int swiglu,
+                      int layerscale, int prefix_tokens, float ln_eps, int pre_norm, int patch_bias) {
+  DVT_REQUIRE(out, "dvt_vit_create_ex: null out");
+  return vit_create(reinterpret_cast<Vit**>(out), embed, depth, heads, patch, mlp_hidden, swiglu, layerscale,
+                    prefix_tokens, ln_eps, pre_norm, patch_bias);
 }
 void dvt_vit_destroy(dvt_vit_t* h) { vit_destroy(reinterpret_cast<Vit*>(h)); }
 int dvt_vit_load(dvt_vit_t* h, const char* timm_key, const float* src, size_t numel) {

@@ -254,6 +254,17 @@ __device__ __forceinline__ uint64_t make_wgmma_desc(uint32_t smem_addr, uint32_t
   d |= 1ull << 62;  // layout type: 128B swizzle
   return d;
 }
+// The same descriptor for the 32-byte swizzle (CU_TENSOR_MAP_SWIZZLE_32B: rows of 32 B = 16 bf16, 8-row atoms of 256 B).
+//   K-major operand: one k16 step per 32-byte row; 8-row groups `sbo` = 256 B apart.
+//   MN-major operand: [MN / 16 atoms, `lbo` bytes apart][K rows of 32 B, 8-row groups `sbo` = 256 B apart].
+__device__ __forceinline__ uint64_t make_wgmma_desc_sw32(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
+  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
+  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
+  d |= 3ull << 62;  // layout type: 32B swizzle
+  return d;
+}
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
@@ -298,6 +309,35 @@ __device__ __forceinline__ void wgmma_64_bf16_rs(float (&d)[32], const uint32_t 
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t}\n"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(1), "n"(TB));
+}
+
+// m64n32k16 (half a 64-query tile of the head_dim-80 attention backward): 16 accumulators per thread.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_32_bf16(float (&d)[16], uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "r"(1), "n"(TA), "n"(TB));
+}
+
+// m64n16k16 forms (the 16-column tail of head_dim 80): D[64 x 16], 8 accumulators per thread.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_16_bf16(float (&d)[8], uint64_t a, uint64_t b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a), "l"(b), "r"(1), "n"(TA), "n"(TB));
+}
+
+template <int TB>
+__device__ __forceinline__ void wgmma_16_bf16_rs(float (&d)[8], const uint32_t (&a)[4], uint64_t b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, %14;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(1), "n"(TB));
 }
 
@@ -397,9 +437,11 @@ enum TmapDtype { TMAP_BF16 = 0, TMAP_F32 = 1 };
 // 2-D row-major tensor [rows, cols] with `row_pitch_bytes`; box = [box_rows, box_cols]; 128B swizzle.
 int make_tmap_2d(CUtensorMap* out, const void* base, TmapDtype dt, uint64_t rows, uint64_t cols,
                  uint64_t row_pitch_bytes, uint32_t box_rows, uint32_t box_cols);
-// 3-D tensor [d2, d1, d0(contiguous)] with byte strides for d1 and d2; box = [1, box1, box0].
+// 3-D tensor [d2, d1, d0(contiguous)] with byte strides for d1 and d2; box = [1, box1, box0].  swizzle_bytes: 128
+// (default) or 32 (boxes of 32-byte rows: the 16-column tail slab of the head_dim-80 attention tiles).
 int make_tmap_3d(CUtensorMap* out, const void* base, TmapDtype dt, uint64_t d0, uint64_t d1, uint64_t d2,
-                 uint64_t stride1_bytes, uint64_t stride2_bytes, uint32_t box0, uint32_t box1, uint32_t box2 = 1);
+                 uint64_t stride1_bytes, uint64_t stride2_bytes, uint32_t box0, uint32_t box1, uint32_t box2 = 1,
+                 int swizzle_bytes = 128);
 
 int num_sms();
 

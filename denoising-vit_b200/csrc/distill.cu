@@ -276,7 +276,7 @@ int launch_layernorm_bwd_grouped(const float* x, const float* gamma, const float
 // ----------------------------------------------------------------------------------------------------
 int launch_vit_embed_fwd(const __nv_bfloat16* patches, int Kp, const __nv_bfloat16* w, const float* bias, const float* pos_patch,
                          const float* prefix_rows, int B, int np, int prefix, int C, float* out, cudaStream_t st, int impl) {
-  DVT_REQUIRE(patches && w && bias && pos_patch && prefix_rows && out, "vit_embed_fwd: null argument");
+  DVT_REQUIRE(patches && w && pos_patch && prefix_rows && out, "vit_embed_fwd: null argument");  // bias may be null
   DVT_REQUIRE(B > 0 && np > 0 && prefix >= 1 && C % 4 == 0 && Kp % 8 == 0, "vit_embed_fwd: bad shape");
   const int ntok = np + prefix;
   GemmEpi e;

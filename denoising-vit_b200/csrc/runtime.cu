@@ -62,7 +62,7 @@ static EncodeTiledFn get_encode() {
 }
 
 static int encode(CUtensorMap* out, const void* base, TmapDtype dt, int rank, const cuuint64_t* dims,
-                  const cuuint64_t* strides, const cuuint32_t* box) {
+                  const cuuint64_t* strides, const cuuint32_t* box, int swizzle_bytes = 128) {
   EncodeTiledFn fn = get_encode();
   if (!fn) {
     set_last_error("cuTensorMapEncodeTiled is not available (no CUDA driver?)");
@@ -72,7 +72,7 @@ static int encode(CUtensorMap* out, const void* base, TmapDtype dt, int rank, co
   CUtensorMapDataType cdt = dt == TMAP_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   CUresult r = fn(out, cdt, (cuuint32_t)rank, const_cast<void*>(base), dims, strides, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_128B,
+                  swizzle_bytes == 32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_128B,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -93,11 +93,12 @@ int make_tmap_2d(CUtensorMap* out, const void* base, TmapDtype dt, uint64_t rows
 }
 
 int make_tmap_3d(CUtensorMap* out, const void* base, TmapDtype dt, uint64_t d0, uint64_t d1, uint64_t d2,
-                 uint64_t stride1_bytes, uint64_t stride2_bytes, uint32_t box0, uint32_t box1, uint32_t box2) {
+                 uint64_t stride1_bytes, uint64_t stride2_bytes, uint32_t box0, uint32_t box1, uint32_t box2,
+                 int swizzle_bytes) {
   cuuint64_t dims[3] = {d0, d1, d2};
   cuuint64_t strides[2] = {stride1_bytes, stride2_bytes};
   cuuint32_t box[3] = {box0, box1, box2};
-  return encode(out, base, dt, 3, dims, strides, box);
+  return encode(out, base, dt, 3, dims, strides, box, swizzle_bytes);
 }
 
 }  // namespace dvt

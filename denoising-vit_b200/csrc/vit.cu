@@ -4,7 +4,7 @@
 //
 // Data flow per call (M = B * tokens, C = embed dim), all activations resident in HBM workspaces owned by the
 // handle; the residual stream is fp32, GEMM operands bf16 with fp32 accumulation in registers (wgmma):
-//   im2col -> [GEMM patch-embed + bias + pos-embed -> x] -> prefix rows
+//   im2col -> [GEMM patch-embed (+ bias) + pos-embed -> x] -> prefix rows [-> norm_pre LayerNorm (CLIP: pre_norm)]
 //   per block: LN1 -> [GEMM qkv + bias] -> attention -> [GEMM proj + bias, x += ls1 * .] ->
 //              LN2 -> [GEMM fc1 + bias + GELU] -> [GEMM fc2 + bias, x += ls2 * .]
 //   final LayerNorm + prefix strip -> NHWC fp32 (the layout main_img_denoising.py:323 permutes to)
@@ -25,7 +25,7 @@ int launch_layernorm(const float* x, int ldx, const float* gamma, const float* b
 int launch_im2col(const void* x, bool x_bf16, __nv_bfloat16* out, int B, int H, int W, int P, int S, int h, int w,
                   int Kp, cudaStream_t stream);
 int launch_attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int N, int heads, cudaStream_t stream,
-                     int impl, float* lse = nullptr);
+                     int impl, float* lse = nullptr, int head_dim = 64);
 __global__ void strip_copy_kernel(const float*, int, float*, int, int, int, int, int);
 __global__ void prefix_rows_kernel(const float*, float*, int, int, int, int);
 __global__ void swiglu_kernel(const __nv_bfloat16*, __nv_bfloat16*, size_t, int);
@@ -40,15 +40,18 @@ struct VitBlock {
 
 struct Vit {
   int embed, depth, heads, patch, mlp_hidden, swiglu, layerscale, prefix;
+  int head_dim, pre_norm, patch_bias;
   float ln_eps;
   int Kp;  // padded patch-embed K
   __nv_bfloat16* pe_w = nullptr;
   float *pe_b = nullptr, *norm_w = nullptr, *norm_b = nullptr;
+  float *npre_w = nullptr, *npre_b = nullptr;  // norm_pre (pre_norm only)
   std::vector<VitBlock> blocks;
   std::vector<void*> owned;
   // workspace
   size_t cap_tokens = 0, cap_patches = 0;
   float* x = nullptr;
+  float* x_embed = nullptr;  // token assembly output when pre_norm (norm_pre then writes x)
   __nv_bfloat16 *xn = nullptr, *qkv = nullptr, *attn = nullptr, *hid = nullptr, *hid2 = nullptr, *patches = nullptr;
   float* stage = nullptr;
   size_t stage_cap = 0;
@@ -62,16 +65,18 @@ static int dev_alloc(Vit* v, void** p, size_t bytes) {
 }
 
 int vit_create(Vit** out, int embed, int depth, int heads, int patch, int mlp_hidden, int swiglu, int layerscale,
-               int prefix, float ln_eps) {
+               int prefix, float ln_eps, int pre_norm, int patch_bias) {
   {
     int prc = gemm_prepare();
     if (prc) return prc;
   }
-  DVT_REQUIRE(embed == heads * 64, "vit: only head_dim 64 is supported (embed=%d heads=%d)", embed, heads);
+  DVT_REQUIRE(heads > 0 && (embed == heads * 64 || embed == heads * 80),
+              "vit: head_dim must be 64 or 80 (embed=%d heads=%d)", embed, heads);
   DVT_REQUIRE(embed % 8 == 0 && mlp_hidden % 8 == 0 && depth > 0 && patch > 0 && prefix >= 1, "vit: bad config");
   Vit* v = new Vit();
   v->embed = embed; v->depth = depth; v->heads = heads; v->patch = patch; v->mlp_hidden = mlp_hidden;
   v->swiglu = swiglu; v->layerscale = layerscale; v->prefix = prefix; v->ln_eps = ln_eps;
+  v->head_dim = embed / heads; v->pre_norm = pre_norm ? 1 : 0; v->patch_bias = patch_bias ? 1 : 0;
   v->Kp = (3 * patch * patch + 7) / 8 * 8;
   v->blocks.resize(depth);
   const int C = embed, Hm = mlp_hidden, fc2_in = swiglu ? mlp_hidden / 2 : mlp_hidden;
@@ -79,6 +84,7 @@ int vit_create(Vit** out, int embed, int depth, int heads, int patch, int mlp_hi
   auto A = [&](void** p, size_t bytes) { if (!rc) rc = dev_alloc(v, p, bytes); };
   A((void**)&v->pe_w, (size_t)C * v->Kp * 2);
   A((void**)&v->pe_b, C * 4); A((void**)&v->norm_w, C * 4); A((void**)&v->norm_b, C * 4);
+  if (v->pre_norm) { A((void**)&v->npre_w, C * 4); A((void**)&v->npre_b, C * 4); }
   for (auto& b : v->blocks) {
     A((void**)&b.n1w, C * 4); A((void**)&b.n1b, C * 4); A((void**)&b.n2w, C * 4); A((void**)&b.n2b, C * 4);
     A((void**)&b.qkv_b, 3 * C * 4); A((void**)&b.proj_b, C * 4); A((void**)&b.fc1_b, Hm * 4); A((void**)&b.fc2_b, C * 4);
@@ -95,7 +101,7 @@ void vit_destroy(Vit* v) {
   if (!v) return;
   for (void* p : v->owned) cudaFree(p);
   cudaFree(v->x); cudaFree(v->xn); cudaFree(v->qkv); cudaFree(v->attn); cudaFree(v->hid); cudaFree(v->hid2);
-  cudaFree(v->patches); cudaFree(v->stage);
+  cudaFree(v->x_embed); cudaFree(v->patches); cudaFree(v->stage);
   delete v;
 }
 
@@ -108,7 +114,9 @@ int vit_load(Vit* v, const char* name_c, const float* src, size_t numel) {
   size_t expect = 0;
   bool pad_pe = false;
   if (name == "patch_embed.proj.weight") { bf_dst = v->pe_w; expect = (size_t)C * 3 * v->patch * v->patch; pad_pe = true; }
-  else if (name == "patch_embed.proj.bias") { f32_dst = v->pe_b; expect = C; }
+  else if (name == "patch_embed.proj.bias" && v->patch_bias) { f32_dst = v->pe_b; expect = C; }
+  else if (name == "norm_pre.weight" && v->pre_norm) { f32_dst = v->npre_w; expect = C; }
+  else if (name == "norm_pre.bias" && v->pre_norm) { f32_dst = v->npre_b; expect = C; }
   else if (name == "norm.weight") { f32_dst = v->norm_w; expect = C; }
   else if (name == "norm.bias") { f32_dst = v->norm_b; expect = C; }
   else if (name.rfind("blocks.", 0) == 0) {
@@ -165,8 +173,10 @@ int vit_reserve(Vit* v, size_t tokens, size_t patches) {
   const int C = v->embed;
   if (tokens > v->cap_tokens) {
     cudaFree(v->x); cudaFree(v->xn); cudaFree(v->qkv); cudaFree(v->attn); cudaFree(v->hid); cudaFree(v->hid2);
-    v->x = nullptr; v->xn = v->qkv = v->attn = v->hid = v->hid2 = nullptr; v->cap_tokens = 0;
+    cudaFree(v->x_embed);
+    v->x = v->x_embed = nullptr; v->xn = v->qkv = v->attn = v->hid = v->hid2 = nullptr; v->cap_tokens = 0;
     DVT_CUDA_OK(cudaMalloc(&v->x, tokens * C * 4));
+    if (v->pre_norm) DVT_CUDA_OK(cudaMalloc(&v->x_embed, tokens * C * 4));
     DVT_CUDA_OK(cudaMalloc(&v->xn, tokens * C * 2));
     DVT_CUDA_OK(cudaMalloc(&v->qkv, tokens * 3 * C * 2));
     DVT_CUDA_OK(cudaMalloc(&v->attn, tokens * C * 2));
@@ -199,17 +209,22 @@ int vit_forward(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int 
 
   rc = launch_im2col(x_in, x_bf16, v->patches, B, H, W, P, stride, h, w, v->Kp, stream);
   if (rc) return rc;
+  float* x_tok = v->pre_norm ? v->x_embed : v->x;  // token assembly target
   {
     GemmEpi e;
-    e.bias = v->pe_b; e.out_mode = OUT_F32_REMAP; e.out = v->x; e.ldo = C; e.addend = pos_patch;
+    e.bias = v->patch_bias ? v->pe_b : nullptr; e.out_mode = OUT_F32_REMAP; e.out = x_tok; e.ldo = C; e.addend = pos_patch;
     e.rows_per_group = np; e.group_stride = ntok; e.row_offset = v->prefix;
     GemmShape s{B * np, C, v->Kp, 1};
     rc = launch_gemm_tn(v->patches, v->Kp, v->pe_w, v->Kp, TMAP_BF16, s, e, stream, gi);
     if (rc) return rc;
   }
-  prefix_rows_kernel<<<B * v->prefix, 256, 0, stream>>>(prefix_rows, v->x, B, v->prefix, ntok, C);
+  prefix_rows_kernel<<<B * v->prefix, 256, 0, stream>>>(prefix_rows, x_tok, B, v->prefix, ntok, C);
   DVT_CUDA_OK(cudaGetLastError());
   count_launch();
+  if (v->pre_norm) {  // timm norm_pre over every token row (f32 -> f32, out of place)
+    rc = launch_layernorm(v->x_embed, C, v->npre_w, v->npre_b, v->x, C, false, (int)M, C, v->ln_eps, 1, 0, stream);
+    if (rc) return rc;
+  }
 
   const int Mi = (int)M;
   // Programmatic dependent launch along the block stack is available (DVT_VIT_PDL=1) but OFF by default: these kernels
@@ -236,7 +251,8 @@ int vit_forward(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int 
       rc = launch_gemm_tn(v->xn, C, b.qkv_w, C, TMAP_BF16, s, e, stream, gi);
       if (rc) return rc;
     }
-    rc = launch_attention(v->qkv, v->attn, B, ntok, v->heads, stream, gi < 0 ? default_gemm_impl() : gi);
+    rc = launch_attention(v->qkv, v->attn, B, ntok, v->heads, stream, gi < 0 ? default_gemm_impl() : gi, nullptr,
+                          v->head_dim);
     if (rc) return rc;
     {
       GemmEpi e; e.bias = b.proj_b; e.out_mode = OUT_F32_RESID; e.out = v->x; e.ldo = C;

@@ -42,6 +42,10 @@ SIGNATURES = {
     "dvt_layernorm": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_int,
                               c_int, c_void_p]),
     "dvt_attention_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "dvt_attention_fwd_hd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "dvt_attention_fwd_lse_hd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "dvt_attention_bwd_hd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                     c_int, c_void_p]),
     "dvt_attention_fwd_lse": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "dvt_attention_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                   c_void_p]),
@@ -83,6 +87,8 @@ SIGNATURES = {
     "dvt_view_crops": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p,
                                c_int, c_int, c_void_p]),
     "dvt_vit_create": (c_int, [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float]),
+    "dvt_vit_create_ex": (c_int, [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_int,
+                                  c_int]),
     "dvt_vit_destroy": (None, [c_void_p]),
     "dvt_vit_load": (c_int, [c_void_p, c_char_p, c_void_p, c_size_t]),
     "dvt_vit_reserve": (c_int, [c_void_p, c_int, c_int, c_int, c_int]),

@@ -56,16 +56,22 @@ MODEL_LIST = [
 
 IMAGENET_MEAN, IMAGENET_STD = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)
 HALF_MEAN, HALF_STD = (0.5, 0.5, 0.5), (0.5, 0.5, 0.5)
+OPENAI_CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)
+OPENAI_CLIP_STD = (0.26862954, 0.26130258, 0.27577711)
 
 
 def _arch(embed, depth, heads, img, mlp=None, swiglu=False, ls=False, reg=0, no_embed_class=False,
-          mean=IMAGENET_MEAN, std=IMAGENET_STD):
+          mean=IMAGENET_MEAN, std=IMAGENET_STD, pre_norm=False, patch_bias=True, ln_eps=1e-6):
     return dict(embed=embed, depth=depth, heads=heads, img=img, mlp=mlp or 4 * embed, swiglu=swiglu, ls=ls, reg=reg,
-                no_embed_class=no_embed_class, mean=mean, std=std)
+                no_embed_class=no_embed_class, mean=mean, std=std, pre_norm=pre_norm, patch_bias=patch_bias,
+                ln_eps=ln_eps)
 
 
-# Plain pre-LN ViTs with head_dim 64 (what the CUDA path implements).  CLIP (pre-norm + quick-gelu), EVA02 (RoPE,
-# SwiGLU+sub-LN) and ViT-H/14 MAE (head_dim 80) are listed in MODEL_LIST for CLI compatibility but raise here.
+# Pre-LN ViTs with head_dim 64 or 80 (what the CUDA path implements).  The CLIP towers are timm's pre_norm=True,
+# norm_layer=nn.LayerNorm build: a `norm_pre` LayerNorm before the first block, LayerNorm eps 1e-5, a patch embedding
+# without bias, OpenAI CLIP normalisation; their MLP is erf GELU (timm 1.0.7 keeps QuickGELU to the separate
+# *_clip_quickgelu_* models).  ViT-H/14 MAE has head_dim 1280 / 16 = 80.  EVA02 (2-D RoPE, SwiGLU with sub-LN, inner
+# attention norm) is listed in MODEL_LIST for CLI compatibility but raises here (DESIGN.md section 8).
 ARCHS = {
     "vit_small_patch8_224.dino": _arch(384, 12, 6, 224),
     "vit_small_patch16_224.dino": _arch(384, 12, 6, 224),
@@ -82,6 +88,11 @@ ARCHS = {
                                                    no_embed_class=True),
     "vit_base_patch16_224.mae": _arch(768, 12, 12, 224),
     "vit_large_patch16_224.mae": _arch(1024, 24, 16, 224),
+    "vit_huge_patch14_224.mae": _arch(1280, 32, 16, 224),
+    "vit_base_patch16_clip_384.laion2b_ft_in12k_in1k": _arch(768, 12, 12, 384, mean=OPENAI_CLIP_MEAN, std=OPENAI_CLIP_STD,
+                                                             pre_norm=True, patch_bias=False, ln_eps=1e-5),
+    "vit_base_patch16_clip_224.openai": _arch(768, 12, 12, 224, mean=OPENAI_CLIP_MEAN, std=OPENAI_CLIP_STD, pre_norm=True,
+                                              patch_bias=False, ln_eps=1e-5),
     "deit3_base_patch16_224.fb_in1k": _arch(768, 12, 12, 224, ls=True, no_embed_class=True),
     "vit_base_patch16_384.augreg_in21k_ft_in1k": _arch(768, 12, 12, 384, mean=HALF_MEAN, std=HALF_STD),
 }
@@ -109,21 +120,21 @@ class _Mlp(nn.Module):
 
 
 class _Block(nn.Module):
-    def __init__(self, dim, heads, hidden, swiglu, ls):
+    def __init__(self, dim, heads, hidden, swiglu, ls, eps=1e-6):
         super().__init__()
-        self.norm1 = nn.LayerNorm(dim, eps=1e-6)
+        self.norm1 = nn.LayerNorm(dim, eps=eps)
         self.attn = _Attn(dim, heads)
         self.ls1 = _LayerScale(dim) if ls else nn.Identity()
-        self.norm2 = nn.LayerNorm(dim, eps=1e-6)
+        self.norm2 = nn.LayerNorm(dim, eps=eps)
         self.mlp = _Mlp(dim, hidden, swiglu)
         self.ls2 = _LayerScale(dim) if ls else nn.Identity()
 
 
 class _PatchEmbed(nn.Module):
-    def __init__(self, patch, dim):
+    def __init__(self, patch, dim, bias=True):
         super().__init__()
         self.patch_size = (patch, patch)
-        self.proj = nn.Conv2d(3, dim, kernel_size=patch, stride=patch)
+        self.proj = nn.Conv2d(3, dim, kernel_size=patch, stride=patch, bias=bias)
 
     def dynamic_feat_size(self, img_size: Tuple[int, int]) -> Tuple[int, int]:
         # reference vit_wrapper.py:81-87
@@ -146,14 +157,17 @@ class B200VisionTransformer(nn.Module):
         self.dynamic_img_size = True
         grid = a["img"] // patch
         self.native_grid = (grid, grid)
-        self.patch_embed = _PatchEmbed(patch, dim)
+        self.patch_embed = _PatchEmbed(patch, dim, bias=a["patch_bias"])
         self.cls_token = nn.Parameter(torch.zeros(1, 1, dim))
         if a["reg"]:
             self.reg_token = nn.Parameter(torch.zeros(1, a["reg"], dim))
         n_pos = grid * grid + (0 if a["no_embed_class"] else 1)
         self.pos_embed = nn.Parameter(torch.randn(1, n_pos, dim) * 0.02)
-        self.blocks = nn.ModuleList([_Block(dim, a["heads"], a["mlp"], a["swiglu"], a["ls"]) for _ in range(a["depth"])])
-        self.norm = nn.LayerNorm(dim, eps=1e-6)
+        eps = a["ln_eps"]
+        if a["pre_norm"]:  # timm pre_norm=True (CLIP): LayerNorm over the assembled tokens before the first block
+            self.norm_pre = nn.LayerNorm(dim, eps=eps)
+        self.blocks = nn.ModuleList([_Block(dim, a["heads"], a["mlp"], a["swiglu"], a["ls"], eps) for _ in range(a["depth"])])
+        self.norm = nn.LayerNorm(dim, eps=eps)
         self._init_weights()
         self._handle: Optional[c_void_p] = None
         self._dirty = True
@@ -201,9 +215,9 @@ class B200VisionTransformer(nn.Module):
             self._pos_cache = {}
         if self._handle is None:
             h = c_void_p()
-            check(lib().dvt_vit_create(byref(h), a["embed"], a["depth"], a["heads"], self.patch_embed.patch_size[0],
-                                       a["mlp"], int(a["swiglu"]), int(a["ls"]), self.num_prefix_tokens, 1e-6),
-                  "dvt_vit_create")
+            check(lib().dvt_vit_create_ex(byref(h), a["embed"], a["depth"], a["heads"], self.patch_embed.patch_size[0],
+                                          a["mlp"], int(a["swiglu"]), int(a["ls"]), self.num_prefix_tokens, a["ln_eps"],
+                                          int(a["pre_norm"]), int(a["patch_bias"])), "dvt_vit_create_ex")
             self._handle = h
         if not self._dirty:
             return
@@ -284,11 +298,14 @@ class B200VisionTransformer(nn.Module):
         h, w = (H - P) // stride + 1, (W - P) // stride + 1
         prefix, ntok, C = self.num_prefix_tokens, self.num_prefix_tokens + h * w, self.embed_dim
         pos_patch, prefix_rows = self._pos_tables_train(h, w)
+        eps = self.arch["ln_eps"]
         t = train_ops.vit_embed(x, self.patch_embed.proj.weight, self.patch_embed.proj.bias, pos_patch, prefix_rows, stride)
+        if self.arch["pre_norm"]:
+            t = train_ops.vit_layernorm(t, self.norm_pre.weight, self.norm_pre.bias, eps)
         for i in range(layer_index + 1):
-            t = train_ops.vit_block_forward(t, self.blocks[i], self.arch["heads"], B, checkpoint=self._grad_ckpt)
+            t = train_ops.vit_block_forward(t, self.blocks[i], self.arch["heads"], B, checkpoint=self._grad_ckpt, eps=eps)
         if norm:
-            y = train_ops.vit_norm_strip(t, self.norm.weight, self.norm.bias, ntok, prefix)
+            y = train_ops.vit_norm_strip(t, self.norm.weight, self.norm.bias, ntok, prefix, eps)
         else:
             y = t.view(B, ntok, C)[:, prefix:]
         return y.reshape(B, h, w, C)
@@ -392,7 +409,7 @@ class PretrainedViTWrapper(nn.Module):
         from torchvision import transforms
         if model_identifier not in ARCHS:
             raise NotImplementedError(
-                f"{model_identifier}: architecture outside the plain pre-LN / head_dim-64 ViT family is not "
+                f"{model_identifier}: architecture outside the pre-LN ViT family (head_dim 64 / 80) is not "
                 "implemented by the H100 path (see DESIGN.md, out of scope)")
         a = dict(ARCHS[model_identifier])
         patch = int(kwargs.pop("patch_size", self.patch_size))

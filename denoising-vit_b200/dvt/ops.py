@@ -65,13 +65,16 @@ def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: flo
     return y
 
 
-def attention(qkv: torch.Tensor, heads: int) -> torch.Tensor:
-    """qkv bf16 [B, N, 3*heads*64] (timm Attention.qkv output) -> bf16 [B, N, heads*64]."""
+def attention(qkv: torch.Tensor, heads: int, head_dim: int = 64) -> torch.Tensor:
+    """qkv bf16 [B, N, 3*heads*head_dim] (timm Attention.qkv output) -> bf16 [B, N, heads*head_dim]; head_dim 64 or 80."""
     _need_cuda(qkv)
-    assert qkv.dtype == torch.bfloat16 and qkv.is_contiguous() and qkv.shape[2] == 3 * heads * 64
+    assert qkv.dtype == torch.bfloat16 and qkv.is_contiguous() and qkv.shape[2] == 3 * heads * head_dim
     B, N, _ = qkv.shape
-    out = torch.empty((B, N, heads * 64), device=qkv.device, dtype=torch.bfloat16)
-    check(lib().dvt_attention_fwd(ptr(qkv), ptr(out), B, N, heads, cur_stream()), "dvt_attention_fwd")
+    out = torch.empty((B, N, heads * head_dim), device=qkv.device, dtype=torch.bfloat16)
+    if head_dim == 64:
+        check(lib().dvt_attention_fwd(ptr(qkv), ptr(out), B, N, heads, cur_stream()), "dvt_attention_fwd")
+    else:
+        check(lib().dvt_attention_fwd_hd(ptr(qkv), ptr(out), B, N, heads, head_dim, cur_stream()), "dvt_attention_fwd_hd")
     return out
 
 

@@ -19,26 +19,35 @@ def _dt(t: torch.Tensor) -> int:
     return DT_BF16 if t.dtype == torch.bfloat16 else DT_F32
 
 
-def attention_fwd_lse(qkv: torch.Tensor, heads: int) -> Tuple[torch.Tensor, torch.Tensor]:
-    """qkv bf16 [B, N, 3*heads*64] -> (out bf16 [B, N, heads*64], lse f32 [B, heads, N])."""
+def attention_fwd_lse(qkv: torch.Tensor, heads: int, head_dim: int = 64) -> Tuple[torch.Tensor, torch.Tensor]:
+    """qkv bf16 [B, N, 3*heads*head_dim] -> (out bf16 [B, N, heads*head_dim], lse f32 [B, heads, N]); head_dim 64 or 80."""
     assert qkv.is_cuda and qkv.dtype == torch.bfloat16 and qkv.is_contiguous()
     B, N, _ = qkv.shape
-    out = torch.empty((B, N, heads * 64), device=qkv.device, dtype=torch.bfloat16)
+    out = torch.empty((B, N, heads * head_dim), device=qkv.device, dtype=torch.bfloat16)
     lse = torch.empty((B, heads, N), device=qkv.device, dtype=torch.float32)
-    check(lib().dvt_attention_fwd_lse(ptr(qkv), ptr(out), ptr(lse), B, N, heads, cur_stream()), "dvt_attention_fwd_lse")
+    if head_dim == 64:
+        check(lib().dvt_attention_fwd_lse(ptr(qkv), ptr(out), ptr(lse), B, N, heads, cur_stream()), "dvt_attention_fwd_lse")
+    else:
+        check(lib().dvt_attention_fwd_lse_hd(ptr(qkv), ptr(out), ptr(lse), B, N, heads, head_dim, cur_stream()),
+              "dvt_attention_fwd_lse_hd")
     return out, lse
 
 
-def attention_bwd(qkv: torch.Tensor, out: torch.Tensor, dout: torch.Tensor, lse: torch.Tensor, heads: int) -> torch.Tensor:
-    """Gradient of flash attention w.r.t. qkv (bf16 [B, N, 3C])."""
+def attention_bwd(qkv: torch.Tensor, out: torch.Tensor, dout: torch.Tensor, lse: torch.Tensor, heads: int,
+                  head_dim: int = 64) -> torch.Tensor:
+    """Gradient of flash attention w.r.t. qkv (bf16 [B, N, 3C], C = heads * head_dim)."""
     assert all(t.is_cuda and t.is_contiguous() for t in (qkv, out, dout, lse))
     assert qkv.dtype == out.dtype == dout.dtype == torch.bfloat16 and lse.dtype == torch.float32
     B, N, _ = qkv.shape
     dqkv = torch.empty_like(qkv)
-    dq_ws = torch.empty((B, N, heads * 64), device=qkv.device, dtype=torch.float32)
+    dq_ws = torch.empty((B, N, heads * head_dim), device=qkv.device, dtype=torch.float32)
     delta = torch.empty((B, heads, N), device=qkv.device, dtype=torch.float32)
-    check(lib().dvt_attention_bwd(ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(dqkv), ptr(dq_ws), ptr(delta), B, N, heads,
-                                  cur_stream()), "dvt_attention_bwd")
+    if head_dim == 64:
+        check(lib().dvt_attention_bwd(ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(dqkv), ptr(dq_ws), ptr(delta), B, N, heads,
+                                      cur_stream()), "dvt_attention_bwd")
+    else:
+        check(lib().dvt_attention_bwd_hd(ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(dqkv), ptr(dq_ws), ptr(delta), B, N,
+                                         heads, head_dim, cur_stream()), "dvt_attention_bwd_hd")
     return dqkv
 
 
@@ -304,10 +313,12 @@ class _VitEmbedFn(torch.autograd.Function):
         out = torch.empty((B * (np_ + prefix), C), device=img.device, dtype=torch.float32)
         pp = pos_patch.detach().float().contiguous()
         pr = prefix_rows.detach().float().contiguous()
-        check(lib().dvt_vit_embed_fwd(ptr(patches), Kp, ptr(wpad), ptr(pe_b.detach().float().contiguous()), ptr(pp), ptr(pr), B,
-                                      np_, prefix, C, ptr(out), cur_stream()), "dvt_vit_embed_fwd")
+        bias = None if pe_b is None else pe_b.detach().float().contiguous()   # None: patch embedding without bias (CLIP)
+        check(lib().dvt_vit_embed_fwd(ptr(patches), Kp, ptr(wpad), ptr(bias), ptr(pp), ptr(pr), B, np_, prefix, C, ptr(out),
+                                      cur_stream()), "dvt_vit_embed_fwd")
         ctx.save_for_backward(patches)
         ctx.meta = (B, prefix, C, P, K)
+        ctx.has_bias = pe_b is not None
         return out
 
     @staticmethod
@@ -316,28 +327,57 @@ class _VitEmbedFn(torch.autograd.Function):
         B, prefix, C, P, K = ctx.meta
         dpatch, dpos, dprefix, dbias = vit_embed_bwd(dx0.detach().float().contiguous(), B, prefix)
         gw = wgrad(dpatch, patches)[:, :K].reshape(C, 3, P, P)
-        return None, gw, dbias, dpos, dprefix, None
+        return None, gw, (dbias if ctx.has_bias else None), dpos, dprefix, None
 
 
 def vit_embed(img: torch.Tensor, patch_embed_w, patch_embed_b, pos_patch, prefix_rows, stride: int) -> torch.Tensor:
-    """Token rows f32 [B * (prefix + h*w), C] of images [B, 3, H, W] (f32 or bf16)."""
+    """Token rows f32 [B * (prefix + h*w), C] of images [B, 3, H, W] (f32 or bf16).  patch_embed_b None: no bias (and no
+    bias gradient)."""
     return _VitEmbedFn.apply(img, patch_embed_w, patch_embed_b, pos_patch, prefix_rows, stride)
 
 
-def _vit_block_fwd(x0, wts, heads: int, batch: int, keep: bool):
+class _VitLayerNormFn(torch.autograd.Function):
+    """LayerNorm over every token row, f32 in and out (timm `norm_pre` of the pre_norm ViTs, the CLIP towers); backward
+    through dvt_layernorm_bwd."""
+
+    @staticmethod
+    def forward(ctx, x, w, b, eps: float):
+        if not x.is_cuda:
+            raise _lib.DvtError("dvt_b200 ViT training needs CUDA tensors (no CPU fallback)")
+        x = x.detach().float().contiguous()
+        wf, bf = w.detach().float().contiguous(), b.detach().float().contiguous()
+        y = ops.layernorm(x, wf, bf, eps, out_dtype=torch.float32)
+        ctx.save_for_backward(x, wf)
+        ctx.eps = eps
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, wf = ctx.saved_tensors
+        dx = torch.zeros_like(x)
+        dg, db = layernorm_bwd_(dx, x, wf, dy.detach().float().contiguous(), ctx.eps)
+        return dx, dg, db, None
+
+
+def vit_layernorm(x: torch.Tensor, w, b, eps: float = 1e-6) -> torch.Tensor:
+    """x f32 [rows, C] -> LayerNorm(x) f32 [rows, C], differentiable w.r.t. x, w and b."""
+    return _VitLayerNormFn.apply(x, w, b, eps)
+
+
+def _vit_block_fwd(x0, wts, heads: int, batch: int, keep: bool, eps: float = 1e-6):
     """Forward of one pre-LN ViT block on prepared weights; returns (x2, activations for the backward or None)."""
     n1w, n1b, wq, qkvb, wp, projb, ls1, n2w, n2b, w1, fc1b, w2, fc2b, ls2 = wts
     M, C = x0.shape
     N = M // batch
-    xn1 = ops.layernorm(x0, n1w, n1b, 1e-6, out_dtype=torch.bfloat16)
+    xn1 = ops.layernorm(x0, n1w, n1b, eps, out_dtype=torch.bfloat16)
     qkv = ops.gemm_tn(xn1, wq, qkvb, None, torch.bfloat16)
-    att, lse = attention_fwd_lse(qkv.view(batch, N, 3 * C), heads)
+    att, lse = attention_fwd_lse(qkv.view(batch, N, 3 * C), heads, C // heads)
     att = att.view(M, C)
     branch = lambda g: torch.empty((M, C), device=x0.device, dtype=torch.bfloat16) if (keep and g is not None) else None  # noqa
     x1 = x0.clone()
     br1 = branch(ls1)
     gemm_tn_residual_ex_(x1, att, wp, projb, ls1, br1)
-    xn2 = ops.layernorm(x1, n2w, n2b, 1e-6, out_dtype=torch.bfloat16)
+    xn2 = ops.layernorm(x1, n2w, n2b, eps, out_dtype=torch.bfloat16)
     hpre = ops.gemm_tn(xn2, w1, fc1b, None, torch.bfloat16)
     hid = gelu(hpre)
     x2 = x1.clone()
@@ -354,7 +394,7 @@ class _VitBlockFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x0, n1w, n1b, qkvw, qkvb, projw, projb, ls1, n2w, n2b, fc1w, fc1b, fc2w, fc2b, ls2, heads: int, batch: int,
-                checkpoint: bool):
+                checkpoint: bool, eps: float):
         if not x0.is_cuda:
             raise _lib.DvtError("dvt_b200 ViT training needs CUDA tensors (no CPU fallback)")
         f32 = lambda t: None if t is None else t.detach().float().contiguous()      # noqa: E731
@@ -362,18 +402,18 @@ class _VitBlockFn(torch.autograd.Function):
         wts = (f32(n1w), f32(n1b), b16(qkvw), f32(qkvb), b16(projw), f32(projb), f32(ls1), f32(n2w), f32(n2b), b16(fc1w),
                f32(fc1b), b16(fc2w), f32(fc2b), f32(ls2))
         x0 = x0.detach().float().contiguous()
-        x2, acts = _vit_block_fwd(x0, wts, heads, batch, keep=not checkpoint)
-        ctx.wts, ctx.heads, ctx.batch, ctx.checkpoint = wts, heads, batch, checkpoint
+        x2, acts = _vit_block_fwd(x0, wts, heads, batch, keep=not checkpoint, eps=eps)
+        ctx.wts, ctx.heads, ctx.batch, ctx.checkpoint, ctx.eps = wts, heads, batch, checkpoint, eps
         ctx.save_for_backward(x0, *(acts if acts is not None else ()))
         return x2
 
     @staticmethod
     def backward(ctx, dx2):
         x0, *acts = ctx.saved_tensors
-        wts, heads, batch = ctx.wts, ctx.heads, ctx.batch
+        wts, heads, batch, eps = ctx.wts, ctx.heads, ctx.batch, ctx.eps
         n1w, _, wq, _, wp, _, ls1, n2w, _, w1, _, w2, _, ls2 = wts
         if ctx.checkpoint:
-            _, acts = _vit_block_fwd(x0, wts, heads, batch, keep=True)
+            _, acts = _vit_block_fwd(x0, wts, heads, batch, keep=True, eps=eps)
         x1, xn1, qkv, att, lse, br1, xn2, hpre, hid, br2 = acts
         M, C = x0.shape
         N = M // batch
@@ -386,29 +426,31 @@ class _VitBlockFn(torch.autograd.Function):
         g_fc1b = colsum(dhpre)
         dxn2 = dgrad(dhpre, w1, torch.float32)
         dx1 = dx2.clone()
-        g_n2w, g_n2b = layernorm_bwd_(dx1, x1, n2w, dxn2)
+        g_n2w, g_n2b = layernorm_bwd_(dx1, x1, n2w, dxn2, eps)
         # ---- attention branch: x1 = x0 + ls1 * proj(attn(qkv(LN1(x0)))) ----
         d1, g_projb, g_ls1 = layerscale_bwd(dx1, br1, ls1)
         g_projw = wgrad(d1, att)
         datt = dgrad(d1, wp, torch.bfloat16)
-        dqkv = attention_bwd(qkv.view(batch, N, 3 * C), att.view(batch, N, C), datt.view(batch, N, C), lse, heads).view(M, 3 * C)
+        dqkv = attention_bwd(qkv.view(batch, N, 3 * C), att.view(batch, N, C), datt.view(batch, N, C), lse, heads,
+                             C // heads).view(M, 3 * C)
         g_qkvw = wgrad(dqkv, xn1)
         g_qkvb = colsum(dqkv)
         dxn1 = dgrad(dqkv, wq, torch.float32)
         dx0 = dx1
-        g_n1w, g_n1b = layernorm_bwd_(dx0, x0, n1w, dxn1)
+        g_n1w, g_n1b = layernorm_bwd_(dx0, x0, n1w, dxn1, eps)
         return (dx0, g_n1w, g_n1b, g_qkvw, g_qkvb, g_projw, g_projb, g_ls1, g_n2w, g_n2b, g_fc1w, g_fc1b, g_fc2w, g_fc2b, g_ls2,
-                None, None, None)
+                None, None, None, None)
 
 
-def vit_block_forward(x: torch.Tensor, blk, heads: int, batch: int, checkpoint: bool = False) -> torch.Tensor:
+def vit_block_forward(x: torch.Tensor, blk, heads: int, batch: int, checkpoint: bool = False,
+                      eps: float = 1e-6) -> torch.Tensor:
     """x f32 [batch * tokens, C] through one ViT block (`blk`: module with timm Block parameter names; ls1 / ls2 either
-    LayerScale modules with `gamma` or identities)."""
+    LayerScale modules with `gamma` or identities).  head_dim = C / heads (64 or 80); eps of both LayerNorms."""
     ls1 = getattr(blk.ls1, "gamma", None)
     ls2 = getattr(blk.ls2, "gamma", None)
     return _VitBlockFn.apply(x, blk.norm1.weight, blk.norm1.bias, blk.attn.qkv.weight, blk.attn.qkv.bias, blk.attn.proj.weight,
                              blk.attn.proj.bias, ls1, blk.norm2.weight, blk.norm2.bias, blk.mlp.fc1.weight, blk.mlp.fc1.bias,
-                             blk.mlp.fc2.weight, blk.mlp.fc2.bias, ls2, heads, batch, checkpoint)
+                             blk.mlp.fc2.weight, blk.mlp.fc2.bias, ls2, heads, batch, checkpoint, eps)
 
 
 class _VitNormStripFn(torch.autograd.Function):
@@ -416,22 +458,22 @@ class _VitNormStripFn(torch.autograd.Function):
     [B * ntok, C] -> f32 [B * (ntok - prefix), C]; backward through dvt_layernorm_bwd_grouped (prefix rows get zero)."""
 
     @staticmethod
-    def forward(ctx, x, w, b, ntok: int, prefix: int):
+    def forward(ctx, x, w, b, ntok: int, prefix: int, eps: float):
         x = x.detach().float().contiguous()
         wf, bf = w.detach().float().contiguous(), b.detach().float().contiguous()
-        y = ops.layernorm(x, wf, bf, 1e-6, out_dtype=torch.float32, in_group=ntok, skip=prefix)
+        y = ops.layernorm(x, wf, bf, eps, out_dtype=torch.float32, in_group=ntok, skip=prefix)
         ctx.save_for_backward(x, wf)
-        ctx.meta = (ntok, prefix)
+        ctx.meta = (ntok, prefix, eps)
         return y
 
     @staticmethod
     def backward(ctx, dy):
         x, wf = ctx.saved_tensors
-        ntok, prefix = ctx.meta
+        ntok, prefix, eps = ctx.meta
         dx = torch.zeros_like(x)
-        dg, db = layernorm_bwd_grouped_(dx, x, wf, dy.detach().float().contiguous(), ntok, prefix)
-        return dx, dg, db, None, None
+        dg, db = layernorm_bwd_grouped_(dx, x, wf, dy.detach().float().contiguous(), ntok, prefix, eps)
+        return dx, dg, db, None, None, None
 
 
-def vit_norm_strip(x: torch.Tensor, w, b, ntok: int, prefix: int) -> torch.Tensor:
-    return _VitNormStripFn.apply(x, w, b, ntok, prefix)
+def vit_norm_strip(x: torch.Tensor, w, b, ntok: int, prefix: int, eps: float = 1e-6) -> torch.Tensor:
+    return _VitNormStripFn.apply(x, w, b, ntok, prefix, eps)

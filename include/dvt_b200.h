@@ -79,6 +79,9 @@ int dvt_layernorm(const float* x, int ldx, const float* gamma, const float* beta
  * Replaces: timm Attention.forward -> F.scaled_dot_product_attention
  * (reference restatement: evaluation/vitdet/vision_transformer.py:73-91). */
 int dvt_attention_fwd(const void* qkv_bf16, void* out_bf16, int B, int N, int heads, void* stream);
+/* dvt_attention_fwd for head_dim 64 or 80 (embed = heads * head_dim, scale head_dim^-0.5; 80: ViT-H/14).  head_dim 64
+ * is exactly dvt_attention_fwd. */
+int dvt_attention_fwd_hd(const void* qkv_bf16, void* out_bf16, int B, int N, int heads, int head_dim, void* stream);
 
 /* Patch extraction for Conv2d(3->C, kernel P, stride S): x [B,3,H,W] (f32 or bf16) -> bf16 [B*h*w, Kp],
  * Kp = round_up(3*P*P, 8), column = c*P*P + i*P + j.  h = (H-P)/S+1, w = (W-P)/S+1
@@ -94,6 +97,12 @@ typedef struct dvt_vit dvt_vit_t;
 /* prefix_tokens = 1 (cls) + number of register tokens.  Only head_dim 64 (embed == 64*heads). */
 int dvt_vit_create(dvt_vit_t** out, int embed, int depth, int heads, int patch, int mlp_hidden, int swiglu,
                    int layerscale, int prefix_tokens, float ln_eps);
+/* General form: head_dim = embed / heads is 64 or 80.  pre_norm != 0: a LayerNorm `norm_pre` (weights loaded as
+ * "norm_pre.weight" / "norm_pre.bias") over all token rows between the token assembly and the first block (timm
+ * pre_norm=True: the CLIP towers).  patch_bias == 0: the patch embedding has no bias ("patch_embed.proj.bias" is not a
+ * key).  ln_eps applies to every LayerNorm.  dvt_vit_create(...) is dvt_vit_create_ex(..., 0, 1). */
+int dvt_vit_create_ex(dvt_vit_t** out, int embed, int depth, int heads, int patch, int mlp_hidden, int swiglu,
+                      int layerscale, int prefix_tokens, float ln_eps, int pre_norm, int patch_bias);
 void dvt_vit_destroy(dvt_vit_t* h);
 /* Loads one fp32 tensor by its timm state-dict key (without the wrapper's "model." prefix), e.g.
  * "blocks.3.attn.qkv.weight".  `src` may be host or device memory.  cls_token / reg_token / pos_embed are not
@@ -209,11 +218,18 @@ int dvt_fit_sweep_once(dvt_fit_t* h, int ctas, void* stream);
  * ------------------------------------------------------------------------------------------------------- */
 /* dvt_attention_fwd that also writes lse f32 [B, heads, N]: log2-domain log-sum-exp of the scaled scores. */
 int dvt_attention_fwd_lse(const void* qkv_bf16, void* out_bf16, float* lse, int B, int N, int heads, void* stream);
+/* dvt_attention_fwd_lse for head_dim 64 or 80 (same lse convention). */
+int dvt_attention_fwd_lse_hd(const void* qkv_bf16, void* out_bf16, float* lse, int B, int N, int heads, int head_dim,
+                             void* stream);
 /* Flash-attention backward (replaces autograd through F.scaled_dot_product_attention in timm Attention): dqkv bf16
  * [B, N, 3*heads*64] from qkv, the forward output `out`, its gradient `dout` (bf16 [B, N, heads*64]) and lse.
  * Workspaces: dq_workspace f32 [B, N, heads*64], delta_workspace f32 [B, heads, N]. */
 int dvt_attention_bwd(const void* qkv_bf16, const void* out_bf16, const void* dout_bf16, const float* lse, void* dqkv_bf16,
                       float* dq_workspace, float* delta_workspace, int B, int N, int heads, void* stream);
+/* dvt_attention_bwd for head_dim 64 or 80: every heads*64 above becomes heads*head_dim. */
+int dvt_attention_bwd_hd(const void* qkv_bf16, const void* out_bf16, const void* dout_bf16, const float* lse,
+                         void* dqkv_bf16, float* dq_workspace, float* delta_workspace, int B, int N, int heads, int head_dim,
+                         void* stream);
 /* LayerNorm backward: dx_accum [rows, C] += d/dx, dgamma / dbeta [C] += their gradients (all f32; x is the LN input). */
 int dvt_layernorm_bwd(const float* x, const float* gamma, const float* dy, float* dx_accum, float* dgamma, float* dbeta,
                       int rows, int C, float eps, void* stream);
@@ -256,7 +272,8 @@ int dvt_layerscale_bwd(const float* dx, int ldx, const void* branch_bf16, const 
                        float* dgamma, float* workspace, int rows, int C, void* stream);
 /* Token assembly of the ViT forward on caller-owned tensors: out [B, prefix + np, C] f32 = patch rows
  * patches (bf16 [B*np, Kp], dvt_im2col) . w^T (bf16 [C, Kp], zero-padded conv weight) + bias + pos_patch[p] after
- * `prefix` rows copied from prefix_rows [prefix, C] (what dvt_vit_forward does before the first block). */
+ * `prefix` rows copied from prefix_rows [prefix, C] (what dvt_vit_forward does before the first block).  bias may be
+ * NULL: a patch embedding without bias (the CLIP towers). */
 int dvt_vit_embed_fwd(const void* patches_bf16, int Kp, const void* w_bf16, const float* bias, const float* pos_patch,
                       const float* prefix_rows, int B, int np, int prefix, int C, float* out, void* stream);
 /* Backward of dvt_vit_embed_fwd w.r.t. everything but the image: from dx0 (f32 [B, ntok, C], ntok = prefix + np) writes

@@ -11,12 +11,13 @@
 //           dG atomics, loss log), dgrad, dgrad, grid backward (vector atomics + touched-entry stamps),
 //           encode of the NEXT step (hash-grid gather / interpolation with the pending Adam steps applied on the fly)
 //   sides : gather of the sampled bank rows, residual MLP forward (3 GEMM) / backward (5 GEMM), weight-gradient GEMMs,
-//           Adam(small params), and the dense Adam sweep of the hash table (software-pipelined two steps deep)
+//           Adam(small params), and the dense Adam sweep of the hash table (one pass per window of k steps,
+//           software-pipelined one to two windows deep)
 // All GEMMs run on the tensor cores (gemm.cu) as 3xTF32 products of fp32 hi/lo planes (fp32-accurate: bf16 operands cannot
 // hold the cosine >= 0.999 parity bar, see DESIGN.md); weight-gradient GEMMs read the activations as MN-major
 // operands, so no transposed copies exist; bias gradients come from a ones column appended to the activation buffers.
 //
-// HBM layout: table p/m/v as two ping-pong copies of three fp32 arrays of n_entries*8, gradients as a ring of three
+// HBM layout: table p/m/v as two ping-pong copies of three fp32 arrays of n_entries*8, gradients as a ring of 2k
 // such arrays with per-entry step stamps; "small" params (field MLP, G as [h*w, C],
 // residual MLP) in one flat fp32 buffer with identically laid out m / v / grad buffers and TF32 hi/lo operand planes.
 #include "common.cuh"
@@ -32,6 +33,7 @@ namespace dvt {
 
 constexpr int FIT_MAX_LEVELS = 16;
 constexpr int FIT_F = 8;  // features per level
+constexpr int FIT_MAX_WINDOW = 8;  // steps per pipelined table sweep (DVT_FIT_SWEEP_STEPS)
 
 struct GridLevels {
   int n_levels;
@@ -118,19 +120,24 @@ __device__ __forceinline__ void adam1(float& p, float& m, float& v, float g, flo
   p = fmaf(-ss, __fdividef(m, denom), p);
 }
 
-// Optimiser state of the hash table.  State S_t (after t Adam steps) lives in p/m/v[t & 1]: the dense sweep of step t
-// reads buffer t & 1 and writes the other one, so S_t stays readable while the sweep runs.  The gradient of step t is
-// accumulated into g[t % 3]; stamp[t % 3][entry] == t + 1 marks the entries it touched.
+// Optimiser state of the hash table.  The state S_b at the start of a sweep window lives in p/m/v[buf]: a window sweep
+// reads buffer buf and writes the other one, so S_b stays readable while the sweep runs.  buf is the number of sweeps
+// since fit_begin (step_base[1], advanced with the step counter) plus the sweeps enqueued before it in the same epoch,
+// mod 2.  The gradient of step t is accumulated into ring slot t % ring; stamp[slot][entry] == t + 1 marks the entries
+// it touched (the first touch of a step overwrites the slot's stale value, so no slot is ever re-zeroed).
 struct TableBufs {
   float* p[2];
   float* m[2];
   float* v[2];
-  float* g[3];
-  uint32_t* stamp[3];
+  float* g;          // [ring][n_entries * FIT_F]
+  uint32_t* stamp;   // [ring][n_entries]
+  int ring;
+  size_t n_entries;
+  __device__ __forceinline__ int slot(int step) const { return step % ring; }
+  __device__ __forceinline__ float* g_of(int step) const { return g + (size_t)slot(step) * n_entries * FIT_F; }
+  __device__ __forceinline__ uint32_t* stamp_of(int step) const { return stamp + (size_t)slot(step) * n_entries; }
 };
-__device__ __forceinline__ int mod3(int x) { return x % 3; }
 #define DVT_SEL2(arr, i) ((i) ? (arr)[1] : (arr)[0])
-#define DVT_SEL3(arr, i) ((i) == 0 ? (arr)[0] : ((i) == 1 ? (arr)[1] : (arr)[2]))
 
 __device__ __forceinline__ void adam8(float4& pa, float4& pb, float4& ma, float4& mb, float4& va, float4& vb,
                                       const float4& ga, const float4& gb, float wd, const AdamScalars s) {
@@ -145,12 +152,15 @@ __device__ __forceinline__ void adam8(float4& pa, float4& pb, float4& ma, float4
 }
 
 // One thread per (sample, level, corner); the four corners of a cell sit in adjacent lanes and are combined with two
-// shuffles.  npeek = number of Adam steps (0, 1 or 2) that are still pending in the sweeps and are applied on the fly:
-// the encoded step is s, the state that is read is S_{s - npeek}.  table_fixed != nullptr: read that table (query mode).
+// shuffles.  npeek = number of Adam steps (0 .. MAXPEEK) that are still pending in the sweeps and are applied on the fly:
+// the encoded step is s, the state that is read is S_{s - npeek}, in state buffer (step_base[1] + buf_off) & 1.  All
+// stamp and gradient loads are issued before the first adam8 (the encode is on the critical path).
+// table_fixed != nullptr: read that table (query mode).
+template <int MAXPEEK>
 __global__ void __launch_bounds__(256)
 fit_encode_kernel(GridLevels g, TableBufs tb, const float* __restrict__ table_fixed, const float* __restrict__ coords,
                   StepRows sr, int n, float* __restrict__ enc, int ld_enc, size_t plane,
-                  const AdamScalars* __restrict__ sc, float wd, int npeek) {
+                  const AdamScalars* __restrict__ sc, float wd, int npeek, int buf_off) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   const int k = t & 3;
   // Threads past the end stay in the kernel (clamped to the last element, store predicated off): the shuffles below name
@@ -174,30 +184,32 @@ fit_encode_kernel(GridLevels g, TableBufs tb, const float* __restrict__ table_fi
   const size_t e = g.offset[l] + grid_index(g, l, cx + dx, cy + dy);
   const float w = (dx ? px : 1.f - px) * (dy ? py : 1.f - py);
   const int b = table_fixed ? 0 : sr.step() - npeek;  // state that is read
-  const float* P = table_fixed ? table_fixed : DVT_SEL2(tb.p, b & 1);
+  const int buf = table_fixed ? 0 : (sr.step_base[1] + buf_off) & 1;
+  const float* P = table_fixed ? table_fixed : DVT_SEL2(tb.p, buf);
   float4 pa = __ldcg(reinterpret_cast<const float4*>(P + e * FIT_F));
   float4 pb = __ldcg(reinterpret_cast<const float4*>(P + e * FIT_F) + 1);
   if (npeek > 0) {
-    const float4* mp = reinterpret_cast<const float4*>(DVT_SEL2(tb.m, b & 1) + e * FIT_F);
-    const float4* vp = reinterpret_cast<const float4*>(DVT_SEL2(tb.v, b & 1) + e * FIT_F);
+    const float4* mp = reinterpret_cast<const float4*>(DVT_SEL2(tb.m, buf) + e * FIT_F);
+    const float4* vp = reinterpret_cast<const float4*>(DVT_SEL2(tb.v, buf) + e * FIT_F);
     float4 ma = __ldcg(mp), mb = __ldcg(mp + 1), va = __ldcg(vp), vb = __ldcg(vp + 1);
-    const int r0 = mod3(b), r1 = mod3(b + 1);
-    const uint32_t s0 = __ldcg(DVT_SEL3(tb.stamp, r0) + e);
-    const uint32_t s1 = npeek > 1 ? __ldcg(DVT_SEL3(tb.stamp, r1) + e) : 0u;
+    uint32_t st[MAXPEEK];
+#pragma unroll
+    for (int j = 0; j < MAXPEEK; ++j) st[j] = j < npeek ? __ldcg(tb.stamp_of(b + j) + e) : 0u;
     const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
-    float4 g0a = z4, g0b = z4, g1a = z4, g1b = z4;
-    if (s0 == (uint32_t)b + 1u) {
-      const float4* gp = reinterpret_cast<const float4*>(DVT_SEL3(tb.g, r0) + e * FIT_F);
-      g0a = __ldcg(gp);
-      g0b = __ldcg(gp + 1);
+    float4 ga[MAXPEEK], gb[MAXPEEK];
+#pragma unroll
+    for (int j = 0; j < MAXPEEK; ++j) {
+      ga[j] = z4;
+      gb[j] = z4;
+      if (j < npeek && st[j] == (uint32_t)(b + j) + 1u) {
+        const float4* gp = reinterpret_cast<const float4*>(tb.g_of(b + j) + e * FIT_F);
+        ga[j] = __ldcg(gp);
+        gb[j] = __ldcg(gp + 1);
+      }
     }
-    if (npeek > 1 && s1 == (uint32_t)b + 2u) {
-      const float4* gp = reinterpret_cast<const float4*>(DVT_SEL3(tb.g, r1) + e * FIT_F);
-      g1a = __ldcg(gp);
-      g1b = __ldcg(gp + 1);
-    }
-    adam8(pa, pb, ma, mb, va, vb, g0a, g0b, wd, sc[b]);
-    if (npeek > 1) adam8(pa, pb, ma, mb, va, vb, g1a, g1b, wd, sc[b + 1]);
+#pragma unroll
+    for (int j = 0; j < MAXPEEK; ++j)
+      if (j < npeek) adam8(pa, pb, ma, mb, va, vb, ga[j], gb[j], wd, sc[b + j]);
   }
   float acc[FIT_F] = {w * pa.x, w * pa.y, w * pa.z, w * pa.w, w * pb.x, w * pb.y, w * pb.z, w * pb.w};
 #pragma unroll
@@ -252,9 +264,11 @@ __global__ void fit_corners_kernel(GridLevels g, const float* __restrict__ coord
 // in shared memory and sorted (bitonic; the keys are unique, so the order is canonical), then the first thread of every run
 // of equal entries sums the run in contribution order and adds it to the entry.
 // `stamp` (optional): stamp[entry] = step + 1 marks the entries that received a gradient this step, so that the dense
-// Adam sweep reads (and re-zeroes) the gradient of touched entries only: 24 B/param of traffic instead of 32.
-// The gradient / stamp buffers form a ring of three (TableBufs): the backward of step t writes ring slot t % 3 while the
-// sweeps of steps t-1 / t-2 may still be reading theirs.  tb.stamp[0] == nullptr: plain accumulation into tb.g[0]
+// Adam sweep reads the gradient of touched entries only: 24 B/param of traffic instead of 32.  An entry whose stamp is
+// not yet this step's holds a stale gradient of an earlier step: its first touch overwrites it (0 + contribution, the
+// value an accumulation into a zeroed slot gives, signed zeros included) instead of adding to it.
+// The gradient / stamp buffers form a ring (TableBufs): the backward of step t writes ring slot t % ring while the
+// sweeps of the two windows before may still be reading theirs.  tb.stamp == nullptr: plain accumulation into tb.g
 // (unit-test entry point).
 constexpr int GB_ROWS = 2048;
 constexpr int GB_N = 4 * GB_ROWS;                  // contributions per chunk (a power of two)
@@ -273,10 +287,9 @@ fit_grid_bwd_kernel(GridLevels g, const float* __restrict__ coords, StepRows sr,
   pdl_trigger();
   const int* rows = sr.rows(n);
   const float* xy_all = sr.coords(coords);
-  const bool stamped = tb.stamp[0] != nullptr;
-  const int slot = stamped ? mod3(sr.step()) : 0;
-  float* gtable = DVT_SEL3(tb.g, slot);
-  uint32_t* stamp = DVT_SEL3(tb.stamp, slot);
+  const bool stamped = tb.stamp != nullptr;
+  float* gtable = stamped ? tb.g_of(sr.step()) : tb.g;
+  uint32_t* stamp = stamped ? tb.stamp_of(sr.step()) : nullptr;
   const uint32_t mark = stamped ? (uint32_t)sr.step() + 1u : 0u;
   const uint32_t base = g.offset[l];
   constexpr unsigned long long PAD = ~0ull;
@@ -328,9 +341,12 @@ fit_grid_bwd_kernel(GridLevels g, const float* __restrict__ coords, StepRows sr,
         sb.x += w * b.x; sb.y += w * b.y; sb.z += w * b.z; sb.w += w * b.w;
       }
       const uint32_t entry = base + e;
+      // (entries are owned by one CTA, whose chunks are ordered by __syncthreads: the stamp read sees its earlier chunks)
+      const bool fresh = stamped && stamp[entry] != mark;
       if (stamped) stamp[entry] = mark;
       float4* dst = reinterpret_cast<float4*>(gtable + (size_t)entry * FIT_F);
-      float4 x = dst[0], y = dst[1];
+      const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+      float4 x = fresh ? z4 : dst[0], y = fresh ? z4 : dst[1];
       x.x += sa.x; x.y += sa.y; x.z += sa.z; x.w += sa.w;
       y.x += sb.x; y.y += sb.y; y.z += sb.z; y.w += sb.w;
       dst[0] = x;
@@ -628,75 +644,93 @@ static int launch_loss(const LossArgs& la, cudaStream_t st, bool pdl) {
 // ----------------------------------------------------------------------------------------------------
 // (AdamScalars / adam1() are defined above, next to the encode kernel that also applies them.)
 
-// Dense sweep of step t: S_{t+1} = Adam(S_t, g_t), read from state buffer t & 1, written to the other one (24 B/param +
-// stamps).  Gradients are read for stamped entries only.  The gradient slot of step t-1 is re-zeroed here (not its own:
-// the encode kernel may still be "peeking" at g_t while this sweep runs); the backward of step t+2, which reuses that
-// slot, is ordered after this sweep by the host.
+// Dense sweep of the window of steps [b, b + len), len <= KW: S_{b+len} = Adam^len(S_b, g_b .. g_{b+len-1}), read
+// from state buffer (step_base[1] + buf_off) & 1, written to the other one.  Every element is loaded once, takes the
+// len Adam steps in registers, one after another (the same adam1() on the same inputs as len one-step sweeps, so the
+// stored bits are the same), and is stored once: 24 B/param per window + len stamp reads per entry.  Gradients are
+// read for stamped entries only.
 // Launch geometries (fit_sweep_geometry): many short-lived 256-thread CTAs (fastest alone: 77 us, the HBM peak), or a
 // few persistent 1024-thread CTAs that fill one SM each and leave the other SMs to the GEMM chain of the next steps.
 // (Measured and rejected: one contiguous slice per CTA -- 133 us, HBM channel imbalance; maximum shared-memory
 // carve-out -- 137 us.)
-constexpr int ADAM_UNROLL = 2;
+template <int KW>
 __global__ void __launch_bounds__(1024, 1)
 fit_adam_table_kernel(TableBufs tb, size_t nvec, const AdamScalars* __restrict__ sc, const int* __restrict__ step_base,
-                      int step_off, float wd) {
+                      int step_off, int len, int buf_off, float wd) {
+  // two elements in flight per thread for one-step windows, one for longer windows; the gradient loads of windows over 4
+  // steps wait for their Adam step instead of being issued with p, m, v (registers: 64 per thread at 1024 threads)
+  constexpr int ADAM_UNROLL = KW == 1 ? 2 : 1;
+  constexpr bool HOIST = KW <= 4;
   pdl_wait();     // (no-ops unless launched with programmatic stream serialisation)
   pdl_trigger();
-  const int step = *step_base + step_off;
-  const int src = step & 1, slot = mod3(step), slot_prev = mod3(step + 2);
+  const int b = step_base[0] + step_off;
+  const int src = (step_base[1] + buf_off) & 1;
   const float4* __restrict__ p = reinterpret_cast<const float4*>(DVT_SEL2(tb.p, src));
   const float4* __restrict__ m = reinterpret_cast<const float4*>(DVT_SEL2(tb.m, src));
   const float4* __restrict__ v = reinterpret_cast<const float4*>(DVT_SEL2(tb.v, src));
   float4* __restrict__ po = reinterpret_cast<float4*>(DVT_SEL2(tb.p, src ^ 1));
   float4* __restrict__ mo = reinterpret_cast<float4*>(DVT_SEL2(tb.m, src ^ 1));
   float4* __restrict__ vo = reinterpret_cast<float4*>(DVT_SEL2(tb.v, src ^ 1));
-  const float4* __restrict__ g = reinterpret_cast<const float4*>(DVT_SEL3(tb.g, slot));
-  const uint32_t* __restrict__ stamp = DVT_SEL3(tb.stamp, slot);
-  float4* __restrict__ gz = reinterpret_cast<float4*>(DVT_SEL3(tb.g, slot_prev));
-  const uint32_t* __restrict__ stamp_z = DVT_SEL3(tb.stamp, slot_prev);
-  const AdamScalars s = sc[step];
-  const uint32_t mark = (uint32_t)step + 1u;
-  const uint32_t mark_z = step > 0 ? (uint32_t)step : 0xffffffffu;  // stamp of step - 1 (never matches at step 0)
   // grid-stride: all CTAs advance one contiguous front together, which spreads the traffic evenly over the HBM channels
   const size_t hi = nvec;
   const size_t stride = (size_t)gridDim.x * blockDim.x;
-  // The gradient load depends on the stamp; stamps are therefore fetched one iteration ahead so that the (rare)
+  // ring slot of step b + j: slot(b) + j, wrapped (len <= KW <= ring / 2)
+  auto slot_ofs = [&](int j) -> size_t {
+    int s = tb.slot(b) + j;
+    s -= s >= tb.ring ? tb.ring : 0;
+    return (size_t)s * tb.n_entries;
+  };
+  // The gradient loads depend on the stamps; stamps are therefore fetched one iteration ahead so that the (rare)
   // gradient loads are issued together with p, m, v instead of one DRAM latency later.
-  uint32_t st_next[ADAM_UNROLL], sz_next[ADAM_UNROLL];
+  uint32_t st_next[ADAM_UNROLL][KW];
   {
     const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
 #pragma unroll
     for (int u = 0; u < ADAM_UNROLL; ++u) {
       const size_t i = i0 + u * stride;
-      st_next[u] = i < hi ? __ldg(stamp + (i >> 1)) : 0u;
-      sz_next[u] = i < hi ? __ldg(stamp_z + (i >> 1)) : 0u;
+#pragma unroll
+      for (int j = 0; j < KW; ++j)
+        st_next[u][j] = (j < len && i < hi) ? __ldg(tb.stamp + slot_ofs(j) + (i >> 1)) : 0u;
     }
   }
   for (size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i0 < hi; i0 += ADAM_UNROLL * stride) {
-    float4 pp[ADAM_UNROLL], mm[ADAM_UNROLL], vv[ADAM_UNROLL], gg[ADAM_UNROLL];
+    float4 pp[ADAM_UNROLL], mm[ADAM_UNROLL], vv[ADAM_UNROLL], gg[ADAM_UNROLL][HOIST ? KW : 1];
+    uint32_t st[ADAM_UNROLL][HOIST ? 1 : KW];
     bool ok[ADAM_UNROLL];
 #pragma unroll
     for (int u = 0; u < ADAM_UNROLL; ++u) {
       const size_t i = i0 + u * stride;
       ok[u] = i < hi;
-      const bool touched = ok[u] && st_next[u] == mark;  // entry = 8 floats = 2 float4
-      const bool stale = ok[u] && sz_next[u] == mark_z;
-      gg[u] = make_float4(0.f, 0.f, 0.f, 0.f);
       if (ok[u]) { pp[u] = p[i]; mm[u] = m[i]; vv[u] = v[i]; }
-      if (touched) gg[u] = g[i];
-      if (stale) gz[i] = make_float4(0.f, 0.f, 0.f, 0.f);
       const size_t inext = i + ADAM_UNROLL * stride;
-      st_next[u] = inext < hi ? __ldg(stamp + (inext >> 1)) : 0u;
-      sz_next[u] = inext < hi ? __ldg(stamp_z + (inext >> 1)) : 0u;
+#pragma unroll
+      for (int j = 0; j < KW; ++j) {
+        if constexpr (HOIST) {
+          gg[u][j] = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (ok[u] && j < len && st_next[u][j] == (uint32_t)(b + j) + 1u)  // entry = 8 floats = 2 float4
+            gg[u][j] = reinterpret_cast<const float4*>(tb.g + slot_ofs(j) * FIT_F)[i];
+        } else {
+          st[u][j] = st_next[u][j];
+        }
+        st_next[u][j] = (j < len && inext < hi) ? __ldg(tb.stamp + slot_ofs(j) + (inext >> 1)) : 0u;
+      }
     }
 #pragma unroll
     for (int u = 0; u < ADAM_UNROLL; ++u) {
       if (!ok[u]) continue;
       const size_t i = i0 + u * stride;
-      adam1(pp[u].x, mm[u].x, vv[u].x, gg[u].x, wd, s.step_size, s.inv_bc2_sqrt);
-      adam1(pp[u].y, mm[u].y, vv[u].y, gg[u].y, wd, s.step_size, s.inv_bc2_sqrt);
-      adam1(pp[u].z, mm[u].z, vv[u].z, gg[u].z, wd, s.step_size, s.inv_bc2_sqrt);
-      adam1(pp[u].w, mm[u].w, vv[u].w, gg[u].w, wd, s.step_size, s.inv_bc2_sqrt);
+#pragma unroll
+      for (int j = 0; j < KW; ++j) {
+        if (j >= len) break;
+        float4 g = make_float4(0.f, 0.f, 0.f, 0.f);
+        if constexpr (HOIST) g = gg[u][j];
+        else if (st[u][j] == (uint32_t)(b + j) + 1u) g = reinterpret_cast<const float4*>(tb.g + slot_ofs(j) * FIT_F)[i];
+        const AdamScalars s = sc[b + j];
+        adam1(pp[u].x, mm[u].x, vv[u].x, g.x, wd, s.step_size, s.inv_bc2_sqrt);
+        adam1(pp[u].y, mm[u].y, vv[u].y, g.y, wd, s.step_size, s.inv_bc2_sqrt);
+        adam1(pp[u].z, mm[u].z, vv[u].z, g.z, wd, s.step_size, s.inv_bc2_sqrt);
+        adam1(pp[u].w, mm[u].w, vv[u].w, g.w, wd, s.step_size, s.inv_bc2_sqrt);
+      }
       po[i] = pp[u]; mo[i] = mm[u]; vo[i] = vv[u];
     }
   }
@@ -704,8 +738,8 @@ fit_adam_table_kernel(TableBufs tb, size_t nvec, const AdamScalars* __restrict__
 
 // ----------------------------------------------------------------------------------------------------
 // EXPERIMENT (DVT_FIT_SWEEP_TMA=1; not the default): the same sweep staged through shared memory by bulk async copies
-// (TMA, cp.async.bulk).  ONE thread per CTA keeps three 52 KB chunks (p, m, v and the two stamp arrays of 512 table
-// entries) in flight per SM through an mbarrier ring of four stages while 512 threads run the Adam arithmetic out of
+// (TMA, cp.async.bulk).  One-step windows only (the host runs the plain kernel for longer ones).  ONE thread per CTA
+// keeps three 50 KB chunks (p, m, v and the stamps of 512 table entries) in flight per SM through an mbarrier ring of four stages while 512 threads run the Adam arithmetic out of
 // shared memory and write the results back with coalesced 16-byte stores.  Idea: memory-level parallelism independent of
 // the thread count, so that a few dozen SMs could saturate HBM (Little's law: the bytes in flight per SM times the SMs
 // the sweep runs on, over the loaded latency, bound its rate).  Same adam1() arithmetic, same stamp rules:
@@ -718,7 +752,7 @@ constexpr int SW_STAGES = 4;
 constexpr int SW_THREADS = 512;
 struct SweepStage {
   float p[SW_FLOATS], m[SW_FLOATS], v[SW_FLOATS];
-  uint32_t stamp[SW_ENT], stamp_z[SW_ENT];
+  uint32_t stamp[SW_ENT];
 };
 constexpr size_t SW_SMEM = SW_STAGES * sizeof(SweepStage) + SW_STAGES * sizeof(uint64_t) + 128;
 static_assert(sizeof(SweepStage) % 128 == 0, "stage size keeps the 16-byte alignment of bulk copies");
@@ -726,7 +760,7 @@ static_assert(SW_SMEM <= 227 * 1024, "sweep stages exceed shared memory");
 
 __global__ void __launch_bounds__(SW_THREADS, 1)
 fit_adam_table_tma_kernel(TableBufs tb, uint32_t n_entries, const AdamScalars* __restrict__ sc,
-                          const int* __restrict__ step_base, int step_off, float wd) {
+                          const int* __restrict__ step_base, int step_off, int buf_off, float wd) {
   extern __shared__ uint8_t sw_smem_raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(sw_smem_raw) + 127) & ~uintptr_t(127));
   SweepStage* stg = reinterpret_cast<SweepStage*>(base);
@@ -739,21 +773,18 @@ fit_adam_table_tma_kernel(TableBufs tb, uint32_t n_entries, const AdamScalars* _
   __syncthreads();
   pdl_wait();     // (no-ops unless launched with programmatic stream serialisation)
   pdl_trigger();
-  const int step = *step_base + step_off;
-  const int src = step & 1, slot = mod3(step), slot_prev = mod3(step + 2);
+  const int step = step_base[0] + step_off;
+  const int src = (step_base[1] + buf_off) & 1;
   const float* __restrict__ p = DVT_SEL2(tb.p, src);
   const float* __restrict__ m = DVT_SEL2(tb.m, src);
   const float* __restrict__ v = DVT_SEL2(tb.v, src);
   float4* __restrict__ po = reinterpret_cast<float4*>(DVT_SEL2(tb.p, src ^ 1));
   float4* __restrict__ mo = reinterpret_cast<float4*>(DVT_SEL2(tb.m, src ^ 1));
   float4* __restrict__ vo = reinterpret_cast<float4*>(DVT_SEL2(tb.v, src ^ 1));
-  const float4* __restrict__ g = reinterpret_cast<const float4*>(DVT_SEL3(tb.g, slot));
-  const uint32_t* __restrict__ stamp = DVT_SEL3(tb.stamp, slot);
-  float4* __restrict__ gz = reinterpret_cast<float4*>(DVT_SEL3(tb.g, slot_prev));
-  const uint32_t* __restrict__ stamp_z = DVT_SEL3(tb.stamp, slot_prev);
+  const float4* __restrict__ g = reinterpret_cast<const float4*>(tb.g_of(step));
+  const uint32_t* __restrict__ stamp = tb.stamp_of(step);
   const AdamScalars s = sc[step];
   const uint32_t mark = (uint32_t)step + 1u;
-  const uint32_t mark_z = step > 0 ? (uint32_t)step : 0xffffffffu;  // stamp of step - 1 (never matches at step 0)
   const uint32_t n_chunks = (n_entries + SW_ENT - 1) / SW_ENT;
 
   auto issue = [&](uint32_t k) {  // thread 0: bulk loads of this CTA's k-th chunk into stage k % SW_STAGES
@@ -763,12 +794,11 @@ fit_adam_table_tma_kernel(TableBufs tb, uint32_t n_entries, const AdamScalars* _
     uint64_t* bar = &full[k % SW_STAGES];
     const uint32_t e0 = c * SW_ENT, ne = min((uint32_t)SW_ENT, n_entries - e0);
     const uint32_t bp = ne * FIT_F * 4, bs = ne * 4;  // entries per level are multiples of 8: both multiples of 32 B
-    mbar_expect_tx(bar, 3 * bp + 2 * bs);
+    mbar_expect_tx(bar, 3 * bp + bs);
     bulk_load_1d(st.p, p + (size_t)e0 * FIT_F, bp, bar);
     bulk_load_1d(st.m, m + (size_t)e0 * FIT_F, bp, bar);
     bulk_load_1d(st.v, v + (size_t)e0 * FIT_F, bp, bar);
     bulk_load_1d(st.stamp, stamp + e0, bs, bar);
-    bulk_load_1d(st.stamp_z, stamp_z + e0, bs, bar);
   };
   if (tid == 0)
     for (uint32_t k = 0; k + 1 < SW_STAGES; ++k) issue(k);
@@ -790,11 +820,9 @@ fit_adam_table_tma_kernel(TableBufs tb, uint32_t n_entries, const AdamScalars* _
       const uint32_t i = tid + u * SW_THREADS;   // float4 index inside the chunk; entry = i / 2
       if (i < ne * 2) {
         const bool touched = st.stamp[i >> 1] == mark;
-        const bool stale = st.stamp_z[i >> 1] == mark_z;
         float4 pp = sp[i], mm = sm[i], vv = sv[i];
         float4 gg = make_float4(0.f, 0.f, 0.f, 0.f);
         if (touched) gg = __ldcg(g + f0 + i);
-        if (stale) gz[f0 + i] = make_float4(0.f, 0.f, 0.f, 0.f);
         adam1(pp.x, mm.x, vv.x, gg.x, wd, s.step_size, s.inv_bc2_sqrt);
         adam1(pp.y, mm.y, vv.y, gg.y, wd, s.step_size, s.inv_bc2_sqrt);
         adam1(pp.z, mm.z, vv.z, gg.z, wd, s.step_size, s.inv_bc2_sqrt);
@@ -837,7 +865,11 @@ __global__ void fit_adam_small_kernel(float4* __restrict__ p, float4* __restrict
   }
 }
 
-__global__ void fit_advance_kernel(int* step_base, int by) { *step_base += by; }
+// step_base[0]: step counter; step_base[1]: table sweeps since fit_begin (parity = state buffer of the current step)
+__global__ void fit_advance_kernel(int* step_base, int steps, int sweeps) {
+  step_base[0] += steps;
+  step_base[1] += sweeps;
+}
 
 __global__ void fit_fill_col_kernel(float* buf, int ld, int col, int rows, float val) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -888,11 +920,17 @@ struct Fit {
   Seg W1, b1, W2, b2, G, R1, rb1, R2, rb2, R3, rb3;
   int n_small = 0;
   // device memory
-  TableBufs tb = {};                           // ping-pong p/m/v, ring of three gradient / stamp buffers
-  int cur_host = 0;                            // steps completed (host view): the current table is tb.p[cur_host & 1]
+  TableBufs tb = {};                           // ping-pong p/m/v, ring of gradient / stamp slots
+  int cur_host = 0;                            // steps completed (host view)
+  int cur_buf = 0;                             // table sweeps completed mod 2 (host view): the current table is tb.p[cur_buf]
   cudaStream_t sD = nullptr;                   // stream of the pipelined table sweeps
-  cudaEvent_t ev_sweep[3] = {};                // completion of the sweep launched at epoch step i (slot i % 3)
-  int epoch_steps = 0;                         // pipelined steps enqueued since the sweeps were last joined
+  cudaEvent_t ev_sweep[3] = {};                // completion of the window sweep w of the epoch (slot w % 3)
+  // Epoch = the steps enqueued since the sweeps were last joined (a graph, or one plain step); its windows are counted from 0
+  int epoch_steps = 0;                         // steps enqueued in this epoch
+  int epoch_windows = 0;                       // table sweeps enqueued in this epoch (the open window's index)
+  int win_first = 0, prev_first = 0;           // epoch step of the first step of the open window / of the window before
+  bool epoch_forked = false;                   // this epoch forked sweeps onto sD (pipelined schedule)
+  int sweep_steps[2] = {4, 4};                 // DVT_FIT_SWEEP_STEPS "k1,k2": window of the pipelined sweep per phase
   bool enc_ready = false;                      // f->enc already holds the encoding of the next step
   int res_x3 = 1;                              // GEMM mode of the residual MLP: 1 = 3xTF32, 2 = plain TF32 (experiment)
   int sweep_threads = 1024;                    // DVT_FIT_SWEEP_THREADS: threads of a persistent sweep CTA (1024 fills the register file of
@@ -948,6 +986,7 @@ struct Fit {
   cudaGraphExec_t graph1 = nullptr, graph2 = nullptr;
   int graph_steps = 0;
   long long graph1_nodes = 0, graph2_nodes = 0;
+  int graph1_sweeps = 0, graph2_sweeps = 0;    // table sweeps per graph launch
   cudaStream_t stream = nullptr;      // main stream of a step (critical path)
   cudaStream_t sB = nullptr, sC = nullptr, sE = nullptr;  // side streams: independent GEMM chains beside the main one
   cudaEvent_t ev_in = nullptr, ev_out = nullptr;
@@ -974,10 +1013,15 @@ static int fit_prepare_kernels() {
   const char* es = getenv("DVT_FIT_CARVEOUT_SWEEP");     // ... the sweep
   const int pct = e ? atoi(e) : 0, pct_sweep = es ? atoi(es) : 0;
 #define DVT_MAX_SHARED(k) DVT_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, pct))
-  if (pct_sweep > 0)
-    DVT_CUDA_OK(cudaFuncSetAttribute(fit_adam_table_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, pct_sweep));
+  if (pct_sweep > 0) {
+#define DVT_SWEEP_SHARED(k) DVT_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, pct_sweep))
+    DVT_SWEEP_SHARED(fit_adam_table_kernel<1>); DVT_SWEEP_SHARED(fit_adam_table_kernel<2>);
+    DVT_SWEEP_SHARED(fit_adam_table_kernel<4>); DVT_SWEEP_SHARED(fit_adam_table_kernel<8>);
+#undef DVT_SWEEP_SHARED
+  }
   if (pct <= 0) return DVT_OK;
-  DVT_MAX_SHARED(fit_encode_kernel);
+  DVT_MAX_SHARED(fit_encode_kernel<2>); DVT_MAX_SHARED(fit_encode_kernel<4>); DVT_MAX_SHARED(fit_encode_kernel<8>);
+  DVT_MAX_SHARED(fit_encode_kernel<10>); DVT_MAX_SHARED(fit_encode_kernel<16>);
   DVT_MAX_SHARED(fit_grid_bwd_kernel);
   DVT_MAX_SHARED(fit_gather_rows_kernel);
   DVT_MAX_SHARED(fit_g_scatter_kernel);
@@ -1014,6 +1058,17 @@ int fit_create(Fit** out, int C, int gh, int gw, int bsz, int n_levels, const fl
     prc = fit_prepare_kernels();
     if (prc) return prc;
   }
+  // DVT_FIT_SWEEP_STEPS="k1[,k2]" per phase: the pipelined sweep makes one pass over the table per window of k steps
+  // (1 <= k <= FIT_MAX_WINDOW; 1 = one pass per step).  The sequential schedule sweeps every step.
+  int win[2] = {Fit().sweep_steps[0], Fit().sweep_steps[1]};
+  if (const char* ss = getenv("DVT_FIT_SWEEP_STEPS")) {
+    const int got = sscanf(ss, "%d,%d", &win[0], &win[1]);
+    if (got == 1) win[1] = win[0];
+    DVT_REQUIRE(got >= 1, "fit: DVT_FIT_SWEEP_STEPS '%s' is not \"k1[,k2]\"", ss);
+  }
+  for (int q = 0; q < 2; ++q)
+    DVT_REQUIRE(win[q] >= 1 && win[q] <= FIT_MAX_WINDOW, "fit: DVT_FIT_SWEEP_STEPS %d out of range [1, %d]", win[q],
+                FIT_MAX_WINDOW);
   Fit* f = new Fit();
   int prio_lo = 0, prio_hi = 0;  // (numerically lower = higher priority)
   DVT_CUDA_OK(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
@@ -1075,6 +1130,7 @@ int fit_create(Fit** out, int C, int gh, int gw, int bsz, int n_levels, const fl
       f->pipe[q] = !off && cfg[q] >= 0;
       f->sweep_ctas[q] = f->pipe[q] ? std::min(cfg[q], num_sms()) : 0;
     }
+    for (int q = 0; q < 2; ++q) f->sweep_steps[q] = f->pipe[q] ? win[q] : 1;
   }
   f->C = C; f->gh = gh; f->gw = gw; f->hw = gh * gw; f->bsz = bsz; f->Lf = n_levels * FIT_F;
   f->grid.n_levels = n_levels;
@@ -1097,9 +1153,14 @@ int fit_create(Fit** out, int C, int gh, int gw, int bsz, int n_levels, const fl
   for (int q = 0; q < 2; ++q) {
     A((void**)&f->tb.p[q], f->n_table * 4); A((void**)&f->tb.m[q], f->n_table * 4); A((void**)&f->tb.v[q], f->n_table * 4);
   }
-  for (int q = 0; q < 3; ++q) {
-    A((void**)&f->tb.g[q], f->n_table * 4); A((void**)&f->tb.stamp[q], f->n_table / FIT_F * 4);
-  }
+  // Gradient ring: the backward of step t (window u) overwrites slot t % ring, last used by step t - ring.  Window u's
+  // first backward waits for the sweep of window u - 2, and every reader of a step's gradient (its window's sweep, the
+  // encodes of its window and of the next one) is done by then; with windows of at most k steps, t - 2k lies before
+  // window u - 1, so 2k slots suffice.
+  f->tb.ring = 2 * std::max(f->sweep_steps[0], f->sweep_steps[1]);
+  f->tb.n_entries = f->n_table / FIT_F;
+  A((void**)&f->tb.g, f->tb.ring * f->n_table * 4);
+  A((void**)&f->tb.stamp, f->tb.ring * f->tb.n_entries * 4);
   A((void**)&f->sp, (size_t)off * 4); A((void**)&f->sm, (size_t)off * 4); A((void**)&f->sv, (size_t)off * 4);
   A((void**)&f->sg, (size_t)off * 4); A((void**)&f->wsplit, (size_t)off * 8);
   const size_t n = bsz;
@@ -1107,7 +1168,7 @@ int fit_create(Fit** out, int C, int gh, int gw, int bsz, int n_levels, const fl
   A((void**)&f->dh1, n * H1 * 8); A((void**)&f->Fout, n * C * 4); A((void**)&f->denc, n * f->Lf * 4);
   A((void**)&f->rawb, n * f->ld_raw * 8); A((void**)&f->r1, n * f->ld_r * 8); A((void**)&f->r2, n * f->ld_r * 8);
   A((void**)&f->dR, n * C * 8); A((void**)&f->dr2, n * Hr * 8); A((void**)&f->dr1, n * Hr * 8);
-  A((void**)&f->Rout, n * C * 4); A((void**)&f->step_base, sizeof(int));
+  A((void**)&f->Rout, n * C * 4); A((void**)&f->step_base, 2 * sizeof(int));
   A((void**)&f->inputs_dev, sizeof(FitInputs));
   A((void**)&f->flags_dev, sizeof(int));
   A((void**)&f->wg_sem, 5 * FIT_SEM_TILES * sizeof(unsigned));
@@ -1208,7 +1269,7 @@ int fit_set_param(Fit* f, const char* name_c, const float* src, size_t numel, cu
   if (rc) return rc;
   cudaStream_t st = f->stream;
   if (name == "table") {
-    DVT_CUDA_OK(cudaMemcpyAsync(f->tb.p[f->cur_host & 1], src, numel * 4, cudaMemcpyDefault, st));
+    DVT_CUDA_OK(cudaMemcpyAsync(f->tb.p[f->cur_buf], src, numel * 4, cudaMemcpyDefault, st));
   } else if (name == "G") {  // [C, h*w] -> [h*w, C]
     if (f->q_stage_cap < numel) DVT_CUDA_OK(cudaStreamSynchronize(st));  // the staging buffer is about to be replaced
     rc = fit_stage(f, numel);
@@ -1228,10 +1289,12 @@ int fit_set_param(Fit* f, const char* name_c, const float* src, size_t numel, cu
 int fit_get_param(Fit* f, const char* name_c, float* dst, size_t numel) {
   const std::string name(name_c);
   DVT_CUDA_OK(cudaDeviceSynchronize());
-  if (name == "table" || name == "table.next") {  // "table.next": the buffer a sweep writes (dvt_fit_sweep_once, tests)
+  // "table.next": the buffer a sweep writes (dvt_fit_sweep_once, tests); "table.m" / "table.v": the table's Adam moments
+  if (name == "table" || name == "table.next" || name == "table.m" || name == "table.v") {
     DVT_REQUIRE(numel == f->n_table, "fit_get_param: table size mismatch");
-    const int b = (f->cur_host & 1) ^ (name == "table" ? 0 : 1);
-    DVT_CUDA_OK(cudaMemcpy(dst, f->tb.p[b], numel * 4, cudaMemcpyDefault));
+    const int b = f->cur_buf ^ (name == "table.next" ? 1 : 0);
+    const float* src = name == "table.m" ? f->tb.m[b] : name == "table.v" ? f->tb.v[b] : f->tb.p[b];
+    DVT_CUDA_OK(cudaMemcpy(dst, src, numel * 4, cudaMemcpyDefault));
     return DVT_OK;
   }
   Seg* s = nullptr;
@@ -1318,6 +1381,7 @@ int fit_init_params(Fit* f, uint64_t seed, cudaStream_t caller) {
     return DVT_OK;
   };
   f->cur_host = 0;
+  f->cur_buf = 0;
   FIT_RC0(launch(f->tb.p[0], f->n_table, 0, 0, 1e-4f));
   struct { Seg* w; Seg* b; uint32_t tid; } lin[] = {{&f->W1, &f->b1, 1}, {&f->W2, &f->b2, 3}, {&f->R1, &f->rb1, 5},
                                                     {&f->R2, &f->rb2, 7}, {&f->R3, &f->rb3, 9}};
@@ -1356,7 +1420,8 @@ __global__ void fit_set_inputs_kernel(FitInputs* dst, const float* bank, const f
   dst->bank = bank;
   dst->coords = coords;
   dst->idx = idx;
-  *step_base = 0;
+  step_base[0] = 0;
+  step_base[1] = 0;
 }
 
 static int fit_flags_to_error(int flags) {
@@ -1458,17 +1523,18 @@ int fit_begin(Fit* f, const float* bank, const float* coords, size_t bank_rows, 
   DVT_CUDA_OK(cudaGetLastError());
   count_launch(2);
   DVT_CUDA_OK(cudaMemsetAsync(f->losses, 0, (size_t)num_iters * 5 * 4, st));
-  if (f->cur_host & 1)  // the schedule restarts at step 0, whose state lives in buffer 0
+  if (f->cur_buf)  // the schedule restarts with no sweep done: its state lives in buffer 0
     DVT_CUDA_OK(cudaMemcpyAsync(f->tb.p[0], f->tb.p[1], f->n_table * 4, cudaMemcpyDeviceToDevice, st));
   f->cur_host = 0;
+  f->cur_buf = 0;
   DVT_CUDA_OK(cudaMemsetAsync(f->tb.m[0], 0, f->n_table * 4, st));
   DVT_CUDA_OK(cudaMemsetAsync(f->tb.v[0], 0, f->n_table * 4, st));
-  for (int q = 0; q < 3; ++q) {
-    DVT_CUDA_OK(cudaMemsetAsync(f->tb.g[q], 0, f->n_table * 4, st));
-    DVT_CUDA_OK(cudaMemsetAsync(f->tb.stamp[q], 0, f->n_table / FIT_F * 4, st));
-  }
+  // stamps of the previous fit would match this one's steps; the gradient slots need no reset (a step's first touch
+  // of an entry overwrites, fit_grid_bwd_kernel)
+  DVT_CUDA_OK(cudaMemsetAsync(f->tb.stamp, 0, (size_t)f->tb.ring * f->tb.n_entries * 4, st));
   f->enc_ready = false;
-  f->epoch_steps = 0;
+  f->epoch_steps = f->epoch_windows = f->win_first = f->prev_first = 0;
+  f->epoch_forked = false;
   DVT_CUDA_OK(cudaMemsetAsync(f->sm, 0, (size_t)f->n_small * 4, st));
   DVT_CUDA_OK(cudaMemsetAsync(f->sv, 0, (size_t)f->n_small * 4, st));
   DVT_CUDA_OK(cudaMemsetAsync(f->sg, 0, (size_t)f->n_small * 4, st));
@@ -1539,57 +1605,87 @@ static void fit_sweep_geometry(const Fit* f, bool phase2, int* grid, int* block)
   else { *grid = num_sms() * 8; *block = 256; }
 }
 
-static int fit_launch_sweep_tma(Fit* f, int ctas, int step_off, cudaStream_t st, bool pdl) {
+static int fit_launch_sweep_tma(Fit* f, int ctas, int step_off, int buf_off, cudaStream_t st, bool pdl) {
   static bool prepared = false;
   if (!prepared) {
     DVT_CUDA_OK(cudaFuncSetAttribute(fit_adam_table_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SW_SMEM));
     prepared = true;
   }
   DVT_CUDA_OK(launch_k(pdl, fit_adam_table_tma_kernel, dim3(ctas), dim3(SW_THREADS), SW_SMEM, st, f->tb,
-                       (uint32_t)(f->n_table / FIT_F), f->sc_main, f->step_base, step_off, f->wd));
+                       (uint32_t)(f->n_table / FIT_F), f->sc_main, f->step_base, step_off, buf_off, f->wd));
   DVT_CUDA_OK(cudaGetLastError());
   count_launch();
   return DVT_OK;
 }
 
-static int fit_launch_sweep(Fit* f, int step_off, bool phase2, cudaStream_t st) {
-  if (f->sweep_tma && f->sweep_ctas[phase2 ? 1 : 0] > 0)
-    return fit_launch_sweep_tma(f, f->sweep_ctas[phase2 ? 1 : 0], step_off, st, f->pdl && f->sweep_pdl);
+// The sweep kernel instance with a window capacity KW >= len (the smallest one: registers).
+static int fit_launch_sweep_kernel(Fit* f, dim3 grid, dim3 block, int step_off, int len, int buf_off, cudaStream_t st,
+                                   bool pdl) {
+  auto go = [&](auto kern) {
+    return launch_k(pdl, kern, grid, block, 0, st, f->tb, f->n_table / 4, f->sc_main, f->step_base, step_off, len, buf_off,
+                    f->wd);
+  };
+  static_assert(FIT_MAX_WINDOW <= 8, "add a sweep kernel instance");
+  DVT_REQUIRE(len >= 1 && len <= FIT_MAX_WINDOW, "fit: sweep window of %d steps", len);
+  if (len == 1) DVT_CUDA_OK(go(fit_adam_table_kernel<1>));
+  else if (len <= 2) DVT_CUDA_OK(go(fit_adam_table_kernel<2>));
+  else if (len <= 4) DVT_CUDA_OK(go(fit_adam_table_kernel<4>));
+  else DVT_CUDA_OK(go(fit_adam_table_kernel<8>));
+  DVT_CUDA_OK(cudaGetLastError());
+  count_launch();
+  return DVT_OK;
+}
+
+// Sweep of the window [step_off, step_off + len) from state buffer (step_base[1] + buf_off) & 1.
+static int fit_launch_sweep(Fit* f, int step_off, int len, int buf_off, bool phase2, cudaStream_t st) {
+  const bool pdl = f->pdl && f->sweep_pdl;
+  if (f->sweep_tma && f->sweep_ctas[phase2 ? 1 : 0] > 0 && len == 1)
+    return fit_launch_sweep_tma(f, f->sweep_ctas[phase2 ? 1 : 0], step_off, buf_off, st, pdl);
   int sg_ = 0, sb_ = 0;
   fit_sweep_geometry(f, phase2, &sg_, &sb_);
-  DVT_CUDA_OK(launch_k(f->pdl && f->sweep_pdl, fit_adam_table_kernel, dim3(sg_), dim3(sb_), 0, st, f->tb, f->n_table / 4, f->sc_main,
-                       f->step_base, step_off, f->wd));
-  DVT_CUDA_OK(cudaGetLastError());
-  count_launch();
-  return DVT_OK;
+  return fit_launch_sweep_kernel(f, dim3(sg_), dim3(sb_), step_off, len, buf_off, st, pdl);
 }
 
-// Encodes step (*step_base + step_off) into f->enc from state S_{step - npeek}, applying the npeek pending Adam steps
-// on the fly.
-static int fit_enqueue_encode(Fit* f, int step_off, int npeek, cudaStream_t st) {
+// Encodes step (*step_base + step_off) into f->enc from state S_{step - npeek} in buffer (step_base[1] + buf_off) & 1,
+// applying the npeek pending Adam steps on the fly.
+static int fit_enqueue_encode(Fit* f, int step_off, int npeek, int buf_off, cudaStream_t st) {
   const int n = f->bsz;
   const StepRows sr{nullptr, f->step_base, step_off, f->inputs_dev};
   const int tb = 256, blocks = (n * f->grid.n_levels * 4 + tb - 1) / tb;
-  DVT_CUDA_OK(launch_k(f->pdl, fit_encode_kernel, dim3(blocks), dim3(tb), 0, st, f->grid, f->tb, nullptr, f->coords, sr, n,
-                       f->enc, f->ld_enc, (size_t)n * f->ld_enc, f->sc_main, f->wd, npeek));
+  auto go = [&](auto kern) {
+    return launch_k(f->pdl, kern, dim3(blocks), dim3(tb), 0, st, f->grid, f->tb, nullptr, f->coords, sr, n, f->enc, f->ld_enc,
+                    (size_t)n * f->ld_enc, f->sc_main, f->wd, npeek, buf_off);
+  };
+  static_assert(2 * FIT_MAX_WINDOW <= 16, "add an encode kernel instance");
+  DVT_REQUIRE(npeek >= 0 && npeek <= 2 * FIT_MAX_WINDOW, "fit: encode with %d pending steps", npeek);
+  if (npeek <= 2) DVT_CUDA_OK(go(fit_encode_kernel<2>));
+  else if (npeek <= 4) DVT_CUDA_OK(go(fit_encode_kernel<4>));
+  else if (npeek <= 8) DVT_CUDA_OK(go(fit_encode_kernel<8>));
+  else if (npeek <= 10) DVT_CUDA_OK(go(fit_encode_kernel<10>));
+  else DVT_CUDA_OK(go(fit_encode_kernel<16>));
   DVT_CUDA_OK(cudaGetLastError());
   count_launch();
   return DVT_OK;
 }
 
-// One optimisation step.
+// One optimisation step.  epoch_end: the last step before the sweeps are joined (end of a graph, or a plain step).
 // Pipelined schedule (f->pipe[phase]): the dense table sweep -- half of a step's time when run in line -- is taken off the
-// critical path entirely.  Sweep(t) runs on stream sD, on its own SMs, beside the chains of steps t+1 and t+2:
-//   main stream : GEMM h1, GEMM F, [join residual fwd], loss, dgrad, dgrad, wait sweep(t-2), grid backward,
-//                 [join side chains], encode(t+1) from S_{t-1} with Adam steps t-1 and t applied on the fly, fork sweep(t)
+// critical path entirely, and makes one pass over the table per window of up to k = f->sweep_steps[phase] steps.  The
+// steps of an epoch form windows [b_0, b_1), [b_1, b_2), ... of k steps (the last one shorter when the epoch ends
+// first).  Sweep(w) runs on stream sD, on its own SMs, beside the chains of windows w+1 and w+2:
+//   main stream : GEMM h1, GEMM F, [join residual fwd], loss, dgrad, dgrad, [first step of window w: wait sweep(w-2)],
+//                 grid backward, [join side chains], encode(t+1) from S_{b_{w-1}} (S_{b_0} in window 0) with Adam steps
+//                 b_{w-1} .. t applied on the fly, [last step of window w: fork sweep(w)]
 //   side B / C  : weight-gradient GEMMs, residual MLP forward / backward, Adam(small params)
-//   side D      : sweep(t): S_t (buffer t & 1) + g_t -> S_{t+1} (other buffer); re-zeroes the gradient slot of step t-1
+//   side D      : sweep(w): S_{b_w} + g_{b_w} .. g_{b_{w+1}-1} -> S_{b_{w+1}} (the other state buffer)
 // The on-the-fly updates use the same adam1() arithmetic on the same inputs as the sweep, so the encoded values are
-// bit-identical to a sequential schedule.  Hazards: encode(t+1) reads S_{t-1}, complete since sweep(t-2) was waited for;
-// sweep(t) overwrites the buffer of S_{t-1} and is forked after encode(t+1); the backward of step t writes the ring slot
-// that sweep(t-2) re-zeroed.  Precondition: f->enc holds the encoding of step t.
+// bit-identical to a sequential schedule.  Hazards: the encodes of window w read S_{b_{w-1}}, complete since sweep(w-2)
+// was waited for, and the gradients of windows w-1 and w; sweep(w) overwrites the buffer of S_{b_{w-1}} and is forked
+// after the last of those encodes; the backward of step t overwrites the gradient ring slot of step t - 2k, which lies
+// before window w-1 (see fit_create).  With k = 1 this is the two-step-deep pipeline: one sweep per step, encodes with
+// two pending steps.  Precondition: f->enc holds the encoding of step t.
 // Sequential schedule (f->pipe[phase] == false): encode(t) at the head of the step, sweep(t) on the main stream at its tail.
-static int fit_enqueue_step(Fit* f, int step_off, bool phase2, cudaStream_t st, int impl) {
+static int fit_enqueue_step(Fit* f, int step_off, bool phase2, bool epoch_end, cudaStream_t st, int impl) {
   const int n = f->bsz, C = f->C, H1 = C / 2, Hr = C / 4, Lf = f->Lf;
   const StepRows sr{nullptr, f->step_base, step_off, f->inputs_dev};
   const int tb = 256;
@@ -1627,7 +1723,7 @@ static int fit_enqueue_step(Fit* f, int step_off, bool phase2, cudaStream_t st, 
   DVT_CUDA_OK(cudaGetLastError());
   count_launch();
   const bool pipe = f->pipe[phase2 ? 1 : 0];
-  if (!pipe) FIT_RC(fit_enqueue_encode(f, step_off, 0, st));  // else f->enc is already this step's (fit_run)
+  if (!pipe) FIT_RC(fit_enqueue_encode(f, step_off, 0, f->epoch_windows, st));  // else f->enc is already this step's (fit_run)
   if (phase2) {
     FIT_RC(fit_linear(rawb, n, C, W(f->R1), Hr, sp + f->rb1.off, ACT_RELU, f->r1, f->ld_r, p_r, true, sB, impl, pdl, f->res_x3, 0, wide));
     FIT_RC(fit_linear(r1, n, Hr, W(f->R2), Hr, sp + f->rb2.off, ACT_RELU, f->r2, f->ld_r, p_r, true, sB, impl, pdl, f->res_x3, 0, wide));
@@ -1666,10 +1762,10 @@ static int fit_enqueue_step(Fit* f, int step_off, bool phase2, cudaStream_t st, 
     DVT_CUDA_OK(cudaGetLastError());
     count_launch();
   }
-  // the gradient ring slot of this step was re-zeroed by the sweep of step t-2, which also produced the state the
-  // next encode reads
-  if (pipe && f->epoch_steps >= 2)
-    DVT_CUDA_OK(cudaStreamWaitEvent(st, f->ev_sweep[(f->epoch_steps - 2) % 3], 0));
+  // the first backward of window w waits for sweep(w-2): the last reader of the gradient slots this window overwrites,
+  // and the producer of the state the encodes of this window read
+  const int w = f->epoch_windows, j = f->epoch_steps - f->win_first;  // window of this step, position in it
+  if (pipe && j == 0 && w >= 2) DVT_CUDA_OK(cudaStreamWaitEvent(st, f->ev_sweep[(w - 2) % 3], 0));
   DVT_CUDA_OK(launch_k(pdl, fit_grid_bwd_kernel, dim3(f->grid.n_levels, GB_PARTS), dim3(GB_THREADS), (size_t)GB_SMEM, st, f->grid,
                        f->coords, sr, n, f->denc, Lf, f->tb));
   DVT_CUDA_OK(cudaGetLastError());
@@ -1698,41 +1794,58 @@ static int fit_enqueue_step(Fit* f, int step_off, bool phase2, cudaStream_t st, 
   DVT_CUDA_OK(cudaGetLastError());
   count_launch();
   if (!pipe) {
-    FIT_RC(fit_launch_sweep(f, step_off, phase2, st));
+    FIT_RC(fit_launch_sweep(f, step_off, 1, f->epoch_windows, phase2, st));
     FIT_RC(join(sB, f->ev[8]));
+    f->epoch_steps += 1;
+    f->epoch_windows += 1;
     f->enc_ready = false;
     return DVT_OK;
   }
-  // ---- encode of the NEXT step: one pending Adam step right after a join of the sweeps, two in steady state ----
-  FIT_RC(fit_enqueue_encode(f, step_off + 1, f->epoch_steps == 0 ? 1 : 2, st));
+  // ---- encode of the NEXT step, from the state before the previous window (the epoch's first state in window 0) ----
+  const int read_first = w >= 1 ? f->prev_first : 0;
+  FIT_RC(fit_enqueue_encode(f, step_off + 1, f->epoch_steps + 1 - read_first, std::max(w - 1, 0), st));
   FIT_RC(join(sB, f->ev[8]));
-  // ---- dense table sweep of this step ----
-  FIT_RC(fork(sD, f->ev[10]));
-  FIT_RC(fit_launch_sweep(f, step_off, phase2, sD));
-  DVT_CUDA_OK(cudaEventRecord(f->ev_sweep[f->epoch_steps % 3], sD));
+  // ---- dense table sweep of the window this step closes ----
+  if (j + 1 == f->sweep_steps[phase2 ? 1 : 0] || epoch_end) {
+    FIT_RC(fork(sD, f->ev[10]));
+    FIT_RC(fit_launch_sweep(f, step_off - j, j + 1, w, phase2, sD));
+    DVT_CUDA_OK(cudaEventRecord(f->ev_sweep[w % 3], sD));
+    f->epoch_forked = true;
+    f->epoch_windows += 1;
+    f->prev_first = f->win_first;
+    f->win_first = f->epoch_steps + 1;
+  }
   f->epoch_steps += 1;
   f->enc_ready = true;
   return DVT_OK;
 }
 
-// Waits (on `st`) for all pending table sweeps (sD executes them in order: the last event covers the others).
-static int fit_sync_sweep(Fit* f, cudaStream_t st) {
-  if (f->epoch_steps == 0) return DVT_OK;
-  DVT_CUDA_OK(cudaStreamWaitEvent(st, f->ev_sweep[(f->epoch_steps - 1) % 3], 0));
-  f->epoch_steps = 0;
+// Waits (on `st`) for all pending table sweeps (sD executes them in order: the last event covers the others) and starts
+// a new epoch.  Returns the number of sweeps the epoch enqueued.
+static int fit_sync_sweep(Fit* f, cudaStream_t st, int* sweeps) {
+  if (f->epoch_forked) {
+    DVT_REQUIRE(f->win_first == f->epoch_steps, "fit: an epoch ends inside a sweep window");
+    DVT_CUDA_OK(cudaStreamWaitEvent(st, f->ev_sweep[(f->epoch_windows - 1) % 3], 0));
+  }
+  *sweeps = f->epoch_windows;
+  f->epoch_steps = f->epoch_windows = f->win_first = f->prev_first = 0;
+  f->epoch_forked = false;
   return DVT_OK;
 }
 
-static int fit_capture(Fit* f, bool phase2, int steps, cudaStream_t st, int impl, cudaGraphExec_t* out, long long* nodes) {
+static int fit_capture(Fit* f, bool phase2, int steps, cudaStream_t st, int impl, cudaGraphExec_t* out, long long* nodes,
+                       int* sweeps) {
   cudaGraph_t graph = nullptr;
   const long long before = launch_count();
   DVT_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
   int rc = DVT_OK;
-  f->epoch_steps = 0;  // graphs start and end with the sweeps joined
-  for (int i = 0; i < steps && rc == DVT_OK; ++i) rc = fit_enqueue_step(f, i, phase2, st, impl);
-  if (rc == DVT_OK) rc = fit_sync_sweep(f, st);  // a capture must join every forked stream
+  // graphs start and end with the sweeps joined
+  f->epoch_steps = f->epoch_windows = f->win_first = f->prev_first = 0;
+  f->epoch_forked = false;
+  for (int i = 0; i < steps && rc == DVT_OK; ++i) rc = fit_enqueue_step(f, i, phase2, i + 1 == steps, st, impl);
+  if (rc == DVT_OK) rc = fit_sync_sweep(f, st, sweeps);  // a capture must join every forked stream
   if (rc == DVT_OK) {
-    fit_advance_kernel<<<1, 1, 0, st>>>(f->step_base, steps);
+    fit_advance_kernel<<<1, 1, 0, st>>>(f->step_base, steps, *sweeps);
     if (cudaGetLastError() != cudaSuccess) rc = DVT_ERR_CUDA;
     count_launch();
   }
@@ -1796,28 +1909,31 @@ int fit_run(Fit* f, int count, int use_graphs, cudaStream_t caller, int impl) {
     if (f->pipe[phase2 ? 1 : 0] && !f->enc_ready) {
       // a pipelined step expects its encoding in f->enc (first step of a fit / after a sequential step): plain encode,
       // all sweeps are joined here
-      FIT_RC(fit_enqueue_encode(f, 0, 0, st));
+      FIT_RC(fit_enqueue_encode(f, 0, 0, 0, st));
       f->enc_ready = true;
     }
     if (use_graphs > 0 && cur + use_graphs <= phase_end) {
       cudaGraphExec_t* g = phase2 ? &f->graph2 : &f->graph1;
       long long* nodes = phase2 ? &f->graph2_nodes : &f->graph1_nodes;
-      if (!*g) FIT_RC(fit_capture(f, phase2, use_graphs, st, impl, g, nodes));
+      int* sweeps = phase2 ? &f->graph2_sweeps : &f->graph1_sweeps;
+      if (!*g) FIT_RC(fit_capture(f, phase2, use_graphs, st, impl, g, nodes, sweeps));
       DVT_CUDA_OK(cudaGraphLaunch(*g, st));
       count_launch(*nodes);
+      f->cur_buf ^= *sweeps & 1;
       f->enc_ready = f->pipe[phase2 ? 1 : 0];  // what the captured steps leave behind
       cur += use_graphs;
     } else {
-      FIT_RC(fit_enqueue_step(f, 0, phase2, st, impl));
+      FIT_RC(fit_enqueue_step(f, 0, phase2, true, st, impl));
       // the sweep reads the device step counter: it must finish before the counter advances
-      FIT_RC(fit_sync_sweep(f, st));
-      fit_advance_kernel<<<1, 1, 0, st>>>(f->step_base, 1);
+      int sweeps = 0;
+      FIT_RC(fit_sync_sweep(f, st, &sweeps));
+      fit_advance_kernel<<<1, 1, 0, st>>>(f->step_base, 1, sweeps);
+      f->cur_buf ^= sweeps & 1;
       DVT_CUDA_OK(cudaGetLastError());
       count_launch();
       cur += 1;
     }
   }
-  FIT_RC(fit_sync_sweep(f, st));
   f->cur_host = end;
   f->cur_step = end;
   DVT_CUDA_OK(cudaEventRecord(f->ev_run_done[f->idx_slot], st));
@@ -1835,13 +1951,10 @@ int fit_sweep_once(Fit* f, int ctas, cudaStream_t st) {
   DVT_REQUIRE(f->cur_host <= f->num_iters, "fit_sweep_once: step counter %d beyond the schedule", f->cur_host);
   // ctas > 0: persistent CTAs as in the pipelined schedule (TMA-staged kernel unless DVT_FIT_SWEEP_TMA=0);
   // ctas < 0: -ctas persistent CTAs of the plain-load kernel; 0: the many-small-CTA geometry of the sequential schedule
-  if (ctas > 0 && f->sweep_tma) return fit_launch_sweep_tma(f, std::min(ctas, num_sms()), 0, st, false);
+  if (ctas > 0 && f->sweep_tma) return fit_launch_sweep_tma(f, std::min(ctas, num_sms()), 0, 0, st, false);
   const int n = ctas < 0 ? -ctas : ctas;
   const int grid = n > 0 ? std::min(n, num_sms()) : num_sms() * 8, block = n > 0 ? 1024 : 256;
-  fit_adam_table_kernel<<<grid, block, 0, st>>>(f->tb, f->n_table / 4, f->sc_main, f->step_base, 0, f->wd);
-  DVT_CUDA_OK(cudaGetLastError());
-  count_launch();
-  return DVT_OK;
+  return fit_launch_sweep_kernel(f, dim3(grid), dim3(block), 0, 1, 0, st, false);
 }
 
 int fit_losses(Fit* f, float* dst_host, int num_iters) {
@@ -1881,8 +1994,8 @@ int fit_query(Fit* f, const float* coords, int n, float* out, cudaStream_t st, i
   const int C = f->C, H1 = C / 2;
   const size_t cap = (size_t)f->q_cap, wp = (size_t)f->n_small;
   const StepRows sr{nullptr, f->step_base, 0};
-  fit_encode_kernel<<<(n * f->grid.n_levels * 4 + 255) / 256, 256, 0, st>>>(
-      f->grid, f->tb, f->tb.p[f->cur_host & 1], coords, sr, n, f->q_enc, f->ld_enc, cap * f->ld_enc, nullptr, 0.f, 0);
+  fit_encode_kernel<2><<<(n * f->grid.n_levels * 4 + 255) / 256, 256, 0, st>>>(
+      f->grid, f->tb, f->tb.p[f->cur_buf], coords, sr, n, f->q_enc, f->ld_enc, cap * f->ld_enc, nullptr, 0.f, 0, 0);
   DVT_CUDA_OK(cudaGetLastError());
   count_launch();
   FIT_RC(fit_linear(Op{f->q_enc, f->ld_enc, cap * f->ld_enc}, n, f->Lf, Op{f->wsplit + f->W1.off, f->Lf, wp}, H1,
@@ -1948,7 +2061,7 @@ int hashgrid_bwd(int n_levels, const float* scale, const uint32_t* res, const ui
   FIT_RC(levels_from_arrays(&g, n_levels, scale, res, size, offset, hashed));
   const StepRows sr{nullptr, nullptr, 0};
   TableBufs tb = {};
-  tb.g[0] = gtable;  // no stamps: plain accumulation
+  tb.g = gtable;  // no stamps: plain accumulation
   FIT_RC(fit_prepare_kernels());
   fit_grid_bwd_kernel<<<dim3(n_levels, GB_PARTS), GB_THREADS, GB_SMEM, st>>>(g, coords, sr, n, dout, n_levels * FIT_F, tb);
   DVT_CUDA_OK(cudaGetLastError());

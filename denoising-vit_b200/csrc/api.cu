@@ -49,6 +49,7 @@ int launch_layernorm_bwd(const float* x, const float* gamma, const float* dy, fl
                          int rows, int C, float eps, cudaStream_t st);
 int launch_colsum(const void* in, bool bf16, int ld, int rows, int cols, float* out, cudaStream_t st);
 int launch_gelu(const __nv_bfloat16* in, __nv_bfloat16* out, size_t n, cudaStream_t st);
+int launch_swiglu(const __nv_bfloat16* hin, __nv_bfloat16* out, size_t M, int Hh, cudaStream_t st);
 int launch_denoise_loss(const float* pred, const float* tgt, float* dpred, float* losses, int rows, int C, float grad_scale,
                         cudaStream_t st);
 int launch_adamw(float* p, const float* g, float* m, float* v, size_t n, double lr, double beta1, double beta2, double eps,
@@ -236,6 +237,24 @@ int dvt_gemm_bf16_bwd(const void* A, int lda, int a_mn, const void* B, int ldb, 
   return launch_gemm_tn(A, lda, B, ldb, TMAP_BF16, s, e, reinterpret_cast<cudaStream_t>(stream), eff_impl());
 }
 /* ---- stage-3 (distillation) operators ---- */
+int dvt_swiglu(const void* hpre_bf16, void* out_bf16, size_t M, int Hh, void* stream) {
+  return launch_swiglu(reinterpret_cast<const __nv_bfloat16*>(hpre_bf16), reinterpret_cast<__nv_bfloat16*>(out_bf16), M, Hh,
+                       reinterpret_cast<cudaStream_t>(stream));
+}
+int dvt_gemm_bf16_dgrad_swiglu(const void* dy_bf16, int ld_dy, const void* w_bf16, int ldw, int M, int Hh, int K,
+                               const void* hpre_bf16, int ld_hpre, void* dhpre_bf16, int ld_dhpre, void* stream) {
+  DVT_REQUIRE(dy_bf16 && w_bf16 && hpre_bf16 && dhpre_bf16, "dvt_gemm_bf16_dgrad_swiglu: null pointer");
+  GemmEpi e;
+  e.out = dhpre_bf16;
+  e.ldo = ld_dhpre;
+  e.out_mode = OUT_BF16;
+  e.mask = reinterpret_cast<const __nv_bfloat16*>(hpre_bf16);
+  e.ldmask = ld_hpre;
+  e.mask_mode = 2;
+  GemmShape s{M, Hh, K, 1};
+  s.b_mn = 1;
+  return launch_gemm_tn(dy_bf16, ld_dy, w_bf16, ldw, TMAP_BF16, s, e, reinterpret_cast<cudaStream_t>(stream), eff_impl());
+}
 int dvt_layerscale_bwd(const float* dx, int ldx, const void* branch_bf16, const float* gamma, void* dbranch_bf16, float* dbias,
                        float* dgamma, float* workspace, int rows, int C, void* stream) {
   return launch_layerscale_bwd(dx, ldx, reinterpret_cast<const __nv_bfloat16*>(branch_bf16), gamma,

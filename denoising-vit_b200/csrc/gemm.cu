@@ -207,6 +207,77 @@ __device__ __forceinline__ void epi_chunk(const GemmEpi& e, const GemmShape& s, 
   }
   }
 
+// SwiGLU backward (mask_mode 2, dvt_gemm_bf16_dgrad_swiglu).  The product is dh = dY . W2 [M, Hh] with Hh = s.N; e.mask is
+// the saved fc1 output hpre [M, 2 Hh] = [g | u] (timm SwiGLUPacked chunk order), e.out receives dhpre bf16 [M, 2 Hh]:
+//   dhpre[m, n] = dh * u * silu'(g),   dhpre[m, n + Hh] = dh * silu(g).
+// silu(g) = g / (1 + exp(-g)) is the expression of swiglu_kernel (the forward); silu'(g) = s + silu(g) (1 - s) with
+// s = 1 / (1 + exp(-g)) stays finite where exp(-g) overflows (s = 0, silu(g) = -0).  Returns (dg, du).
+__device__ __forceinline__ float2 swiglu_bwd(float dh, float g, float u) {
+  const float den = 1.0f + __expf(-g);
+  const float s = 1.0f / den;
+  const float sl = g / den;
+  return make_float2(dh * u * fmaf(sl, 1.0f - s, s), dh * sl);
+}
+
+__device__ __forceinline__ void swiglu_bwd_store1(const GemmEpi& e, int m, int n, int Hh, float dh) {
+  const size_t ri = (size_t)m * e.ldmask, ro = (size_t)m * e.ldo;
+  const float2 d = swiglu_bwd(dh, __bfloat162float(e.mask[ri + n]), __bfloat162float(e.mask[ri + n + Hh]));
+  __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(e.out);
+  o[ro + n] = __float2bfloat16_rn(d.x);
+  o[ro + n + Hh] = __float2bfloat16_rn(d.y);
+}
+
+// epi_chunk of the SwiGLU backward: each lane reads 4 consecutive g and the 4 matching u of 8 rows (all loads issued before
+// any use) and stores 4 columns in each half, both coalesced.  An Hh that is not a multiple of 4 (possible with a padded
+// W2) takes the scalar path everywhere: the second half would not be 8-byte aligned.
+__device__ __forceinline__ void epi_chunk_swiglu_bwd(const GemmEpi& e, const GemmShape& s, const float* scr, int pitch,
+                                                     int lane, int n_base, int m0, bool has_k) {
+  const int col4 = (lane & 7) * 4;
+  const int n = n_base + col4;
+  const int Hh = s.N;
+  if (n >= Hh) return;
+  if ((Hh & 3) == 0) {
+    uint2 gv[8], uv[8];
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const int m = m0 + 4 * jj;
+      if (m < s.M) {
+        const __nv_bfloat16* h = e.mask + (size_t)m * e.ldmask + n;
+        gv[jj] = *reinterpret_cast<const uint2*>(h);
+        uv[jj] = *reinterpret_cast<const uint2*>(h + Hh);
+      }
+    }
+    __nv_bfloat16* outp = reinterpret_cast<__nv_bfloat16*>(e.out);
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const int m = m0 + 4 * jj;
+      if (m >= s.M) continue;
+      float4 x = *reinterpret_cast<const float4*>(scr + ((lane >> 3) + 4 * jj) * pitch + col4);
+      if (!has_k) x = make_float4(0.f, 0.f, 0.f, 0.f);
+      const float2 g01 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&gv[jj].x));
+      const float2 g23 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&gv[jj].y));
+      const float2 u01 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&uv[jj].x));
+      const float2 u23 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&uv[jj].y));
+      const float2 d0 = swiglu_bwd(x.x, g01.x, u01.x), d1 = swiglu_bwd(x.y, g01.y, u01.y);
+      const float2 d2 = swiglu_bwd(x.z, g23.x, u23.x), d3 = swiglu_bwd(x.w, g23.y, u23.y);
+      __nv_bfloat16* o = outp + (size_t)m * e.ldo + n;
+      *reinterpret_cast<uint2*>(o) = make_uint2(pack_bf16x2(d0.x, d1.x), pack_bf16x2(d2.x, d3.x));
+      *reinterpret_cast<uint2*>(o + Hh) = make_uint2(pack_bf16x2(d0.y, d1.y), pack_bf16x2(d2.y, d3.y));
+    }
+  } else {
+#pragma unroll 1
+    for (int jj = 0; jj < 8; ++jj) {
+      const int m = m0 + 4 * jj;
+      if (m >= s.M) continue;
+#pragma unroll 1
+      for (int q = 0; q < 4 && n + q < Hh; ++q) {
+        const float x = scr[((lane >> 3) + 4 * jj) * pitch + col4 + q];
+        swiglu_bwd_store1(e, m, n + q, Hh, has_k ? x : 0.0f);
+      }
+    }
+  }
+}
+
 
 // Tile t of a launch: (split, tile_n, tile_m), split fastest.
 struct TileIdx {
@@ -228,8 +299,9 @@ __device__ __forceinline__ TileIdx tile_of(const GemmShape& s, int bn, int bk) {
 }
 
 // Epilogue of a tile whose fp32 accumulators sit in shared memory ([BM][pitch]): warp w of `nwarps` takes the 32 x 32
-// chunks w, w + nwarps, ...
-template <bool FIT, int BN>
+// chunks w, w + nwarps, ...  GLU: the SwiGLU-backward epilogue (epi_chunk_swiglu_bwd) instead of epi_chunk; a compile-time
+// switch, so that no other instantiation carries its code.
+template <bool FIT, int BN, bool GLU = false>
 __device__ __forceinline__ void epi_tile(const GemmEpi& e, const GemmShape& s, const float* tile, int pitch, int warp,
                                          int nwarps, int lane, int tm, int tn, bool has_k) {
 #pragma unroll 1
@@ -237,13 +309,18 @@ __device__ __forceinline__ void epi_tile(const GemmEpi& e, const GemmShape& s, c
     const int rb = c / (BN / 32), cb = c % (BN / 32);
     const int n_base = tn * BN + cb * 32;
     if (n_base >= s.N || tm * BM + rb * 32 >= s.M) continue;  // whole chunk out of range (warp-uniform)
-    epi_chunk<FIT>(e, s, tile + rb * 32 * pitch + cb * 32, pitch, lane, n_base, tm * BM + rb * 32 + (lane >> 3), has_k);
+    if constexpr (GLU)
+      epi_chunk_swiglu_bwd(e, s, tile + rb * 32 * pitch + cb * 32, pitch, lane, n_base, tm * BM + rb * 32 + (lane >> 3), has_k);
+    else
+      epi_chunk<FIT>(e, s, tile + rb * 32 * pitch + cb * 32, pitch, lane, n_base, tm * BM + rb * 32 + (lane >> 3), has_k);
   }
 }
 
-template <bool TF32, bool A_MN, bool B_MN>
-__global__ void __launch_bounds__(WG_THREADS, 2)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmShape s, GemmEpi e) {
+// Body of the wgmma kernels (below): gemm_wgmma_kernel<TF32, A_MN, B_MN> with the general epilogue and
+// gemm_wgmma_swiglu_bwd_kernel (bf16, B MN-major) with the SwiGLU-backward one.
+template <bool TF32, bool A_MN, bool B_MN, bool GLU>
+__device__ __forceinline__ void wgmma_gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& s,
+                                                const GemmEpi& e) {
   static_assert(!(TF32 && (A_MN || B_MN)), "TF32 wgmma operands are K-major only");
   constexpr int BK = KB_BYTES / (TF32 ? 4 : 2);  // elements of K per stage
   constexpr int A_BYTES = BM * KB_BYTES;
@@ -342,8 +419,21 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     }
   }
   named_bar(1, 256);
-  epi_tile<false, WG_BN>(e, s, tile, EPI_PITCH, warp, 8, lane, ti.tm, ti.tn, ti.kb0 < ti.kb_total);
+  epi_tile<false, WG_BN, GLU>(e, s, tile, EPI_PITCH, warp, 8, lane, ti.tm, ti.tn, ti.kb0 < ti.kb_total);
   if (threadIdx.x == 0) stamp_ts(e, 6);
+}
+
+template <bool TF32, bool A_MN, bool B_MN>
+__global__ void __launch_bounds__(WG_THREADS, 2)
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmShape s, GemmEpi e) {
+  wgmma_gemm_body<TF32, A_MN, B_MN, false>(tmA, tmB, s, e);
+}
+
+// fc2 data gradient of a SwiGLU MLP: dY [M, C] (K-major) . W2 stored [C, Hh] (MN-major), SwiGLU backward in the epilogue
+__global__ void __launch_bounds__(WG_THREADS, 2)
+gemm_wgmma_swiglu_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmShape s,
+                             GemmEpi e) {
+  wgmma_gemm_body<false, false, true, true>(tmA, tmB, s, e);
 }
 
 // ----------------------------------------------------------------------------------------------------
@@ -533,15 +623,20 @@ __global__ void gemm_tn_simt_kernel(const T* __restrict__ A, int lda, const T* _
     __syncthreads();
   }
   if (m < s.M && n < s.N) {
-    epi_post1(e, m, n, epi_pre(e, m, n, acc));
+    if (e.mask_mode == 2) swiglu_bwd_store1(e, m, n, s.N, acc);
+    else epi_post1(e, m, n, epi_pre(e, m, n, acc));
   }
 }
 
-template <bool TF32, bool A_MN, bool B_MN>
+template <bool TF32, bool A_MN, bool B_MN, bool GLU = false>
 int launch_wgmma(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& s, const GemmEpi& e, cudaStream_t stream) {
   const int tiles = ((s.M + BM - 1) / BM) * ((s.N + WG_BN - 1) / WG_BN) * s.splits;
-  DVT_CUDA_OK(launch_kx(LaunchOpt{s.pdl != 0, s.prio_drop}, gemm_wgmma_kernel<TF32, A_MN, B_MN>, dim3(tiles),
-                        dim3(WG_THREADS), (size_t)WG_SMEM, stream, tmA, tmB, s, e));
+  if constexpr (GLU)
+    DVT_CUDA_OK(launch_kx(LaunchOpt{s.pdl != 0, s.prio_drop}, gemm_wgmma_swiglu_bwd_kernel, dim3(tiles), dim3(WG_THREADS),
+                          (size_t)WG_SMEM, stream, tmA, tmB, s, e));
+  else
+    DVT_CUDA_OK(launch_kx(LaunchOpt{s.pdl != 0, s.prio_drop}, gemm_wgmma_kernel<TF32, A_MN, B_MN>, dim3(tiles),
+                          dim3(WG_THREADS), (size_t)WG_SMEM, stream, tmA, tmB, s, e));
   count_launch();
   DVT_CUDA_OK(cudaGetLastError());
   return DVT_OK;
@@ -574,6 +669,7 @@ int gemm_prepare() {
   if ((rc = set_smem(gemm_wgmma_kernel<false, false, false>, WG_SMEM))) return rc;
   if ((rc = set_smem(gemm_wgmma_kernel<false, false, true>, WG_SMEM))) return rc;
   if ((rc = set_smem(gemm_wgmma_kernel<false, true, true>, WG_SMEM))) return rc;
+  if ((rc = set_smem(gemm_wgmma_swiglu_bwd_kernel, WG_SMEM))) return rc;
   if ((rc = set_smem(gemm_x3_kernel<64, false, false>, X3Smem<64>::TOTAL))) return rc;
   if ((rc = set_smem(gemm_x3_kernel<64, false, true>, X3Smem<64>::TOTAL))) return rc;
   if ((rc = set_smem(gemm_x3_kernel<64, true, true>, X3Smem<64>::TOTAL))) return rc;
@@ -610,6 +706,12 @@ int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dty
   epi.last_col_n = epi.last_col_out ? s.N - 1 : -1;
   // the vector post-stage must not straddle the redirected column: keep N-1 in a scalar tail
   DVT_REQUIRE(epi.last_col_out == nullptr || (s.N - 1) % 4 == 0, "gemm: last_col_out needs (N-1) %% 4 == 0 (N=%d)", s.N);
+  const bool glu = epi.mask_mode == 2;
+  DVT_REQUIRE(!glu || (dtype == TMAP_BF16 && !s.a_mn && s.b_mn && !s.x3 && s.splits == 1 && epi.out_mode == OUT_BF16 &&
+                       epi.mask && epi.ldmask % 4 == 0 && epi.ldmask >= 2 * s.N && epi.ldo >= 2 * s.N &&
+                       ((reinterpret_cast<uintptr_t>(epi.mask) | reinterpret_cast<uintptr_t>(epi.out)) & 7) == 0),
+              "gemm: the SwiGLU-backward epilogue needs bf16 A K-major / B MN-major, no split-K, bf16 output and 8-byte "
+              "aligned [M, >= 2N] pre-activation / output with pitches that are multiples of 4");
 
   if (impl == GEMM_SIMT_DEBUG) {
     dim3 grid((s.N + 15) / 16, (s.M + 15) / 16), block(16, 16);
@@ -668,6 +770,7 @@ int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dty
   else rc = make_tmap_2d(&tmB, B, dtype, (uint64_t)s.N, (uint64_t)s.K, (uint64_t)ldb * elem, WG_BN, bk);
   if (rc) return rc;
   if (dtype == TMAP_F32) return launch_wgmma<true, false, false>(tmA, tmB, s, epi, stream);
+  if (glu) return launch_wgmma<false, false, true, true>(tmA, tmB, s, epi, stream);
   if (s.a_mn) return launch_wgmma<false, true, true>(tmA, tmB, s, epi, stream);
   if (s.b_mn) return launch_wgmma<false, false, true>(tmA, tmB, s, epi, stream);
   return launch_wgmma<false, false, false>(tmA, tmB, s, epi, stream);

@@ -26,7 +26,8 @@ struct GemmEpi {
   const float* mask_f32 = nullptr;      // same, fp32 mask tensor
   int ldmask = 0;
   int mask_mode = 0;                  // bf16 `mask` only: 0 = gate (v *= mask > 0), 1 = v *= gelu'(mask)  (GELU backward:
-                                      // `mask` holds the pre-activation of the forward pass)
+                                      // `mask` holds the pre-activation of the forward pass), 2 = SwiGLU backward (`mask`
+                                      // = [g | u] of width 2N, bf16 output of width 2N; its own kernel, gemm.cu)
   float alpha = 1.0f;                 // v *= alpha (after activation / mask)
   // post-stage (coalesced)
   int out_mode = OUT_BF16;

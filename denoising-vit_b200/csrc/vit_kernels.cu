@@ -222,6 +222,17 @@ __global__ void swiglu_kernel(const __nv_bfloat16* __restrict__ hin, __nv_bfloat
   }
 }
 
+// swiglu_kernel on caller-owned tensors (the training forward): the same launch as the inference forward in vit.cu, so both
+// produce the same bits
+int launch_swiglu(const __nv_bfloat16* hin, __nv_bfloat16* out, size_t M, int Hh, cudaStream_t st) {
+  DVT_REQUIRE(hin && out && Hh > 0, "swiglu: bad arguments");
+  if (M == 0) return DVT_OK;
+  swiglu_kernel<<<num_sms() * 8, 256, 0, st>>>(hin, out, M, Hh);
+  DVT_CUDA_OK(cudaGetLastError());
+  count_launch();
+  return DVT_OK;
+}
+
 __global__ void cast_f32_bf16_kernel(const float* __restrict__ in, __nv_bfloat16* __restrict__ out, size_t n) {
   for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (size_t)gridDim.x * blockDim.x)
     out[e] = __float2bfloat16_rn(in[e]);

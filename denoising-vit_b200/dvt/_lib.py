@@ -39,6 +39,9 @@ SIGNATURES = {
                                   c_void_p]),
     "dvt_layernorm_bwd_grouped": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                           c_float, c_int, c_int, c_void_p]),
+    "dvt_swiglu": (c_int, [c_void_p, c_void_p, c_size_t, c_int, c_void_p]),
+    "dvt_gemm_bf16_dgrad_swiglu": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p,
+                                           c_int, c_void_p]),
     "dvt_layernorm": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_int,
                               c_int, c_void_p]),
     "dvt_attention_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),

@@ -4,7 +4,7 @@ executed by libdvt_b200.so (hand-written sm_90a kernels) instead of timm.
 
 Training (stage 3, reference main_distillation.py): after `set_trainable()`, calls made with gradients enabled return a
 differentiable result whose backward is hand-written CUDA too (dvt.train_ops: patch embedding, pre-LN blocks with
-LayerScale, final norm with the prefix strip); `set_grad_checkpointing(True)` makes every block recompute its forward in
+LayerScale and a GELU or SwiGLU MLP, final norm with the prefix strip); `set_grad_checkpointing(True)` makes every block recompute its forward in
 the backward instead of keeping its activations.  Without `set_trainable()` every call is the inference forward.
 
 `self.model` is a parameter container whose state-dict keys are timm's, so checkpoints of the wrapper
@@ -285,8 +285,6 @@ class B200VisionTransformer(nn.Module):
 
     def _run_train(self, x: torch.Tensor, layer_index: int, norm: bool) -> torch.Tensor:
         """Differentiable forward to the [B, h, w, C] map of `layer_index` (prefix tokens stripped)."""
-        if self.arch["swiglu"]:
-            raise NotImplementedError(f"{self.identifier}: the training path has no SwiGLU backward (ViT-g)")
         if not x.is_cuda:
             raise _lib.DvtError("dvt_b200 ViT training needs a CUDA tensor (no CPU fallback)")
         if x.dtype not in (torch.float32, torch.bfloat16):
@@ -448,8 +446,9 @@ class PretrainedViTWrapper(nn.Module):
 
     def set_trainable(self, flag: bool = True):
         """Opt in to the training path (stage-3 distillation): with gradients enabled, `get_intermediate_layers` returns a
-        differentiable result (one layer, no prefix tokens; not for the SwiGLU ViT-g backbones).  Off by default: the
-        frozen-backbone callers keep the inference forward even when their parameters require grad."""
+        differentiable result (one layer, no prefix tokens), for every backbone of `ARCHS`, the SwiGLU ViT-g/14 ones
+        included.  Off by default: the frozen-backbone callers keep the inference forward even when their parameters
+        require grad."""
         self.model._trainable = bool(flag)
         return self
 

@@ -78,6 +78,30 @@ def gelu(x: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def swiglu(hpre: torch.Tensor) -> torch.Tensor:
+    """hpre bf16 [rows, 2 Hh] = [g | u] (timm SwiGLUPacked chunk order) -> silu(g) * u bf16 [rows, Hh]; the kernel of the
+    inference forward, so both produce the same bits."""
+    assert hpre.is_cuda and hpre.dtype == torch.bfloat16 and hpre.is_contiguous() and hpre.dim() == 2 and hpre.shape[1] % 2 == 0
+    rows, Hh = hpre.shape[0], hpre.shape[1] // 2
+    out = torch.empty((rows, Hh), device=hpre.device, dtype=torch.bfloat16)
+    check(lib().dvt_swiglu(ptr(hpre), ptr(out), rows, Hh, cur_stream()), "dvt_swiglu")
+    return out
+
+
+def dgrad_swiglu(dy: torch.Tensor, w2: torch.Tensor, hpre: torch.Tensor) -> torch.Tensor:
+    """Gradient w.r.t. the fc1 output of a SwiGLU MLP: dh = dy [rows, C] @ w2 [C, Hh] (fc2's nn.Linear storage, read as an
+    MN-major operand; a row pitch larger than Hh is allowed), and the SwiGLU backward on hpre [rows, 2 Hh] in the GEMM
+    epilogue -> dhpre bf16 [rows, 2 Hh]."""
+    assert dy.dtype == w2.dtype == hpre.dtype == torch.bfloat16 and dy.is_contiguous() and hpre.is_contiguous()
+    assert w2.stride(1) == 1 and dy.shape[1] == w2.shape[0] and hpre.shape == (dy.shape[0], 2 * w2.shape[1])
+    rows, C = dy.shape
+    Hh = w2.shape[1]
+    out = torch.empty((rows, 2 * Hh), device=dy.device, dtype=torch.bfloat16)
+    check(lib().dvt_gemm_bf16_dgrad_swiglu(ptr(dy), C, ptr(w2), w2.stride(0), rows, Hh, C, ptr(hpre), 2 * Hh, ptr(out), 2 * Hh,
+                                           cur_stream()), "dvt_gemm_bf16_dgrad_swiglu")
+    return out
+
+
 def _sms() -> int:
     return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
 
@@ -364,8 +388,14 @@ def vit_layernorm(x: torch.Tensor, w, b, eps: float = 1e-6) -> torch.Tensor:
     return _VitLayerNormFn.apply(x, w, b, eps)
 
 
+def _is_swiglu(w1: torch.Tensor, w2: torch.Tensor) -> bool:
+    """SwiGLUPacked MLP (ViT-g/14): fc2's input width is half of fc1's output width."""
+    return 2 * w2.shape[1] == w1.shape[0]
+
+
 def _vit_block_fwd(x0, wts, heads: int, batch: int, keep: bool, eps: float = 1e-6):
-    """Forward of one pre-LN ViT block on prepared weights; returns (x2, activations for the backward or None)."""
+    """Forward of one pre-LN ViT block on prepared weights; returns (x2, activations for the backward or None).  The MLP is
+    GELU, or SwiGLU when fc2's input width is half of fc1's output width."""
     n1w, n1b, wq, qkvb, wp, projb, ls1, n2w, n2b, w1, fc1b, w2, fc2b, ls2 = wts
     M, C = x0.shape
     N = M // batch
@@ -379,7 +409,7 @@ def _vit_block_fwd(x0, wts, heads: int, batch: int, keep: bool, eps: float = 1e-
     gemm_tn_residual_ex_(x1, att, wp, projb, ls1, br1)
     xn2 = ops.layernorm(x1, n2w, n2b, eps, out_dtype=torch.bfloat16)
     hpre = ops.gemm_tn(xn2, w1, fc1b, None, torch.bfloat16)
-    hid = gelu(hpre)
+    hid = swiglu(hpre) if _is_swiglu(w1, w2) else gelu(hpre)
     x2 = x1.clone()
     br2 = branch(ls2)
     gemm_tn_residual_ex_(x2, hid, w2, fc2b, ls2, br2)
@@ -387,9 +417,10 @@ def _vit_block_fwd(x0, wts, heads: int, batch: int, keep: bool, eps: float = 1e-
 
 
 class _VitBlockFn(torch.autograd.Function):
-    """timm ViT `Block` (pre-LN attention + GELU MLP, LayerScale ls1 / ls2 when given) forward / backward on the CUDA
-    kernels; bf16 GEMM operands, fp32 residual stream and fp32 master weights, as `_BlockFn`.  Saved for the backward: what
-    `_BlockFn` saves, plus the bf16 pre-LayerScale branch values of the two residual GEMMs (LayerScale blocks only).
+    """timm ViT `Block` (pre-LN attention + GELU or SwiGLUPacked MLP, LayerScale ls1 / ls2 when given) forward / backward on
+    the CUDA kernels; bf16 GEMM operands, fp32 residual stream and fp32 master weights, as `_BlockFn`.  Saved for the
+    backward: what `_BlockFn` saves, plus the bf16 pre-LayerScale branch values of the two residual GEMMs (LayerScale blocks
+    only); for SwiGLU the MLP pair is the fc1 output [g | u] (bf16 [M, 2 Hh]) and silu(g) * u (bf16 [M, Hh]).
     checkpoint=True saves the block input only and recomputes the forward during the backward."""
 
     @staticmethod
@@ -418,10 +449,13 @@ class _VitBlockFn(torch.autograd.Function):
         M, C = x0.shape
         N = M // batch
         dx2 = dx2.detach().float().contiguous()
-        # ---- MLP branch: x2 = x1 + ls2 * (fc2(gelu(fc1(LN2(x1)))) ----
+        # ---- MLP branch: x2 = x1 + ls2 * fc2(act(fc1(LN2(x1)))), act = gelu or swiglu ----
         d2, g_fc2b, g_ls2 = layerscale_bwd(dx2, br2, ls2)
         g_fc2w = wgrad(d2, hid)
-        dhpre = dgrad(d2, w2, torch.bfloat16, gelu_preact=hpre)
+        if _is_swiglu(w1, w2):
+            dhpre = dgrad_swiglu(d2, w2, hpre)
+        else:
+            dhpre = dgrad(d2, w2, torch.bfloat16, gelu_preact=hpre)
         g_fc1w = wgrad(dhpre, xn2)
         g_fc1b = colsum(dhpre)
         dxn2 = dgrad(dhpre, w1, torch.float32)

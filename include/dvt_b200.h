@@ -286,6 +286,15 @@ int dvt_vit_embed_bwd(const float* dx0, int B, int ntok, int prefix, int C, void
  * (the skipped rows are not touched); dgamma / dbeta [C] are overwritten. */
 int dvt_layernorm_bwd_grouped(const float* x, const float* gamma, const float* dy, float* dx_accum, float* dgamma, float* dbeta,
                               float* workspace, int rows, int C, float eps, int in_group, int skip, void* stream);
+/* SwiGLU MLP (timm SwiGLUPacked, ViT-g/14): out [M, Hh] = silu(g) * u with [g | u] = hpre [M, 2 Hh] (bf16, contiguous), the
+ * kernel of the inference forward, so a training forward produces the same bits. */
+int dvt_swiglu(const void* hpre_bf16, void* out_bf16, size_t M, int Hh, void* stream);
+/* fc2 data gradient of a SwiGLU MLP with the SwiGLU backward fused into the epilogue (the fp32 dh never reaches memory):
+ * dh = dy (bf16 [M, K], row pitch ld_dy) . w (fc2 weight, bf16 [K, Hh] in its nn.Linear storage, row pitch ldw), then
+ * dhpre[m, n] = dh * u * silu'(g) and dhpre[m, n + Hh] = dh * silu(g), g = hpre[m, n], u = hpre[m, n + Hh] (the saved fc1
+ * output).  hpre / dhpre bf16 [M, >= 2 Hh], pitches multiples of 4, 8-byte aligned.  Plain stores: deterministic. */
+int dvt_gemm_bf16_dgrad_swiglu(const void* dy_bf16, int ld_dy, const void* w_bf16, int ldw, int M, int Hh, int K,
+                               const void* hpre_bf16, int ld_hpre, void* dhpre_bf16, int ld_dhpre, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * view generation (SURVEY.md 8(f-1), the step in front of HP-1)

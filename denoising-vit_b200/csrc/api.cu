@@ -63,6 +63,13 @@ int launch_layernorm_bwd_grouped(const float* x, const float* gamma, const float
                                  cudaStream_t st);
 int launch_vit_embed_fwd(const __nv_bfloat16* patches, int Kp, const __nv_bfloat16* w, const float* bias, const float* pos_patch,
                          const float* prefix_rows, int B, int np, int prefix, int C, float* out, cudaStream_t st, int impl);
+int launch_attention_bwd_det(const __nv_bfloat16* qkv, const __nv_bfloat16* out, const __nv_bfloat16* dout, const float* lse,
+                             __nv_bfloat16* dqkv, float* delta, int B, int N, int heads, cudaStream_t stream, int head_dim);
+int launch_colsum_ordered(const void* in, bool bf16, int ld, int rows, int cols, float* out, float* workspace, cudaStream_t st);
+int launch_denoise_loss_ordered(const float* pred, const float* tgt, float* dpred, float* losses, float* workspace, int rows,
+                                int C, float grad_scale, cudaStream_t st);
+int launch_resample_bwd(const float* wh, const float* ww, const float* dout, float* tmp, float* dgrid, int h, int w, int gh,
+                        int gw, int C, cudaStream_t st);
 const char* last_error();
 extern int g_debug_impl_override;
 int g_debug_impl_override = -1;
@@ -284,6 +291,48 @@ int dvt_denoise_loss(const float* pred, const float* target, float* dpred, float
 int dvt_adamw(float* p, const float* g, float* m, float* v, size_t n, double lr, double beta1, double beta2, double eps,
               double weight_decay, long long step, void* stream) {
   return launch_adamw(p, g, m, v, n, lr, beta1, beta2, eps, weight_decay, step, reinterpret_cast<cudaStream_t>(stream));
+}
+
+/* ---- deterministic training step (torch.use_deterministic_algorithms) ---- */
+int dvt_attention_bwd_det(const void* qkv_bf16, const void* out_bf16, const void* dout_bf16, const float* lse,
+                          void* dqkv_bf16, float* delta_workspace, int B, int N, int heads, int head_dim, void* stream) {
+  return launch_attention_bwd_det(reinterpret_cast<const __nv_bfloat16*>(qkv_bf16), reinterpret_cast<const __nv_bfloat16*>(out_bf16),
+                                  reinterpret_cast<const __nv_bfloat16*>(dout_bf16), lse, reinterpret_cast<__nv_bfloat16*>(dqkv_bf16),
+                                  delta_workspace, B, N, heads, reinterpret_cast<cudaStream_t>(stream), head_dim);
+}
+int dvt_gemm_bf16_wgrad_ordered(const void* dy_bf16, int ld_dy, const void* x_bf16, int ldx, int M, int N, int K, float* out,
+                                int ldo, int splits, float* workspace, void* stream) {
+  DVT_REQUIRE(dy_bf16 && x_bf16 && out, "dvt_gemm_bf16_wgrad_ordered: null pointer");
+  DVT_REQUIRE(splits == 1 || workspace, "dvt_gemm_bf16_wgrad_ordered: split-K needs the workspace");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  GemmEpi e;
+  e.ldo = ldo;
+  GemmShape s{M, N, K, splits < 1 ? 1 : splits};
+  s.a_mn = 1;
+  s.b_mn = 1;
+  if (s.splits == 1) {
+    e.out = out;
+    e.out_mode = OUT_F32;
+    return launch_gemm_tn(dy_bf16, ld_dy, x_bf16, ldx, TMAP_BF16, s, e, st, eff_impl());
+  }
+  e.out = workspace;
+  e.out_mode = OUT_F32_PLANES;
+  e.out_plane = (size_t)M * ldo;
+  int rc = launch_gemm_tn(dy_bf16, ld_dy, x_bf16, ldx, TMAP_BF16, s, e, st, eff_impl());
+  if (rc) return rc;
+  return launch_splitk_planes_sum(workspace, s.splits, (size_t)M * ldo, M, N, ldo, out, st);
+}
+int dvt_colsum_ordered(const void* in, int dtype, int ld, int rows, int cols, float* out, float* workspace, void* stream) {
+  return launch_colsum_ordered(in, dtype == DVT_DTYPE_BF16, ld, rows, cols, out, workspace, reinterpret_cast<cudaStream_t>(stream));
+}
+int dvt_denoise_loss_ordered(const float* pred, const float* target, float* dpred, float* losses3, float* workspace, int rows,
+                             int C, float grad_scale, void* stream) {
+  return launch_denoise_loss_ordered(pred, target, dpred, losses3, workspace, rows, C, grad_scale,
+                                     reinterpret_cast<cudaStream_t>(stream));
+}
+int dvt_resample_bwd(const float* wh, const float* ww, const float* dout, float* tmp, float* dgrid, int h, int w, int gh, int gw,
+                     int C, void* stream) {
+  return launch_resample_bwd(wh, ww, dout, tmp, dgrid, h, w, gh, gw, C, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int dvt_im2col(const void* x, int x_dtype, void* out_bf16, int B, int H, int W, int P, int S, void* stream) {

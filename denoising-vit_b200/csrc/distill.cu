@@ -19,9 +19,19 @@ static int det_chunks(int rows) { return std::max(1, std::min(kDetChunks, (rows 
 //   part1[chunk] = sum_rows dx * branch.
 // Block = 8 row lanes x 32 column lanes, 4 consecutive columns per thread (128 columns per block); blockIdx.y = row chunk.
 // gamma == NULL: unit scale (cast + sum only); branch == NULL: no part1; dbranch == NULL: no bf16 output.
+// T = bf16: dx is a bf16 matrix (the fixed-order bias gradient of a bf16 dY, dvt_colsum_ordered).
 // ----------------------------------------------------------------------------------------------------
+__device__ __forceinline__ float4 ld_col4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
+__device__ __forceinline__ float4 ld_col4(const __nv_bfloat16* p) {
+  const uint2 v = __ldg(reinterpret_cast<const uint2*>(p));
+  const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&v.x));
+  const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&v.y));
+  return make_float4(a.x, a.y, b.x, b.y);
+}
+
+template <typename T>
 __global__ void __launch_bounds__(256)
-branch_bwd_partial_kernel(const float* __restrict__ dx, int ldx, const __nv_bfloat16* __restrict__ branch,
+branch_bwd_partial_kernel(const T* __restrict__ dx, int ldx, const __nv_bfloat16* __restrict__ branch,
                           const float* __restrict__ gamma, __nv_bfloat16* __restrict__ dbranch, float* __restrict__ part,
                           int rows, int C, int chunks) {
   __shared__ float4 s_b[8][32], s_g[8][32];
@@ -33,7 +43,7 @@ branch_bwd_partial_kernel(const float* __restrict__ dx, int ldx, const __nv_bflo
   if (c < C) {
     const float4 g = gamma ? __ldg(reinterpret_cast<const float4*>(gamma + c)) : make_float4(1.f, 1.f, 1.f, 1.f);
     for (int r = r0 + ty; r < r1; r += 8) {
-      const float4 d = __ldg(reinterpret_cast<const float4*>(dx + (size_t)r * ldx + c));
+      const float4 d = ld_col4(dx + (size_t)r * ldx + c);
       const float4 gd = make_float4(g.x * d.x, g.y * d.y, g.z * d.z, g.w * d.w);
       ab.x += gd.x; ab.y += gd.y; ab.z += gd.z; ab.w += gd.w;
       if (dbranch) {
@@ -95,11 +105,29 @@ int launch_layerscale_bwd(const float* dx, int ldx, const __nv_bfloat16* branch,
   DVT_REQUIRE(C % 4 == 0 && ldx % 4 == 0, "layerscale_bwd: C=%d and ldx=%d must be multiples of 4", C, ldx);
   DVT_REQUIRE(!dgamma || (branch && gamma), "layerscale_bwd: dgamma needs the saved branch and gamma");
   const int chunks = det_chunks(rows);
-  branch_bwd_partial_kernel<<<dim3((C + 127) / 128, chunks), 256, 0, st>>>(dx, ldx, dgamma ? branch : nullptr, gamma, dbranch,
+  branch_bwd_partial_kernel<float><<<dim3((C + 127) / 128, chunks), 256, 0, st>>>(dx, ldx, dgamma ? branch : nullptr, gamma, dbranch,
                                                                           workspace, rows, C, chunks);
   DVT_CUDA_OK(cudaGetLastError());
   count_launch();
   return launch_partial_final(workspace, chunks, C, dbias, dgamma, st);
+}
+
+// Fixed-order column sums out[c] = sum_rows in[r, c] of a bf16 or fp32 [rows, cols] matrix (the bias gradients of the
+// deterministic training step): the partial / final passes of the LayerScale backward without scale or bf16 output.
+int launch_colsum_ordered(const void* in, bool bf16, int ld, int rows, int cols, float* out, float* workspace, cudaStream_t st) {
+  DVT_REQUIRE(in && out && workspace && rows > 0 && cols > 0, "colsum_ordered: bad arguments");
+  DVT_REQUIRE(cols % 4 == 0 && ld % 4 == 0, "colsum_ordered: cols=%d and ld=%d must be multiples of 4", cols, ld);
+  const int chunks = det_chunks(rows);
+  const dim3 grid((cols + 127) / 128, chunks);
+  if (bf16)
+    branch_bwd_partial_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(in), ld, nullptr,
+                                                                  nullptr, nullptr, workspace, rows, cols, chunks);
+  else
+    branch_bwd_partial_kernel<float><<<grid, 256, 0, st>>>(reinterpret_cast<const float*>(in), ld, nullptr, nullptr, nullptr,
+                                                          workspace, rows, cols, chunks);
+  DVT_CUDA_OK(cudaGetLastError());
+  count_launch();
+  return launch_partial_final(workspace, chunks, cols, out, nullptr, st);
 }
 
 // ----------------------------------------------------------------------------------------------------

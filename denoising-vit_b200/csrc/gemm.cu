@@ -316,9 +316,10 @@ __device__ __forceinline__ void epi_tile(const GemmEpi& e, const GemmShape& s, c
   }
 }
 
-// Body of the wgmma kernels (below): gemm_wgmma_kernel<TF32, A_MN, B_MN> with the general epilogue and
-// gemm_wgmma_swiglu_bwd_kernel (bf16, B MN-major) with the SwiGLU-backward one.
-template <bool TF32, bool A_MN, bool B_MN, bool GLU>
+// Body of the wgmma kernels (below): gemm_wgmma_kernel<TF32, A_MN, B_MN> with the general epilogue,
+// gemm_wgmma_swiglu_bwd_kernel (bf16, B MN-major) with the SwiGLU-backward one and gemm_wgmma_planes_kernel (bf16, both
+// MN-major; PLANES: split k stores its partial tile into plane k of e.out, the OUT_F32_PLANES mode).
+template <bool TF32, bool A_MN, bool B_MN, bool GLU, bool PLANES = false>
 __device__ __forceinline__ void wgmma_gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& s,
                                                 const GemmEpi& e) {
   static_assert(!(TF32 && (A_MN || B_MN)), "TF32 wgmma operands are K-major only");
@@ -419,7 +420,14 @@ __device__ __forceinline__ void wgmma_gemm_body(const CUtensorMap& tmA, const CU
     }
   }
   named_bar(1, 256);
-  epi_tile<false, WG_BN, GLU>(e, s, tile, EPI_PITCH, warp, 8, lane, ti.tm, ti.tn, ti.kb0 < ti.kb_total);
+  if constexpr (PLANES) {  // plain fp32 stores into this split's plane
+    GemmEpi ep = e;
+    ep.out_mode = OUT_F32;
+    ep.out = reinterpret_cast<float*>(e.out) + (size_t)(blockIdx.x % s.splits) * e.out_plane;
+    epi_tile<false, WG_BN, false>(ep, s, tile, EPI_PITCH, warp, 8, lane, ti.tm, ti.tn, ti.kb0 < ti.kb_total);
+  } else {
+    epi_tile<false, WG_BN, GLU>(e, s, tile, EPI_PITCH, warp, 8, lane, ti.tm, ti.tn, ti.kb0 < ti.kb_total);
+  }
   if (threadIdx.x == 0) stamp_ts(e, 6);
 }
 
@@ -434,6 +442,13 @@ __global__ void __launch_bounds__(WG_THREADS, 2)
 gemm_wgmma_swiglu_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmShape s,
                              GemmEpi e) {
   wgmma_gemm_body<false, false, true, true>(tmA, tmB, s, e);
+}
+
+// Split-K weight gradient without atomics (OUT_F32_PLANES): A and B MN-major (activations in their [rows, features] storage)
+__global__ void __launch_bounds__(WG_THREADS, 2)
+gemm_wgmma_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmShape s,
+                         GemmEpi e) {
+  wgmma_gemm_body<false, true, true, false, true>(tmA, tmB, s, e);
 }
 
 // ----------------------------------------------------------------------------------------------------
@@ -628,10 +643,13 @@ __global__ void gemm_tn_simt_kernel(const T* __restrict__ A, int lda, const T* _
   }
 }
 
-template <bool TF32, bool A_MN, bool B_MN, bool GLU = false>
+template <bool TF32, bool A_MN, bool B_MN, bool GLU = false, bool PLANES = false>
 int launch_wgmma(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& s, const GemmEpi& e, cudaStream_t stream) {
   const int tiles = ((s.M + BM - 1) / BM) * ((s.N + WG_BN - 1) / WG_BN) * s.splits;
-  if constexpr (GLU)
+  if constexpr (PLANES)
+    DVT_CUDA_OK(launch_kx(LaunchOpt{s.pdl != 0, s.prio_drop}, gemm_wgmma_planes_kernel, dim3(tiles), dim3(WG_THREADS),
+                          (size_t)WG_SMEM, stream, tmA, tmB, s, e));
+  else if constexpr (GLU)
     DVT_CUDA_OK(launch_kx(LaunchOpt{s.pdl != 0, s.prio_drop}, gemm_wgmma_swiglu_bwd_kernel, dim3(tiles), dim3(WG_THREADS),
                           (size_t)WG_SMEM, stream, tmA, tmB, s, e));
   else
@@ -658,7 +676,36 @@ int set_smem(K kern, int bytes) {
   return DVT_OK;
 }
 
+// out[m, n] = sum_k planes[k * plane + m * ldo + n] for k = 0, 1, ... in order (the second step of the ordered split-K)
+__global__ void splitk_planes_sum_kernel(const float* __restrict__ planes, int splits, size_t plane, int M, int N, int ldo,
+                                         float* __restrict__ out) {
+  const int n4 = N >> 2;
+  const size_t total = (size_t)M * n4;
+  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
+    const int m = (int)(e / n4), n = (int)(e - (size_t)m * n4) * 4;
+    const size_t off = (size_t)m * ldo + n;
+    float4 acc = __ldg(reinterpret_cast<const float4*>(planes + off));
+    for (int k = 1; k < splits; ++k) {
+      const float4 v = __ldg(reinterpret_cast<const float4*>(planes + (size_t)k * plane + off));
+      acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+    }
+    *reinterpret_cast<float4*>(out + off) = acc;
+  }
+}
+
 }  // namespace
+
+int launch_splitk_planes_sum(const float* planes, int splits, size_t plane, int M, int N, int ldo, float* out,
+                             cudaStream_t st) {
+  DVT_REQUIRE(planes && out && splits >= 1 && M > 0 && N > 0, "splitk_planes_sum: bad arguments");
+  DVT_REQUIRE(N % 4 == 0 && ldo % 4 == 0 && plane % 4 == 0, "splitk_planes_sum: N, ldo and the plane size must be multiples of 4");
+  const size_t total = (size_t)M * (N / 4);
+  const int blocks = (int)std::min<size_t>((total + 255) / 256, (size_t)num_sms() * 8);
+  splitk_planes_sum_kernel<<<blocks, 256, 0, st>>>(planes, splits, plane, M, N, ldo, out);
+  DVT_CUDA_OK(cudaGetLastError());
+  count_launch();
+  return DVT_OK;
+}
 
 // Opts every instantiation into its dynamic shared memory size.  Called once, outside any stream capture.
 int gemm_prepare() {
@@ -670,6 +717,7 @@ int gemm_prepare() {
   if ((rc = set_smem(gemm_wgmma_kernel<false, false, true>, WG_SMEM))) return rc;
   if ((rc = set_smem(gemm_wgmma_kernel<false, true, true>, WG_SMEM))) return rc;
   if ((rc = set_smem(gemm_wgmma_swiglu_bwd_kernel, WG_SMEM))) return rc;
+  if ((rc = set_smem(gemm_wgmma_planes_kernel, WG_SMEM))) return rc;
   if ((rc = set_smem(gemm_x3_kernel<64, false, false>, X3Smem<64>::TOTAL))) return rc;
   if ((rc = set_smem(gemm_x3_kernel<64, false, true>, X3Smem<64>::TOTAL))) return rc;
   if ((rc = set_smem(gemm_x3_kernel<64, true, true>, X3Smem<64>::TOTAL))) return rc;
@@ -700,7 +748,14 @@ int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dty
   GemmEpi epi = epi_in;
   if (s.splits < 1) s.splits = 1;
   DVT_REQUIRE(s.M > 0 && s.N > 0 && s.K > 0, "gemm: empty shape M=%d N=%d K=%d", s.M, s.N, s.K);
-  DVT_REQUIRE(s.splits == 1 || epi.out_mode == OUT_F32_ATOMIC, "gemm: split-K needs OUT_F32_ATOMIC");
+  DVT_REQUIRE(s.splits == 1 || epi.out_mode == OUT_F32_ATOMIC || epi.out_mode == OUT_F32_PLANES,
+              "gemm: split-K needs OUT_F32_ATOMIC or OUT_F32_PLANES");
+  const bool planes = epi.out_mode == OUT_F32_PLANES;
+  DVT_REQUIRE(!planes || (impl == GEMM_TC && dtype == TMAP_BF16 && s.a_mn && s.b_mn && !s.x3 && epi.out && !epi.bias &&
+                          epi.act == ACT_NONE && !epi.mask && !epi.mask_f32 && epi.alpha == 1.0f && !epi.last_col_out &&
+                          epi.out_plane >= (size_t)s.M * epi.ldo),
+              "gemm: OUT_F32_PLANES needs the tensor-core path, bf16 operands both MN-major, a plain epilogue and planes of at "
+              "least M * ldo elements");
   DVT_REQUIRE(epi.out == nullptr || epi.ldo % 4 == 0, "gemm: ldo must be a multiple of 4 (got %d)", epi.ldo);
   DVT_REQUIRE(epi.last_col_out == nullptr || epi.out_mode == OUT_F32_ATOMIC, "gemm: last_col_out needs OUT_F32_ATOMIC");
   epi.last_col_n = epi.last_col_out ? s.N - 1 : -1;
@@ -771,6 +826,7 @@ int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dty
   if (rc) return rc;
   if (dtype == TMAP_F32) return launch_wgmma<true, false, false>(tmA, tmB, s, epi, stream);
   if (glu) return launch_wgmma<false, false, true, true>(tmA, tmB, s, epi, stream);
+  if (planes) return launch_wgmma<false, true, true, false, true>(tmA, tmB, s, epi, stream);
   if (s.a_mn) return launch_wgmma<false, true, true>(tmA, tmB, s, epi, stream);
   if (s.b_mn) return launch_wgmma<false, false, true>(tmA, tmB, s, epi, stream);
   return launch_wgmma<false, false, false>(tmA, tmB, s, epi, stream);

@@ -13,6 +13,8 @@ enum GemmOut {
   OUT_F32_RESID = 3,   // out[m, n] += gamma[n] * v         (fp32 residual stream, in place; gamma may be null)
   OUT_F32_REMAP = 4,   // out[remap(m), n] = v + addend[m % rows_per_group, n]   (patch-embed -> token rows)
   OUT_F32_SPLIT = 5,   // out[m, n] = tf32_hi(v), out[out_plane + m*ldo + n] = v - tf32_hi(v)   (operand of an x3 GEMM)
+  OUT_F32_PLANES = 6,  // out[split * out_plane + m*ldo + n] = v   (split-K partials, plain stores, one plane per split;
+                       // bf16 wgmma with both operands MN-major only: its own kernel, gemm.cu)
 };
 
 // fp32 value -> (hi, lo) with hi exactly representable in TF32 (low 13 mantissa bits zero) and hi + lo == v exactly
@@ -33,7 +35,7 @@ struct GemmEpi {
   int out_mode = OUT_BF16;
   void* out = nullptr;
   int ldo = 0;
-  size_t out_plane = 0;               // OUT_F32_SPLIT: element offset of the lo plane
+  size_t out_plane = 0;               // OUT_F32_SPLIT: element offset of the lo plane; OUT_F32_PLANES: between split planes
   unsigned long long* debug_ts = nullptr;  // optional [8]: globaltimer (ns) milestones of CTA 0 (profiling aid)
   int last_col_n = -1;                // = N-1 when last_col_out is set (filled in by launch_gemm)
   float* last_col_out = nullptr;      // OUT_F32_ATOMIC only: column N-1 is accumulated into last_col_out[m] instead
@@ -207,6 +209,9 @@ enum GemmImpl { GEMM_TC = 0 /* tensor cores: wgmma, mma.sync for 3xTF32 */, GEMM
 int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dtype, const GemmShape& shape,
                    const GemmEpi& epi, cudaStream_t stream, int impl = -1 /* -1: process default */);
 
+// out [M, N] (row pitch ldo) = the `splits` fp32 planes of an OUT_F32_PLANES GEMM summed in split order
+int launch_splitk_planes_sum(const float* planes, int splits, size_t plane, int M, int N, int ldo, float* out,
+                             cudaStream_t st);
 int default_gemm_impl();
 int gemm_prepare();
 int gemm_x3_tile_n(int N, int wide_min_n);  // 64 or 128: tile width launch_gemm_tn picks for a 3xTF32 product

@@ -206,8 +206,10 @@ int launch_gelu(const __nv_bfloat16* in, __nv_bfloat16* out, size_t n, cudaStrea
 //   l2 = mean_{rows, C} (pred - tgt)^2,   cos = 1 - mean_rows <pred, tgt> / (max(|pred|, 1e-8) max(|tgt|, 1e-8))
 //   dpred = grad_scale * [ 2 (pred - tgt) / (rows C)  -  (tgt / (|p||t|) - cos_r pred / |p|^2) / rows ]
 // losses[0..2] += (l2 + cos, l2, cos) contributions (zeroed by the caller).
+// ORDERED: CTA k writes its (l2, cos) pair to losses[2 k], losses[2 k + 1] (a workspace) instead; loss_final_kernel adds
+// the pairs in CTA order (the fixed-order loss of the deterministic training step).
 // ----------------------------------------------------------------------------------------------------
-template <int NV>
+template <int NV, bool ORDERED = false>
 __global__ void __launch_bounds__(256)
 denoise_loss_kernel(const float* __restrict__ pred, const float* __restrict__ tgt, float* __restrict__ dpred,
                     float* __restrict__ losses, int rows, int C, float grad_scale) {
@@ -278,10 +280,28 @@ denoise_loss_kernel(const float* __restrict__ pred, const float* __restrict__ tg
       l2 += s_part[k][0];
       cs += s_part[k][1];
     }
-    atomicAdd(losses + 0, l2 + cs);
-    atomicAdd(losses + 1, l2);
-    atomicAdd(losses + 2, cs);
+    if constexpr (ORDERED) {
+      losses[2 * blockIdx.x] = l2;
+      losses[2 * blockIdx.x + 1] = cs;
+    } else {
+      atomicAdd(losses + 0, l2 + cs);
+      atomicAdd(losses + 1, l2);
+      atomicAdd(losses + 2, cs);
+    }
   }
+}
+
+// losses[1] = sum_k part[2 k], losses[2] = sum_k part[2 k + 1] (k ascending), losses[0] = losses[1] + losses[2]
+__global__ void loss_final_kernel(const float* __restrict__ part, int n, float* __restrict__ losses) {
+  if (threadIdx.x != 0) return;
+  float l2 = 0.f, cs = 0.f;
+  for (int k = 0; k < n; ++k) {
+    l2 += part[2 * k];
+    cs += part[2 * k + 1];
+  }
+  losses[0] = l2 + cs;
+  losses[1] = l2;
+  losses[2] = cs;
 }
 
 int launch_denoise_loss(const float* pred, const float* tgt, float* dpred, float* losses, int rows, int C, float grad_scale,
@@ -301,6 +321,67 @@ int launch_denoise_loss(const float* pred, const float* tgt, float* dpred, float
   DVT_CUDA_OK(cudaGetLastError());
   count_launch();
   return DVT_OK;
+}
+
+// Fixed-order form of launch_denoise_loss: the same per-row arithmetic and dpred; workspace f32 [2 * ceil(rows / 8)].
+int launch_denoise_loss_ordered(const float* pred, const float* tgt, float* dpred, float* losses, float* workspace, int rows,
+                                int C, float grad_scale, cudaStream_t st) {
+  DVT_REQUIRE(pred && tgt && losses && workspace && rows > 0, "denoise_loss_ordered: bad arguments");
+  DVT_REQUIRE(C % 4 == 0 && C <= 2048, "denoise_loss_ordered: C=%d unsupported", C);
+  const int nv = (C / 4 + 31) / 32;
+  const int blocks = std::min(num_sms() * 4, (rows + 7) / 8);
+#define DVT_DL(NV) denoise_loss_kernel<NV, true><<<blocks, 256, 0, st>>>(pred, tgt, dpred, workspace, rows, C, grad_scale)
+  if (nv <= 3) DVT_DL(3);
+  else if (nv <= 6) DVT_DL(6);
+  else if (nv <= 8) DVT_DL(8);
+  else if (nv <= 12) DVT_DL(12);
+  else DVT_DL(16);
+#undef DVT_DL
+  DVT_CUDA_OK(cudaGetLastError());
+  count_launch();
+  loss_final_kernel<<<1, 32, 0, st>>>(workspace, blocks, losses);
+  DVT_CUDA_OK(cudaGetLastError());
+  count_launch();
+  return DVT_OK;
+}
+
+// ----------------------------------------------------------------------------------------------------
+// Backward of the position-embedding resampling (bicubic, antialias; separable): with the exact fp32 weight matrices
+// Wh [h, gh] and Ww [w, gw] of the forward, dgrid[i, j, c] = sum_y sum_x Wh[y, i] Ww[x, j] dout[y, x, c], one axis per
+// pass.  One thread per output element sums over its axis in index order: a fixed order, no atomics.
+//   dst[o, i, k] = sum_{y < n_out} W[y, i] src[o, y, k]   (src [outer, n_out, inner], dst [outer, n_in, inner])
+// ----------------------------------------------------------------------------------------------------
+__global__ void resample_axis_bwd_kernel(const float* __restrict__ W, int n_out, int n_in, const float* __restrict__ src,
+                                         int outer, int inner, float* __restrict__ dst) {
+  const size_t total = (size_t)outer * n_in * inner;
+  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
+    const int k = (int)(e % inner);
+    const size_t oi = e / inner;
+    const int i = (int)(oi % n_in), o = (int)(oi / n_in);
+    const float* sp = src + (size_t)o * n_out * inner + k;
+    float acc = 0.f;
+    for (int y = 0; y < n_out; ++y) acc = fmaf(__ldg(W + (size_t)y * n_in + i), __ldg(sp + (size_t)y * inner), acc);
+    dst[e] = acc;
+  }
+}
+
+static int launch_resample_axis_bwd(const float* W, int n_out, int n_in, const float* src, int outer, int inner, float* dst,
+                                    cudaStream_t st) {
+  const size_t total = (size_t)outer * n_in * inner;
+  const int blocks = (int)std::min<size_t>((total + 255) / 256, (size_t)num_sms() * 16);
+  resample_axis_bwd_kernel<<<blocks, 256, 0, st>>>(W, n_out, n_in, src, outer, inner, dst);
+  DVT_CUDA_OK(cudaGetLastError());
+  count_launch();
+  return DVT_OK;
+}
+
+int launch_resample_bwd(const float* wh, const float* ww, const float* dout, float* tmp, float* dgrid, int h, int w, int gh,
+                        int gw, int C, cudaStream_t st) {
+  DVT_REQUIRE(wh && ww && dout && tmp && dgrid, "resample_bwd: null argument");
+  DVT_REQUIRE(h > 0 && w > 0 && gh > 0 && gw > 0 && C > 0, "resample_bwd: bad shape h=%d w=%d gh=%d gw=%d C=%d", h, w, gh, gw, C);
+  int rc = launch_resample_axis_bwd(wh, h, gh, dout, 1, w * C, tmp, st);   // tmp [gh, w, C]
+  if (rc) return rc;
+  return launch_resample_axis_bwd(ww, w, gw, tmp, gh, C, dgrid, st);     // dgrid [gh, gw, C]
 }
 
 // ----------------------------------------------------------------------------------------------------

@@ -42,6 +42,13 @@ SIGNATURES = {
     "dvt_swiglu": (c_int, [c_void_p, c_void_p, c_size_t, c_int, c_void_p]),
     "dvt_gemm_bf16_dgrad_swiglu": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p,
                                            c_int, c_void_p]),
+    "dvt_attention_bwd_det": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                      c_void_p]),
+    "dvt_gemm_bf16_wgrad_ordered": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int,
+                                            c_void_p, c_void_p]),
+    "dvt_colsum_ordered": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "dvt_denoise_loss_ordered": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
+    "dvt_resample_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "dvt_layernorm": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_int,
                               c_int, c_void_p]),
     "dvt_attention_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),

@@ -113,7 +113,7 @@ class Denoiser(nn.Module):
         if (h, w) == (gh, gw):
             return self.pos_embed.float()
         g = self.pos_embed.float().reshape(1, gh, gw, -1).permute(0, 3, 1, 2)
-        g = F.interpolate(g, size=(h, w), mode="bicubic", antialias=True)
+        g = train_ops.resample_bicubic(g, h, w)
         return g.permute(0, 2, 3, 1).reshape(1, h * w, -1)
 
     def forward(self, x, return_dict=False, return_channel_first=False, return_class_token=False, norm=True):

@@ -270,7 +270,7 @@ class B200VisionTransformer(nn.Module):
         if (h, w) != (gh, gw):
             C = grid.shape[-1]
             g = grid.reshape(1, gh, gw, C).permute(0, 3, 1, 2)
-            g = F.interpolate(g, size=(h, w), mode="bicubic", antialias=True)
+            g = train_ops.resample_bicubic(g, h, w)
             grid = g.permute(0, 2, 3, 1).reshape(1, h * w, C)
         cls = self.cls_token.float()[0]
         if not self.no_embed_class:

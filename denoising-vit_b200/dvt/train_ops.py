@@ -2,14 +2,20 @@
 two autograd functions the training step is made of -- the denoiser block (`block_forward`) and the distillation loss
 (`denoise_loss`).  Every kernel behind them is hand-written sm_90a code of libdvt_b200.so; torch only owns the tensors.
 
+Deterministic training: when `torch.are_deterministic_algorithms_enabled()` is true at call time, the helpers that
+reduce with float atomics (`attention_bwd`, `wgrad`, `colsum`, `layernorm_bwd_`, the loss) and the position-embedding
+resample (`resample_bicubic`) run fixed-order kernels instead, so that two runs from the same seed on the same GPU model
+give bit-identical weights, optimiser moments and losses.  The flag is read at every call.
+
 Reference step (main_denoiser.py:213-220): pred = model(original_feats); loss = mse(pred, denoised) + 1 - mean cosine;
 loss.backward(); AdamW.step() -- through timm `Block` (pre-LN attention + GELU MLP, no LayerScale)."""
 from __future__ import annotations
 
 import ctypes
-from typing import Tuple
+from typing import Dict, Tuple
 
 import torch
+import torch.nn.functional as F
 
 from . import _lib, ops
 from ._lib import DT_BF16, DT_F32, check, cur_stream, lib, ptr
@@ -17,6 +23,10 @@ from ._lib import DT_BF16, DT_F32, check, cur_stream, lib, ptr
 
 def _dt(t: torch.Tensor) -> int:
     return DT_BF16 if t.dtype == torch.bfloat16 else DT_F32
+
+
+def _deterministic() -> bool:
+    return torch.are_deterministic_algorithms_enabled()
 
 
 def attention_fwd_lse(qkv: torch.Tensor, heads: int, head_dim: int = 64) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -40,8 +50,12 @@ def attention_bwd(qkv: torch.Tensor, out: torch.Tensor, dout: torch.Tensor, lse:
     assert qkv.dtype == out.dtype == dout.dtype == torch.bfloat16 and lse.dtype == torch.float32
     B, N, _ = qkv.shape
     dqkv = torch.empty_like(qkv)
-    dq_ws = torch.empty((B, N, heads * head_dim), device=qkv.device, dtype=torch.float32)
     delta = torch.empty((B, heads, N), device=qkv.device, dtype=torch.float32)
+    if _deterministic():   # dQ from the query-major kernel, no atomics (dK / dV bits unchanged)
+        check(lib().dvt_attention_bwd_det(ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(dqkv), ptr(delta), B, N, heads, head_dim,
+                                          cur_stream()), "dvt_attention_bwd_det")
+        return dqkv
+    dq_ws = torch.empty((B, N, heads * head_dim), device=qkv.device, dtype=torch.float32)
     if head_dim == 64:
         check(lib().dvt_attention_bwd(ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(dqkv), ptr(dq_ws), ptr(delta), B, N, heads,
                                       cur_stream()), "dvt_attention_bwd")
@@ -53,6 +67,8 @@ def attention_bwd(qkv: torch.Tensor, out: torch.Tensor, dout: torch.Tensor, lse:
 
 def layernorm_bwd_(dx_accum: torch.Tensor, x: torch.Tensor, gamma: torch.Tensor, dy: torch.Tensor, eps: float = 1e-6):
     """dx_accum += dLN/dx; returns (dgamma, dbeta).  x, dy, dx_accum f32 [rows, C] contiguous."""
+    if _deterministic():   # the grouped kernel with one row per group is the fixed-order form (same per-row arithmetic)
+        return layernorm_bwd_grouped_(dx_accum, x, gamma, dy, 1, 0, eps)
     rows, C = x.shape
     assert all(t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() for t in (dx_accum, x, dy)) and dy.shape == x.shape
     g = gamma.detach().float().contiguous()
@@ -66,6 +82,11 @@ def layernorm_bwd_(dx_accum: torch.Tensor, x: torch.Tensor, gamma: torch.Tensor,
 def colsum(t: torch.Tensor) -> torch.Tensor:
     """Column sums of a [rows, cols] bf16 / f32 matrix as f32 [cols] (bias gradients)."""
     assert t.is_cuda and t.dim() == 2 and t.stride(1) == 1
+    if _deterministic():
+        out = torch.empty(t.shape[1], device=t.device, dtype=torch.float32)
+        check(lib().dvt_colsum_ordered(ptr(t), _dt(t), t.stride(0), t.shape[0], t.shape[1], ptr(out),
+                                       ptr(_workspace(t.shape[1], t.device)), cur_stream()), "dvt_colsum_ordered")
+        return out
     out = torch.zeros(t.shape[1], device=t.device, dtype=torch.float32)
     check(lib().dvt_colsum(ptr(t), _dt(t), t.stride(0), t.shape[0], t.shape[1], ptr(out), cur_stream()), "dvt_colsum")
     return out
@@ -119,15 +140,27 @@ def dgrad(dy: torch.Tensor, w: torch.Tensor, out_dtype: torch.dtype, gelu_preact
     return out
 
 
+def wgrad_splits(rows: int, n_out: int, n_in: int) -> int:
+    """Split-K factor of `wgrad`: enough CTAs to fill the GPU, at least 4 k-blocks of 64 rows per split."""
+    wide = n_in >= 256 and (n_in % 256 == 0 or n_in > 1024)
+    tiles = ((n_out + 127) // 128) * ((n_in + (255 if wide else 127)) // (256 if wide else 128))
+    return max(1, min(_sms() // max(tiles, 1), ((rows + 63) // 64) // 4))
+
+
 def wgrad(dy: torch.Tensor, x: torch.Tensor) -> torch.Tensor:
     """dW [out, in] f32 = dy [rows, out]^T @ x [rows, in]: both activations are read in place as MN-major operands; the
-    reduction over the rows is split across CTAs (f32 atomics) so that the small output fills the GPU."""
+    reduction over the rows is split across CTAs (f32 atomics) so that the small output fills the GPU.  Deterministic
+    mode: each split stores its partial product into its own workspace plane, and the planes are added in split order."""
     assert dy.dtype == x.dtype == torch.bfloat16 and dy.is_contiguous() and x.is_contiguous() and dy.shape[0] == x.shape[0]
     rows, n_out = dy.shape
     n_in = x.shape[1]
-    wide = n_in >= 256 and (n_in % 256 == 0 or n_in > 1024)
-    tiles = ((n_out + 127) // 128) * ((n_in + (255 if wide else 127)) // (256 if wide else 128))
-    splits = max(1, min(_sms() // max(tiles, 1), ((rows + 63) // 64) // 4))
+    splits = wgrad_splits(rows, n_out, n_in)
+    if _deterministic():
+        out = torch.empty((n_out, n_in), device=dy.device, dtype=torch.float32)
+        ws = torch.empty(splits * n_out * n_in, device=dy.device, dtype=torch.float32) if splits > 1 else None
+        check(lib().dvt_gemm_bf16_wgrad_ordered(ptr(dy), n_out, ptr(x), n_in, n_out, n_in, rows, ptr(out), n_in, splits, ptr(ws),
+                                                cur_stream()), "dvt_gemm_bf16_wgrad_ordered")
+        return out
     out = (torch.zeros if splits > 1 else torch.empty)((n_out, n_in), device=dy.device, dtype=torch.float32)
     check(lib().dvt_gemm_bf16_bwd(ptr(dy), n_out, 1, ptr(x), n_in, 1, n_out, n_in, rows, ptr(out), n_in, DT_F32, splits, None, 0,
                                   cur_stream()), "dvt_gemm_bf16_bwd(wgrad)")
@@ -225,7 +258,13 @@ class _LossFn(torch.autograd.Function):
         t = target.detach().float().contiguous().view(-1, C)
         dpred = torch.empty_like(p)
         losses = torch.empty(3, device=p.device, dtype=torch.float32)
-        check(lib().dvt_denoise_loss(ptr(p), ptr(t), ptr(dpred), ptr(losses), p.shape[0], C, 1.0, cur_stream()), "dvt_denoise_loss")
+        rows = p.shape[0]
+        if _deterministic():   # per-CTA partials added in CTA order
+            ws = torch.empty(2 * ((rows + 7) // 8), device=p.device, dtype=torch.float32)
+            check(lib().dvt_denoise_loss_ordered(ptr(p), ptr(t), ptr(dpred), ptr(losses), ptr(ws), rows, C, 1.0, cur_stream()),
+                  "dvt_denoise_loss_ordered")
+        else:
+            check(lib().dvt_denoise_loss(ptr(p), ptr(t), ptr(dpred), ptr(losses), rows, C, 1.0, cur_stream()), "dvt_denoise_loss")
         ctx.save_for_backward(dpred)
         ctx.shape = pred.shape
         return losses[0], losses[1], losses[2]
@@ -240,6 +279,59 @@ class _LossFn(torch.autograd.Function):
 def denoise_loss(pred: torch.Tensor, target: torch.Tensor):
     """(loss, l2_loss, cosine_similarity_loss) of main_denoiser.py:214-217 in one kernel; differentiable w.r.t. pred."""
     return _LossFn.apply(pred, target)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# position-embedding resampling (timm resample_abs_pos_embed: bicubic, antialias, fp32)
+# ---------------------------------------------------------------------------------------------------------------------
+_RESAMPLE_W: Dict[tuple, torch.Tensor] = {}
+
+
+def resample_weights(n_in: int, n_out: int, device) -> torch.Tensor:
+    """fp32 [n_out, n_in] weights of F.interpolate(bicubic, antialias=True) along one axis (the op is separable with the same
+    1-D weights on both axes), read off ATen itself: a one-hot basis [n_in, 1, n_in] interpolated along its width, the
+    height at size 1 -> 1 (the identity).  (A basis along the height with the width at 1 -> 1 does not reproduce the 2-D
+    op.)  Cached per shape and device."""
+    key = (n_in, n_out, str(device))
+    w = _RESAMPLE_W.get(key)
+    if w is None:
+        with torch.no_grad():
+            eye = torch.eye(n_in, device=device, dtype=torch.float32).reshape(1, n_in, 1, n_in)
+            w = F.interpolate(eye, size=(1, n_out), mode="bicubic", antialias=True)[0, :, 0, :].t().contiguous()
+        _RESAMPLE_W[key] = w
+    return w
+
+
+class _ResampleFn(torch.autograd.Function):
+    """F.interpolate(g, (h, w), bicubic, antialias) with a fixed-order backward: the forward is torch's (same bits), the
+    backward contracts dout with the exact weight matrices of both axes on the CUDA kernel of dvt_resample_bwd."""
+
+    @staticmethod
+    def forward(ctx, g, h: int, w: int):
+        ctx.meta = (tuple(g.shape), h, w)
+        return F.interpolate(g, size=(h, w), mode="bicubic", antialias=True)
+
+    @staticmethod
+    def backward(ctx, dout):
+        (_, C, gh, gw), h, w = ctx.meta
+        if not dout.is_cuda:
+            raise _lib.DvtError("dvt_b200 resample backward needs CUDA tensors (no CPU fallback)")
+        dev = dout.device
+        wh, ww = resample_weights(gh, h, dev), resample_weights(gw, w, dev)
+        d = dout.detach().float()[0].permute(1, 2, 0).contiguous()          # [h, w, C]
+        tmp = torch.empty((gh, w, C), device=dev, dtype=torch.float32)
+        dgrid = torch.empty((gh, gw, C), device=dev, dtype=torch.float32)
+        check(lib().dvt_resample_bwd(ptr(wh), ptr(ww), ptr(d), ptr(tmp), ptr(dgrid), h, w, gh, gw, C, cur_stream()),
+              "dvt_resample_bwd")
+        return dgrid.permute(2, 0, 1).unsqueeze(0), None, None
+
+
+def resample_bicubic(g: torch.Tensor, h: int, w: int) -> torch.Tensor:
+    """g [1, C, gh, gw] fp32 -> F.interpolate(g, (h, w), bicubic, antialias=True), differentiable; in deterministic mode the
+    backward is the fixed-order kernel (torch's CUDA backward of this op adds with atomics)."""
+    if _deterministic():
+        return _ResampleFn.apply(g, h, w)
+    return F.interpolate(g, size=(h, w), mode="bicubic", antialias=True)
 
 
 # ---------------------------------------------------------------------------------------------------------------------

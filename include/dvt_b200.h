@@ -297,6 +297,33 @@ int dvt_gemm_bf16_dgrad_swiglu(const void* dy_bf16, int ld_dy, const void* w_bf1
                                const void* hpre_bf16, int ld_hpre, void* dhpre_bf16, int ld_dhpre, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * Deterministic training step (stages 2 and 3 under torch.use_deterministic_algorithms): fixed-order replacements of
+ * every float-atomic reduction of the backward.  Same inputs and outputs as the calls they replace; repeated calls on
+ * the same GPU model give bit-identical results.  No kernel waits on another CTA.
+ * ------------------------------------------------------------------------------------------------------- */
+/* dvt_attention_bwd_hd without float atomics: dK / dV come from the same key-major kernel (bit-identical to
+ * dvt_attention_bwd_hd's), dQ from a query-major kernel that keeps it in registers over all key tiles and writes it once
+ * (bf16).  No dQ workspace; delta_workspace f32 [B, heads, N]. */
+int dvt_attention_bwd_det(const void* qkv_bf16, const void* out_bf16, const void* dout_bf16, const float* lse,
+                          void* dqkv_bf16, float* delta_workspace, int B, int N, int heads, int head_dim, void* stream);
+/* Weight gradient out [M, N] f32 (row pitch ldo, overwritten) = dy^T . x with dy bf16 [K, M] and x bf16 [K, N] read in
+ * their [rows, features] storage (row pitches ld_dy, ldx).  splits > 1: split s of the K range writes its partial product
+ * with plain stores into plane s of workspace (f32 [splits, M, ldo]), then the planes are added in split order. */
+int dvt_gemm_bf16_wgrad_ordered(const void* dy_bf16, int ld_dy, const void* x_bf16, int ldx, int M, int N, int K, float* out,
+                                int ldo, int splits, float* workspace, void* stream);
+/* out[c] = sum_r in[r, c] (overwritten) in a fixed order; in bf16 or f32 [rows, cols], cols and ld multiples of 4;
+ * workspace f32 [256 * cols]. */
+int dvt_colsum_ordered(const void* in, int dtype, int ld, int rows, int cols, float* out, float* workspace, void* stream);
+/* dvt_denoise_loss with per-CTA partials added in a fixed order (losses3 overwritten); workspace f32 [2 * ceil(rows / 8)]. */
+int dvt_denoise_loss_ordered(const float* pred, const float* target, float* dpred, float* losses3, float* workspace, int rows,
+                             int C, float grad_scale, void* stream);
+/* Backward of a separable resampling of a [gh, gw, C] grid to [h, w, C] (the bicubic antialiased position-embedding
+ * resample) with the forward's fp32 weight matrices wh [h, gh] and ww [w, gw]: dgrid [gh, gw, C] (overwritten) =
+ * sum_y sum_x wh[y, i] ww[x, j] dout[y, x, :]; tmp f32 [gh, w, C]. */
+int dvt_resample_bwd(const float* wh, const float* ww, const float* dout, float* tmp, float* dgrid, int h, int w, int gh, int gw,
+                     int C, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * view generation (SURVEY.md 8(f-1), the step in front of HP-1)
  * Replaces RandomResizedCropFlip.forward (dvt/dataset/transform.py:39-76) + the 8-worker DataLoader of
  * main_img_denoising.py:277-310.  image: device f32 [3, H, W] (already normalised).  boxes_host: HOST int32 [V, 4] =

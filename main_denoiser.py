@@ -76,6 +76,9 @@ def get_args(argv=None):
                         help="train from the in-memory stacks written by main_img_denoising.py --collate_out")
     parser.add_argument("--resume", type=str, default=None, help="checkpoint to continue from (e.g. .../latest.pth)")
     parser.add_argument("--log_freq", default=50, type=int)
+    parser.add_argument("--deterministic", action="store_true",
+                        help="torch.use_deterministic_algorithms(True): fixed-order backward kernels, so that a rerun from "
+                             "the same seed on the same GPU model gives bit-identical weights and losses")
     args = parser.parse_args(argv)
 
     if isinstance(args.input_size, int):
@@ -124,6 +127,8 @@ def main(args):
         os.makedirs(f"{log_dir}/checkpoints", exist_ok=True)
         print("\n".join(f"{k}: {v}" for k, v in sorted(vars(args).items())))
     misc.fix_random_seeds(args.seed)
+    if args.deterministic:
+        torch.use_deterministic_algorithms(True)
 
     # the backbone is needed for its geometry only (the reference builds it, reads patch size / width and deletes it)
     m = re.search(r"patch(\d+)", args.model)

@@ -83,6 +83,9 @@ def get_args(argv=None):
     # H100 extensions (not reference flags)
     parser.add_argument("--resume", type=str, default=None, help="checkpoint to continue from (e.g. .../latest.pth)")
     parser.add_argument("--log_freq", default=50, type=int)
+    parser.add_argument("--deterministic", action="store_true",
+                        help="torch.use_deterministic_algorithms(True): fixed-order backward kernels, so that a rerun from "
+                             "the same seed on the same GPU model gives bit-identical weights and losses")
     args = parser.parse_args(argv)
 
     if isinstance(args.input_size, int):
@@ -130,6 +133,8 @@ def main(args):
         os.makedirs(f"{log_dir}/checkpoints", exist_ok=True)
         print("\n".join(f"{k}: {v}" for k, v in sorted(vars(args).items())))
     misc.fix_random_seeds(args.seed)
+    if args.deterministic:
+        torch.use_deterministic_algorithms(True)
 
     # ---- models (:117-151) ----
     model = DVT.PretrainedViTWrapper(model_identifier=args.model, stride=args.stride_size)

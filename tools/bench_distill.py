@@ -96,7 +96,16 @@ def main():
     ap.add_argument("--arms", choices=("both", "plain", "ckpt"), default="both",
                     help="run the plain step, the gradient-checkpointed step or both (ViT-g at batch 32 and 518 x 518 only "
                          "fits with checkpointing)")
+    ap.add_argument("--deterministic", action="store_true",
+                    help="torch.use_deterministic_algorithms(True): the fixed-order backward kernels")
+    ap.add_argument("--no-empty-fill", action="store_true",
+                    help="with --deterministic: skip torch's NaN fill of torch.empty (measures what that fill costs)")
     a = ap.parse_args()
+    if a.deterministic:
+        torch.use_deterministic_algorithms(True)
+        if a.no_empty_fill:
+            torch.utils.deterministic.fill_uninitialized_memory = False
+        print(f"deterministic mode (NaN fill of empty tensors: {not a.no_empty_fill})")
     rank, world, local = (int(os.environ.get(k, d)) for k, d in (("RANK", "0"), ("WORLD_SIZE", "1"), ("LOCAL_RANK", "0")))
     assert torch.cuda.is_available(), "bench_distill needs a CUDA device"
     torch.cuda.set_device(local)

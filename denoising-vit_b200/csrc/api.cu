@@ -70,6 +70,12 @@ int launch_denoise_loss_ordered(const float* pred, const float* tgt, float* dpre
                                 int C, float grad_scale, cudaStream_t st);
 int launch_resample_bwd(const float* wh, const float* ww, const float* dout, float* tmp, float* dgrid, int h, int w, int gh,
                         int gw, int C, cudaStream_t st);
+int launch_seg_upsample_ce(const float* logits, int B, int h, int w, int K, const uint8_t* labels, int H, int W,
+                           float grad_scale, float* loss_out, float* dlogits, double* workspace, cudaStream_t st);
+int launch_seg_slide_accumulate(const float* logits, int h, int w, int K, int y1, int x1, int wh, int ww, float* acc,
+                                float* count, int Hc, int Wc, cudaStream_t st);
+int launch_seg_predict_hist(float* acc, const float* count, int K, int Hc, int Wc, const uint8_t* labels, int Ho, int Wo,
+                            unsigned long long* hist, cudaStream_t st);
 const char* last_error();
 extern int g_debug_impl_override;
 int g_debug_impl_override = -1;
@@ -507,6 +513,21 @@ int dvt_view_crops(const float* image, int H, int W, const int* boxes_host, cons
                    int out_dtype, int OH, int OW, float* coords_out, int hp, int wp, void* stream) {
   return view_crops(image, H, W, boxes_host, flips_host, V, out, out_dtype == DVT_DTYPE_BF16, OH, OW, coords_out, hp, wp,
                     reinterpret_cast<cudaStream_t>(stream));
+}
+
+int dvt_seg_upsample_ce(const float* logits, int B, int h, int w, int K, const uint8_t* labels, int H, int W, float grad_scale,
+                        float* loss_out, float* dlogits, double* workspace, void* stream) {
+  return launch_seg_upsample_ce(logits, B, h, w, K, labels, H, W, grad_scale, loss_out, dlogits, workspace,
+                                reinterpret_cast<cudaStream_t>(stream));
+}
+int dvt_seg_slide_accumulate(const float* logits, int h, int w, int K, int y1, int x1, int wh, int ww, float* acc, float* count,
+                             int Hc, int Wc, void* stream) {
+  return launch_seg_slide_accumulate(logits, h, w, K, y1, x1, wh, ww, acc, count, Hc, Wc,
+                                     reinterpret_cast<cudaStream_t>(stream));
+}
+int dvt_seg_predict_hist(float* acc, const float* count, int K, int Hc, int Wc, const uint8_t* labels, int Ho, int Wo,
+                         unsigned long long* hist, void* stream) {
+  return launch_seg_predict_hist(acc, count, K, Hc, Wc, labels, Ho, Wo, hist, reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -96,6 +96,11 @@ SIGNATURES = {
     "dvt_fit_sweep_once": (c_int, [c_void_p, c_int, c_void_p]),
     "dvt_view_crops": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p,
                                c_int, c_int, c_void_p]),
+    "dvt_seg_upsample_ce": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_float, c_void_p, c_void_p,
+                                    c_void_p, c_void_p]),
+    "dvt_seg_slide_accumulate": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
+                                         c_int, c_void_p]),
+    "dvt_seg_predict_hist": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "dvt_vit_create": (c_int, [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float]),
     "dvt_vit_create_ex": (c_int, [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_int,
                                   c_int]),

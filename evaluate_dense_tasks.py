@@ -1,0 +1,136 @@
+"""Dense-task linear probe on H100 -- drop-in for the reference's evaluate_dense_tasks.py (semantic segmentation).
+
+Same flags (reference evaluate_dense_tasks.py:34-124), same config files (evaluation/configs/vitb_voc2012_linear_config.py,
+vitb_ade20k_linear_config.py, read as plain Python: no mmcv), same backbones (:177-214: the ViT wrapper at stride = patch,
+optionally with `--load-distilled-model-from`, optionally under the `--load-denoiser-from` Denoiser), same probe (frozen
+backbone behind CenterPadding, BNHead on the `in_index` features, cross-entropy of the bilinearly upsampled logits,
+AdamW + poly schedule with linear warmup, slide inference, mIoU / mAcc / aAcc).  Only the layers `in_index` selects are
+computed.  The full-resolution loss and slide inference run on sm_90a kernels (dvt/dense_eval).
+
+Outputs in the work dir: `iter_<n>.pth` every checkpoint_config.interval iterations and at the end ({"state_dict":
+decode_head.* weights, "optimizer", "iter"}), `latest.pth` pointing at the newest, and `<timestamp>.log.json` (one JSON
+object per line: training losses every log_config.interval iterations, and mIoU, mAcc, aAcc, per-class IoU / Acc of
+every evaluation, as fractions).  `--task depth` (the NYU depth probe) is not implemented.
+
+Launch: `--launcher none` runs one process; `--launcher pytorch` (the default, as in the reference) runs under torchrun,
+one process per GPU, with SyncBatchNorm in the head and DDP over NCCL."""
+import argparse
+import os
+import os.path as osp
+import random
+import sys
+import time
+import warnings
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, os.path.join(ROOT, "denoising-vit_b200"))
+
+from dvt.dense_eval import DictAction, check_supported, load_config, merge_options  # noqa: E402
+
+
+def parse_args(argv=None):
+    parser = argparse.ArgumentParser("Linear Evaluation", add_help=False)
+    parser.add_argument("config", help="train config file path")
+    parser.add_argument("--work-dir", help="the dir to save logs and models")
+    parser.add_argument("--load-denoiser-from", help="the checkpoint file to load weights from")
+    parser.add_argument("--load-distilled-model-from", help="the checkpoint file to load weights from")
+    parser.add_argument("--num_blocks", type=int, default=1)
+    parser.add_argument("--resume-from", help="the checkpoint file to resume from")
+    parser.add_argument("--backbone-type", default="vit_small_patch14_dinov2.lvd142m", help="timm model type")
+    parser.add_argument("--task", type=str, default="segmentation", choices=["segmentation", "depth"], help="task to train")
+    parser.add_argument("--no-validate", action="store_true", help="whether not to evaluate the checkpoint during training")
+    parser.add_argument("--seed", type=int, default=None, help="random seed")
+    parser.add_argument("--diff_seed", action="store_true", help="Whether or not set different seeds for different ranks")
+    parser.add_argument("--deterministic", action="store_true",
+                        help="torch.use_deterministic_algorithms(True): a rerun from the same seed on the same GPU model "
+                             "gives bit-identical head weights and metrics")
+    parser.add_argument("--options", nargs="+", action=DictAction,
+                        help="deprecated alias of --cfg-options (merged after it)")
+    parser.add_argument("--cfg-options", nargs="+", action=DictAction,
+                        help="override settings of the config: key=value pairs with dotted keys, e.g. "
+                             "model.decode_head.num_classes=150 or runner.max_iters=1000; lists as key=[a,b] or key=a,b")
+    parser.add_argument("--launcher", choices=["none", "pytorch", "slurm", "mpi"], default="pytorch", help="job launcher")
+    parser.add_argument("--local-rank", type=int, default=0)
+    parser.add_argument("--auto-resume", action="store_true", help="resume from the latest checkpoint automatically.")
+    args = parser.parse_args(argv)
+    if "LOCAL_RANK" not in os.environ:
+        os.environ["LOCAL_RANK"] = str(args.local_rank)
+    return args
+
+
+def main(args):
+    if args.task == "depth":
+        raise NotImplementedError("--task depth: the NYU depth probe (reference build_depther, evaluation/depth: the "
+                                  "depther, its decode head and datasets) is not implemented; only segmentation is")
+    cfg = load_config(args.config)
+    if args.cfg_options is not None:
+        merge_options(cfg, args.cfg_options)
+    if args.options is not None:
+        warnings.warn("--options is deprecated in favor of --cfg-options")
+        merge_options(cfg, args.options)
+    check_supported(cfg)
+    if args.work_dir is not None:
+        cfg["work_dir"] = args.work_dir
+    elif cfg.get("work_dir") is None:
+        cfg["work_dir"] = osp.join("./work_dirs", osp.splitext(osp.basename(args.config))[0])
+    resume_from = args.resume_from if args.resume_from is not None else cfg.get("resume_from")
+    if resume_from is None and args.auto_resume and osp.exists(osp.join(cfg["work_dir"], "latest.pth")):
+        resume_from = osp.join(cfg["work_dir"], "latest.pth")
+
+    assert torch.cuda.is_available(), "the H100 segmentation probe needs a CUDA device (no CPU fallback)"
+    import torch.distributed as dist
+    if args.launcher == "none":
+        rank, world, local = 0, 1, 0
+    elif args.launcher == "pytorch":
+        if "RANK" not in os.environ or "WORLD_SIZE" not in os.environ:
+            raise RuntimeError("--launcher pytorch runs under torchrun (RANK / WORLD_SIZE are not set); use --launcher none "
+                               "for one process")
+        rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
+    else:
+        raise NotImplementedError(f"--launcher {args.launcher}: only none and pytorch (torchrun) are implemented")
+    torch.cuda.set_device(local)
+    device = torch.device("cuda", local)
+    if args.launcher == "pytorch":
+        dist.init_process_group(cfg.get("dist_params", {}).get("backend", "nccl"), device_id=device)
+    os.makedirs(osp.abspath(cfg["work_dir"]), exist_ok=True)
+    timestamp = time.strftime("%Y%m%d_%H%M%S", time.localtime())
+
+    # init_random_seed: a random seed is drawn on rank 0 and shared; --diff_seed adds the rank
+    seed = args.seed
+    if seed is None:
+        t = torch.tensor([np.random.randint(2 ** 31)], dtype=torch.int64, device=device)
+        if world > 1:
+            dist.broadcast(t, 0)
+        seed = int(t.item())
+    if args.diff_seed:
+        seed += rank
+    random.seed(seed)
+    np.random.seed(seed)
+    torch.manual_seed(seed)
+    torch.cuda.manual_seed_all(seed)
+    if args.deterministic:
+        os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")
+        torch.use_deterministic_algorithms(True)
+        torch.backends.cudnn.benchmark = False
+    elif cfg.get("cudnn_benchmark", False):
+        torch.backends.cudnn.benchmark = True
+    if rank == 0:
+        print(f"Set random seed to {seed}, deterministic: {args.deterministic}; work dir {cfg['work_dir']}", flush=True)
+
+    from dvt.dense_eval.model import build_backbone
+    from dvt.dense_eval.trainer import train
+    backbone = build_backbone(args.backbone_type, args.load_distilled_model_from, args.load_denoiser_from, args.num_blocks,
+                              device)
+    out = train(cfg, backbone, cfg["work_dir"], seed, device, validate=not args.no_validate, resume_from=resume_from,
+                timestamp=timestamp, exp_name=osp.basename(args.config))
+    if world > 1:
+        dist.barrier()
+        dist.destroy_process_group()
+    return out
+
+
+if __name__ == "__main__":
+    main(parse_args())

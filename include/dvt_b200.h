@@ -334,6 +334,31 @@ int dvt_resample_bwd(const float* wh, const float* ww, const float* dout, float*
 int dvt_view_crops(const float* image, int H, int W, const int* boxes_host, const int* flips_host, int V, void* out,
                    int out_dtype, int OH, int OW, float* coords_out, int hp, int wp, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------
+ * Dense-task linear probe, semantic segmentation (reference evaluate_dense_tasks.py with the BNHead configs of
+ * evaluation/configs/vitb_{voc2012,ade20k}_linear_config.py; mmseg 0.27 EncoderDecoder).  Every resize is ATen's bilinear upsample with
+ * align_corners=False, computed in fp32.  No float atomics: repeated calls are bit-identical.
+ * ------------------------------------------------------------------------------------------------------- */
+/* Training loss of the head and its gradient in one call (replaces mmseg's resize(seg_logit, label size) + CrossEntropyLoss
+ * (ignore_index 255, mean over ALL pixels) + their autograd backward).  logits f32 [B, h, w, K] (NHWC), labels u8 [B, H, W];
+ * a label >= K (255: ignore) contributes no loss and no gradient.  loss_out f32 [1] = sum over pixels of the cross-entropy
+ * of the upsampled logits (overwritten); dlogits f32 [B, h, w, K] (overwritten) = grad_scale * d(loss sum)/d logits at the
+ * low resolution.  The full-resolution logits and their gradient are never written.  2 <= K <= 255.
+ * workspace f64 [B * ceil(h / 2) * ceil(w / 2)]. */
+int dvt_seg_upsample_ce(const float* logits, int B, int h, int w, int K, const uint8_t* labels, int H, int W, float grad_scale,
+                        float* loss_out, float* dlogits, double* workspace, void* stream);
+/* Slide inference, one window (mmseg EncoderDecoder.slide_inference): upsamples the window's logits f32 [h, w, K] (NHWC) to
+ * the window size wh x ww and adds them into acc f32 [K, Hc, Wc] at (y1, x1); count f32 [Hc, Wc] += 1 there.  Windows
+ * enqueued in order on one stream add in that order. */
+int dvt_seg_slide_accumulate(const float* logits, int h, int w, int K, int y1, int x1, int wh, int ww, float* acc, float* count,
+                             int Hc, int Wc, void* stream);
+/* Slide inference, end of an image: acc /= count in place, then for every pixel of the original Ho x Wo image the bilinear
+ * resize from Hc x Wc, argmax over K (ties: lowest class) and mmseg's intersect_and_union against labels u8 [Ho, Wo]
+ * (255 ignored; labels >= K count in the prediction histogram only): hist u64 [4, K] += (intersect, union, pred, label).
+ * The resized logits are never written. */
+int dvt_seg_predict_hist(float* acc, const float* count, int K, int Hc, int Wc, const uint8_t* labels, int Ho, int Wo,
+                         unsigned long long* hist, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

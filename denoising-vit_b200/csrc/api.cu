@@ -420,8 +420,7 @@ int dvt_gemm_f32x3(const float* A, int lda, size_t plane_a, int a_mn, const floa
     e.out_mode = OUT_F32;
   }
   GemmShape s{M, N, K, splits < 1 ? 1 : splits};
-  static const int x3_mode = [] { const char* v = getenv("DVT_DEBUG_X3_MODE"); return v ? atoi(v) : 1; }();  // 2: hi.hi only (timing aid)
-  s.a_mn = a_mn; s.b_mn = b_mn; s.x3 = x3_mode; s.plane_a = plane_a; s.plane_b = plane_b;
+  s.a_mn = a_mn; s.b_mn = b_mn; s.x3 = 1; s.plane_a = plane_a; s.plane_b = plane_b;
   return launch_gemm_tn(A, lda, B, ldb, TMAP_F32, s, e, reinterpret_cast<cudaStream_t>(stream), eff_impl());
 }
 

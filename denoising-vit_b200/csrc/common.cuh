@@ -147,43 +147,20 @@ __device__ __forceinline__ void st_release_u32(unsigned* p, unsigned v) {
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-// prio_drop > 0: the kernel runs that many levels BELOW the highest stream priority whatever its stream's priority is
-// (kernels off the critical path that would otherwise take the SMs the next critical kernel is waiting for).
-struct LaunchOpt {
-  bool pdl = false;
-  int prio_drop = 0;
-};
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_kx(LaunchOpt o, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
-                             Args&&... args) {
+inline cudaError_t launch_k(bool pdl, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                            Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  int na = 0;
-  if (o.pdl) {
-    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  if (o.prio_drop > 0) {
-    static int lo = 0, hi = 0;
-    static const cudaError_t range_rc = cudaDeviceGetStreamPriorityRange(&lo, &hi);  // (numerically lower = higher priority)
-    if (range_rc != cudaSuccess) return range_rc;
-    attr[na].id = cudaLaunchAttributePriority;
-    attr[na].val.priority = hi + o.prio_drop < lo ? hi + o.prio_drop : lo;
-    ++na;
-  }
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = na;
+  cfg.numAttrs = pdl ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
-}
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_k(bool pdl, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
-                            Args&&... args) {
-  return launch_kx(LaunchOpt{pdl, 0}, kern, grid, block, smem, st, static_cast<Args&&>(args)...);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -216,14 +193,6 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       ::"r"(smem_u32(smem_dst)),
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
-}
-
-// 1-D bulk copy global -> shared (no tensor map): size and both addresses multiples of 16 bytes
-__device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   smem_u32(smem_dst)),
-               "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
 }
 
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {

@@ -8,11 +8,11 @@
 // One step = a fixed set of kernels on five streams (captured into CUDA graphs of several steps by the host; the full
 // schedule with its hazards is documented at fit_enqueue_step):
 //   main  : GEMM h1 = relu(enc W1^T + b1), GEMM F = h1 W2^T + b2, loss (pred = F + G[r,c] (+R), MSE + cosine, d pred,
-//           dG atomics, loss log), dgrad, dgrad, grid backward (vector atomics + touched-entry stamps),
+//           loss log), dgrad, dgrad, grid backward (sorted, fixed-order sums + touched-entry stamps),
 //           encode of the NEXT step (hash-grid gather / interpolation with the pending Adam steps applied on the fly)
-//   sides : gather of the sampled bank rows, residual MLP forward (3 GEMM) / backward (5 GEMM), weight-gradient GEMMs,
-//           Adam(small params), and the dense Adam sweep of the hash table (one pass per window of k steps,
-//           software-pipelined one to two windows deep)
+//   sides : gather of the sampled bank rows, dG (one warp per cell, rows in ascending order), residual MLP forward
+//           (3 GEMM) / backward (5 GEMM), weight-gradient GEMMs, Adam(small params), and the dense Adam sweep of the
+//           hash table (one pass per window of k steps, software-pipelined one to two windows deep)
 // All GEMMs run on the tensor cores (gemm.cu) as 3xTF32 products of fp32 hi/lo planes (fp32-accurate: bf16 operands cannot
 // hold the cosine >= 0.999 parity bar, see DESIGN.md); weight-gradient GEMMs read the activations as MN-major
 // operands, so no transposed copies exist; bias gradients come from a ones column appended to the activation buffers.
@@ -34,6 +34,9 @@ namespace dvt {
 constexpr int FIT_MAX_LEVELS = 16;
 constexpr int FIT_F = 8;  // features per level
 constexpr int FIT_MAX_WINDOW = 8;  // steps per pipelined table sweep (DVT_FIT_SWEEP_STEPS)
+// threads of a persistent sweep CTA: 1024 fill the register file of their SM, so the GEMM chain of the next steps keeps the
+// other SMs instead of sharing this one
+constexpr int FIT_SWEEP_CTA_THREADS = 1024;
 
 struct GridLevels {
   int n_levels;
@@ -651,10 +654,9 @@ static int launch_loss(const LossArgs& la, cudaStream_t st, bool pdl) {
 // read for stamped entries only.
 // Launch geometries (fit_sweep_geometry): many short-lived 256-thread CTAs (fastest alone: 77 us, the HBM peak), or a
 // few persistent 1024-thread CTAs that fill one SM each and leave the other SMs to the GEMM chain of the next steps.
-// (Measured and rejected: one contiguous slice per CTA -- 133 us, HBM channel imbalance; maximum shared-memory
-// carve-out -- 137 us.)
+// (Measured and rejected: one contiguous slice per CTA -- 133 us, HBM channel imbalance.)
 template <int KW>
-__global__ void __launch_bounds__(1024, 1)
+__global__ void __launch_bounds__(FIT_SWEEP_CTA_THREADS, 1)
 fit_adam_table_kernel(TableBufs tb, size_t nvec, const AdamScalars* __restrict__ sc, const int* __restrict__ step_base,
                       int step_off, int len, int buf_off, float wd) {
   // two elements in flight per thread for one-step windows, one for longer windows; the gradient loads of windows over 4
@@ -733,104 +735,6 @@ fit_adam_table_kernel(TableBufs tb, size_t nvec, const AdamScalars* __restrict__
       }
       po[i] = pp[u]; mo[i] = mm[u]; vo[i] = vv[u];
     }
-  }
-}
-
-// ----------------------------------------------------------------------------------------------------
-// EXPERIMENT (DVT_FIT_SWEEP_TMA=1; not the default): the same sweep staged through shared memory by bulk async copies
-// (TMA, cp.async.bulk).  One-step windows only (the host runs the plain kernel for longer ones).  ONE thread per CTA
-// keeps three 50 KB chunks (p, m, v and the stamps of 512 table entries) in flight per SM through an mbarrier ring of four stages while 512 threads run the Adam arithmetic out of
-// shared memory and write the results back with coalesced 16-byte stores.  Idea: memory-level parallelism independent of
-// the thread count, so that a few dozen SMs could saturate HBM (Little's law: the bytes in flight per SM times the SMs
-// the sweep runs on, over the loaded latency, bound its rate).  Same adam1() arithmetic, same stamp rules:
-// bit-identical results (tests/test_fit_gpu.py::test_sweep_kernels_agree).
-// Chunks are dealt round-robin (chunk c -> CTA c % grid), i.e. all CTAs advance one contiguous front together.
-// ----------------------------------------------------------------------------------------------------
-constexpr int SW_ENT = 512;                       // table entries per chunk
-constexpr int SW_FLOATS = SW_ENT * FIT_F;         // 4096 floats = 16 KB per array and chunk
-constexpr int SW_STAGES = 4;
-constexpr int SW_THREADS = 512;
-struct SweepStage {
-  float p[SW_FLOATS], m[SW_FLOATS], v[SW_FLOATS];
-  uint32_t stamp[SW_ENT];
-};
-constexpr size_t SW_SMEM = SW_STAGES * sizeof(SweepStage) + SW_STAGES * sizeof(uint64_t) + 128;
-static_assert(sizeof(SweepStage) % 128 == 0, "stage size keeps the 16-byte alignment of bulk copies");
-static_assert(SW_SMEM <= 227 * 1024, "sweep stages exceed shared memory");
-
-__global__ void __launch_bounds__(SW_THREADS, 1)
-fit_adam_table_tma_kernel(TableBufs tb, uint32_t n_entries, const AdamScalars* __restrict__ sc,
-                          const int* __restrict__ step_base, int step_off, int buf_off, float wd) {
-  extern __shared__ uint8_t sw_smem_raw[];
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(sw_smem_raw) + 127) & ~uintptr_t(127));
-  SweepStage* stg = reinterpret_cast<SweepStage*>(base);
-  uint64_t* full = reinterpret_cast<uint64_t*>(base + SW_STAGES * sizeof(SweepStage));
-  const int tid = threadIdx.x;
-  if (tid == 0) {
-    for (int s = 0; s < SW_STAGES; ++s) mbar_init(&full[s], 1);
-    fence_mbar_init();
-  }
-  __syncthreads();
-  pdl_wait();     // (no-ops unless launched with programmatic stream serialisation)
-  pdl_trigger();
-  const int step = step_base[0] + step_off;
-  const int src = (step_base[1] + buf_off) & 1;
-  const float* __restrict__ p = DVT_SEL2(tb.p, src);
-  const float* __restrict__ m = DVT_SEL2(tb.m, src);
-  const float* __restrict__ v = DVT_SEL2(tb.v, src);
-  float4* __restrict__ po = reinterpret_cast<float4*>(DVT_SEL2(tb.p, src ^ 1));
-  float4* __restrict__ mo = reinterpret_cast<float4*>(DVT_SEL2(tb.m, src ^ 1));
-  float4* __restrict__ vo = reinterpret_cast<float4*>(DVT_SEL2(tb.v, src ^ 1));
-  const float4* __restrict__ g = reinterpret_cast<const float4*>(tb.g_of(step));
-  const uint32_t* __restrict__ stamp = tb.stamp_of(step);
-  const AdamScalars s = sc[step];
-  const uint32_t mark = (uint32_t)step + 1u;
-  const uint32_t n_chunks = (n_entries + SW_ENT - 1) / SW_ENT;
-
-  auto issue = [&](uint32_t k) {  // thread 0: bulk loads of this CTA's k-th chunk into stage k % SW_STAGES
-    const uint32_t c = blockIdx.x + k * gridDim.x;
-    if (c >= n_chunks) return;
-    SweepStage& st = stg[k % SW_STAGES];
-    uint64_t* bar = &full[k % SW_STAGES];
-    const uint32_t e0 = c * SW_ENT, ne = min((uint32_t)SW_ENT, n_entries - e0);
-    const uint32_t bp = ne * FIT_F * 4, bs = ne * 4;  // entries per level are multiples of 8: both multiples of 32 B
-    mbar_expect_tx(bar, 3 * bp + bs);
-    bulk_load_1d(st.p, p + (size_t)e0 * FIT_F, bp, bar);
-    bulk_load_1d(st.m, m + (size_t)e0 * FIT_F, bp, bar);
-    bulk_load_1d(st.v, v + (size_t)e0 * FIT_F, bp, bar);
-    bulk_load_1d(st.stamp, stamp + e0, bs, bar);
-  };
-  if (tid == 0)
-    for (uint32_t k = 0; k + 1 < SW_STAGES; ++k) issue(k);
-
-  for (uint32_t k = 0;; ++k) {
-    const uint32_t c = blockIdx.x + k * gridDim.x;
-    if (c >= n_chunks) break;
-    // refill the stage that was consumed in iteration k-1 (all its readers passed the __syncthreads below)
-    if (tid == 0) issue(k + SW_STAGES - 1);
-    const SweepStage& st = stg[k % SW_STAGES];
-    mbar_wait(&full[k % SW_STAGES], (k / SW_STAGES) & 1u, 0x51);
-    const uint32_t e0 = c * SW_ENT, ne = min((uint32_t)SW_ENT, n_entries - e0);
-    const size_t f0 = (size_t)e0 * 2;            // first float4 of the chunk
-    const float4* sp = reinterpret_cast<const float4*>(st.p);
-    const float4* sm = reinterpret_cast<const float4*>(st.m);
-    const float4* sv = reinterpret_cast<const float4*>(st.v);
-#pragma unroll
-    for (int u = 0; u < (SW_ENT * 2) / SW_THREADS; ++u) {
-      const uint32_t i = tid + u * SW_THREADS;   // float4 index inside the chunk; entry = i / 2
-      if (i < ne * 2) {
-        const bool touched = st.stamp[i >> 1] == mark;
-        float4 pp = sp[i], mm = sm[i], vv = sv[i];
-        float4 gg = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (touched) gg = __ldcg(g + f0 + i);
-        adam1(pp.x, mm.x, vv.x, gg.x, wd, s.step_size, s.inv_bc2_sqrt);
-        adam1(pp.y, mm.y, vv.y, gg.y, wd, s.step_size, s.inv_bc2_sqrt);
-        adam1(pp.z, mm.z, vv.z, gg.z, wd, s.step_size, s.inv_bc2_sqrt);
-        adam1(pp.w, mm.w, vv.w, gg.w, wd, s.step_size, s.inv_bc2_sqrt);
-        po[f0 + i] = pp; mo[f0 + i] = mm; vo[f0 + i] = vv;
-      }
-    }
-    __syncthreads();
   }
 }
 
@@ -921,7 +825,6 @@ struct Fit {
   int n_small = 0;
   // device memory
   TableBufs tb = {};                           // ping-pong p/m/v, ring of gradient / stamp slots
-  int cur_host = 0;                            // steps completed (host view)
   int cur_buf = 0;                             // table sweeps completed mod 2 (host view): the current table is tb.p[cur_buf]
   cudaStream_t sD = nullptr;                   // stream of the pipelined table sweeps
   cudaEvent_t ev_sweep[3] = {};                // completion of the window sweep w of the epoch (slot w % 3)
@@ -932,19 +835,11 @@ struct Fit {
   bool epoch_forked = false;                   // this epoch forked sweeps onto sD (pipelined schedule)
   int sweep_steps[2] = {4, 4};                 // DVT_FIT_SWEEP_STEPS "k1,k2": window of the pipelined sweep per phase
   bool enc_ready = false;                      // f->enc already holds the encoding of the next step
-  int res_x3 = 1;                              // GEMM mode of the residual MLP: 1 = 3xTF32, 2 = plain TF32 (experiment)
-  int sweep_threads = 1024;                    // DVT_FIT_SWEEP_THREADS: threads of a persistent sweep CTA (1024 fills the register file of
-                                               // its SM; 512 leaves half of it to co-resident CTAs of the chain)
   int x3_wide_min_n[2] = {0, 256};             // DVT_FIT_X3_WIDE_MIN_N "p1,p2": 128 x 128 GEMM tiles when N >= this (0: never)
   int wgrad_sms = 96;                          // DVT_FIT_WGRAD_SMS: weight-gradient GEMMs split K to fill at most this many SMs
-  bool sweep_pdl = true;                       // DVT_FIT_SWEEP_PDL=0: the persistent sweep CTAs of step t+1 are not made resident
-                                               // (waiting, one full SM each) while sweep t still runs
-  int off_path_prio_drop = 0;                  // DVT_FIT_OFFPATH_PRIO: priority levels below the chain for off-path kernels
-  int wgrad_x3 = 1;                            // GEMM mode of the field MLP's weight-gradient GEMMs (DVT_FIT_WGRAD_TF32=1: 2)
-  bool pdl = true;                             // programmatic dependent launch along the kernel chains of a step
+  bool pdl = true;                             // DVT_FIT_PDL: programmatic dependent launch along the kernel chains of a step
   bool pipe[2] = {true, true};                 // software-pipelined table sweep in phase 1 / 2 (see fit_enqueue_step)
   int sweep_ctas[2] = {0, 0};                  // persistent sweep CTAs in phase 1 / 2 (0 = many small CTAs)
-  bool sweep_tma = false;                      // DVT_FIT_SWEEP_TMA=1: persistent sweep = the TMA-staged kernel (experiment)
   float *sp = nullptr, *sm = nullptr, *sv = nullptr, *sg = nullptr;
   float* wsplit = nullptr;  // [2][n_small] TF32 hi / lo planes of the small params (x3 GEMM operands)
   // activations: GEMM operands are stored as two fp32 planes (hi, lo), plane stride = bsz * ld
@@ -955,7 +850,7 @@ struct Fit {
   int ld_enc, ld_h1, ld_raw, ld_r;
   // schedule
   int num_iters = 0, freeze_step = 0;
-  int cur_step = 0;                            // steps of the current schedule already enqueued (host mirror of *step_base)
+  int cur_step = 0;                            // steps of the current schedule already enqueued (host mirror of step_base[0])
   // sampling stream: two device buffers + two pinned staging buffers, so that the upload of the next image's stream
   // runs (on sU) while the current fit is still reading its own
   int* idx[2] = {nullptr, nullptr};            // [num_iters + 1, bsz] each
@@ -999,41 +894,11 @@ struct Fit {
   std::vector<void*> owned;
 };
 
-// EXPERIMENT (DVT_FIT_CARVEOUT=<percent> for the small kernels, DVT_FIT_CARVEOUT_SWEEP=<percent> for the sweep; off by
-// default).  The 3xTF32 GEMM CTAs of the chain need up to ~200 KB of shared memory, and an SM changes its L1 / shared-memory
-// split only when it is idle: a GEMM CTA cannot join an SM on which one of the fit's small kernels (no shared memory, so by
-// default the largest L1) got first.  Asking for a shared-memory carve-out on the fit's own kernels makes the GEMM CTAs
-// resident beside them, at the cost of the L1 the sweep / encode / loss kernels keep their loads in flight in.
 static int fit_prepare_kernels() {
   static bool done = false;
   if (done) return DVT_OK;
   done = true;
   DVT_CUDA_OK(cudaFuncSetAttribute(fit_grid_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GB_SMEM));
-  const char* e = getenv("DVT_FIT_CARVEOUT");            // percent of the unified L1 / shared array, small kernels
-  const char* es = getenv("DVT_FIT_CARVEOUT_SWEEP");     // ... the sweep
-  const int pct = e ? atoi(e) : 0, pct_sweep = es ? atoi(es) : 0;
-#define DVT_MAX_SHARED(k) DVT_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, pct))
-  if (pct_sweep > 0) {
-#define DVT_SWEEP_SHARED(k) DVT_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, pct_sweep))
-    DVT_SWEEP_SHARED(fit_adam_table_kernel<1>); DVT_SWEEP_SHARED(fit_adam_table_kernel<2>);
-    DVT_SWEEP_SHARED(fit_adam_table_kernel<4>); DVT_SWEEP_SHARED(fit_adam_table_kernel<8>);
-#undef DVT_SWEEP_SHARED
-  }
-  if (pct <= 0) return DVT_OK;
-  DVT_MAX_SHARED(fit_encode_kernel<2>); DVT_MAX_SHARED(fit_encode_kernel<4>); DVT_MAX_SHARED(fit_encode_kernel<8>);
-  DVT_MAX_SHARED(fit_encode_kernel<10>); DVT_MAX_SHARED(fit_encode_kernel<16>);
-  DVT_MAX_SHARED(fit_grid_bwd_kernel);
-  DVT_MAX_SHARED(fit_gather_rows_kernel);
-  DVT_MAX_SHARED(fit_g_scatter_kernel);
-  DVT_MAX_SHARED(fit_adam_small_kernel);
-  DVT_MAX_SHARED(fit_advance_kernel);
-  DVT_MAX_SHARED((fit_loss_kernel<1, false>)); DVT_MAX_SHARED((fit_loss_kernel<1, true>));
-  DVT_MAX_SHARED((fit_loss_kernel<2, false>)); DVT_MAX_SHARED((fit_loss_kernel<2, true>));
-  DVT_MAX_SHARED((fit_loss_kernel<3, false>)); DVT_MAX_SHARED((fit_loss_kernel<3, true>));
-  DVT_MAX_SHARED((fit_loss_kernel<6, false>)); DVT_MAX_SHARED((fit_loss_kernel<6, true>));
-  DVT_MAX_SHARED((fit_loss_kernel<8, false>)); DVT_MAX_SHARED((fit_loss_kernel<8, true>));
-  DVT_MAX_SHARED((fit_loss_kernel<12, false>)); DVT_MAX_SHARED((fit_loss_kernel<12, true>));
-#undef DVT_MAX_SHARED
   return DVT_OK;
 }
 
@@ -1045,6 +910,53 @@ static int fit_alloc(Fit* f, void** p, size_t bytes, bool zero = true) {
 }
 
 static int r8(int x) { return (x + 7) / 8 * 8; }
+
+// Schedule knobs, read once per engine (defaults chosen at the headline size; not yet re-tuned for the 132 SMs of an H100):
+//   DVT_FIT_PIPELINE=0            sequential schedule in both phases
+//   DVT_FIT_SWEEP_CTAS="a[,b]"    per phase (1 [, 2]): n > 0 pipelined sweep on n persistent CTAs (one per SM,
+//                                 FIT_SWEEP_CTA_THREADS threads); 0 pipelined sweep on 8 x #SM CTAs of 256 threads;
+//                                 -1 sequential schedule
+//   DVT_FIT_SWEEP_STEPS="k1[,k2]" per phase: the pipelined sweep makes one pass over the table per window of k steps
+//                                 (1 <= k <= FIT_MAX_WINDOW; 1 = one pass per step).  The sequential schedule sweeps every step.
+//   DVT_FIT_PDL=0                 plain stream-ordered launches (no programmatic dependent launch)
+//   DVT_FIT_WGRAD_SMS=n           split-K of the weight-gradient GEMMs fills at most n SMs (they share the GPU with the
+//                                 data-gradient GEMMs of the critical path)
+//   DVT_FIT_X3_WIDE_MIN_N="a[,b]" per phase: 3xTF32 GEMMs with N >= this use 128 x 128 tiles (0: always 128 x 64)
+// (DVT_FIT_DEBUG_GRAPH=1 is read by fit_capture: it prints what each capture recorded.)
+static int fit_read_schedule_env(Fit* f) {
+  int win[2] = {f->sweep_steps[0], f->sweep_steps[1]};
+  if (const char* ss = getenv("DVT_FIT_SWEEP_STEPS")) {
+    const int got = sscanf(ss, "%d,%d", &win[0], &win[1]);
+    if (got == 1) win[1] = win[0];
+    DVT_REQUIRE(got >= 1, "fit: DVT_FIT_SWEEP_STEPS '%s' is not \"k1[,k2]\"", ss);
+  }
+  for (int q = 0; q < 2; ++q)
+    DVT_REQUIRE(win[q] >= 1 && win[q] <= FIT_MAX_WINDOW, "fit: DVT_FIT_SWEEP_STEPS %d out of range [1, %d]", win[q],
+                FIT_MAX_WINDOW);
+  int ctas[2] = {48, 48};
+  if (const char* se = getenv("DVT_FIT_SWEEP_CTAS")) {
+    int a = 0, b = 0;
+    const int got = sscanf(se, "%d,%d", &a, &b);
+    if (got >= 1) { ctas[0] = a; ctas[1] = got >= 2 ? b : a; }
+  }
+  const char* pe = getenv("DVT_FIT_PIPELINE");
+  const bool off = pe && pe[0] == '0';
+  for (int q = 0; q < 2; ++q) {
+    f->pipe[q] = !off && ctas[q] >= 0;
+    f->sweep_ctas[q] = f->pipe[q] ? std::min(ctas[q], num_sms()) : 0;
+    f->sweep_steps[q] = f->pipe[q] ? win[q] : 1;
+  }
+  const char* pd = getenv("DVT_FIT_PDL");
+  f->pdl = !(pd && pd[0] == '0');
+  if (const char* ws = getenv("DVT_FIT_WGRAD_SMS")) f->wgrad_sms = std::max(1, atoi(ws));
+  if (const char* wm = getenv("DVT_FIT_X3_WIDE_MIN_N")) {
+    int a = 0, b = 0;
+    const int got = sscanf(wm, "%d,%d", &a, &b);
+    if (got >= 1) f->x3_wide_min_n[0] = f->x3_wide_min_n[1] = std::max(0, a);
+    if (got == 2) f->x3_wide_min_n[1] = std::max(0, b);
+  }
+  return DVT_OK;
+}
 
 int fit_create(Fit** out, int C, int gh, int gw, int bsz, int n_levels, const float* scale, const uint32_t* res,
                const uint32_t* size, const uint32_t* offset, const uint32_t* hashed) {
@@ -1058,18 +970,8 @@ int fit_create(Fit** out, int C, int gh, int gw, int bsz, int n_levels, const fl
     prc = fit_prepare_kernels();
     if (prc) return prc;
   }
-  // DVT_FIT_SWEEP_STEPS="k1[,k2]" per phase: the pipelined sweep makes one pass over the table per window of k steps
-  // (1 <= k <= FIT_MAX_WINDOW; 1 = one pass per step).  The sequential schedule sweeps every step.
-  int win[2] = {Fit().sweep_steps[0], Fit().sweep_steps[1]};
-  if (const char* ss = getenv("DVT_FIT_SWEEP_STEPS")) {
-    const int got = sscanf(ss, "%d,%d", &win[0], &win[1]);
-    if (got == 1) win[1] = win[0];
-    DVT_REQUIRE(got >= 1, "fit: DVT_FIT_SWEEP_STEPS '%s' is not \"k1[,k2]\"", ss);
-  }
-  for (int q = 0; q < 2; ++q)
-    DVT_REQUIRE(win[q] >= 1 && win[q] <= FIT_MAX_WINDOW, "fit: DVT_FIT_SWEEP_STEPS %d out of range [1, %d]", win[q],
-                FIT_MAX_WINDOW);
   Fit* f = new Fit();
+  if (int env_rc = fit_read_schedule_env(f)) { delete f; return env_rc; }
   int prio_lo = 0, prio_hi = 0;  // (numerically lower = higher priority)
   DVT_CUDA_OK(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
   DVT_CUDA_OK(cudaStreamCreateWithPriority(&f->stream, cudaStreamNonBlocking, prio_hi));
@@ -1084,54 +986,6 @@ int fit_create(Fit** out, int C, int gh, int gw, int bsz, int n_levels, const fl
   for (auto& e : f->ev_sweep) DVT_CUDA_OK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
   DVT_CUDA_OK(cudaEventCreateWithFlags(&f->ev_in, cudaEventDisableTiming));
   DVT_CUDA_OK(cudaEventCreateWithFlags(&f->ev_out, cudaEventDisableTiming));
-  {
-    // Schedule knobs (defaults chosen at the headline size; not yet re-tuned for the 132 SMs of an H100):
-    //   DVT_FIT_SWEEP_CTAS="a[,b]"  per phase (1 [, 2]): n > 0 pipelined sweep on n persistent CTAs (1024 threads, one
-    //                               per SM); 0 pipelined sweep on 8 x #SM CTAs of 256 threads; -1 sequential schedule
-    //   DVT_FIT_PIPELINE=0          sequential schedule in both phases
-    int cfg[2] = {48, 48};
-    if (const char* se = getenv("DVT_FIT_SWEEP_CTAS")) {
-      int a = 0, b = 0;
-      const int got = sscanf(se, "%d,%d", &a, &b);
-      if (got >= 1) { cfg[0] = a; cfg[1] = got >= 2 ? b : a; }
-    }
-    //   DVT_FIT_PDL=0               plain stream-ordered launches (no programmatic dependent launch)
-    //   DVT_FIT_RES_TF32=1          residual-MLP GEMMs in plain TF32 instead of 3xTF32 (experiment; not the default)
-    //   DVT_FIT_SWEEP_TMA=1         persistent sweep CTAs use the TMA-staged kernel instead of plain loads (bit-identical;
-    //                               kept as a tested experiment)
-    const char* tm = getenv("DVT_FIT_SWEEP_TMA");
-    f->sweep_tma = tm && tm[0] == '1';
-    //   DVT_FIT_WGRAD_TF32=1        weight-gradient GEMMs of the field MLP in plain TF32 (experiment; not the default)
-    const char* wt = getenv("DVT_FIT_WGRAD_TF32");
-    f->wgrad_x3 = (wt && wt[0] == '1') ? 2 : 1;
-    //   DVT_FIT_SWEEP_PDL=0         sweep t+1 is launched only when sweep t has completed (no waiting resident CTAs)
-    //   DVT_FIT_X3_WIDE_MIN_N="a[,b]" per phase: 3xTF32 GEMMs with N >= this use 128 x 128 tiles (0: always 128 x 64)
-    //   DVT_FIT_WGRAD_SMS=n         split-K of the weight-gradient GEMMs fills at most n SMs (they share the GPU with the
-    //                               data-gradient GEMMs of the critical path)
-    //   DVT_FIT_OFFPATH_PRIO=n      launch priority of the kernels that only feed Adam(small), n levels below the chain.
-    //                               The graphs keep the attribute (DVT_FIT_DEBUG_GRAPH=1 shows it).  Default 0.
-    if (const char* sp_ = getenv("DVT_FIT_SWEEP_PDL")) f->sweep_pdl = sp_[0] != '0';
-    if (const char* wm = getenv("DVT_FIT_X3_WIDE_MIN_N")) {
-      int a = 0, b = 0;
-      const int got = sscanf(wm, "%d,%d", &a, &b);
-      if (got >= 1) f->x3_wide_min_n[0] = f->x3_wide_min_n[1] = std::max(0, a);
-      if (got == 2) f->x3_wide_min_n[1] = std::max(0, b);
-    }
-    if (const char* st_ = getenv("DVT_FIT_SWEEP_THREADS")) f->sweep_threads = std::min(1024, std::max(128, atoi(st_) / 32 * 32));
-    if (const char* ws = getenv("DVT_FIT_WGRAD_SMS")) f->wgrad_sms = std::max(1, atoi(ws));
-    if (const char* op = getenv("DVT_FIT_OFFPATH_PRIO")) f->off_path_prio_drop = std::max(0, atoi(op));
-    const char* rt = getenv("DVT_FIT_RES_TF32");
-    f->res_x3 = (rt && rt[0] == '1') ? 2 : 1;
-    const char* pd = getenv("DVT_FIT_PDL");
-    f->pdl = !(pd && pd[0] == '0');
-    const char* pe = getenv("DVT_FIT_PIPELINE");
-    const bool off = pe && pe[0] == '0';
-    for (int q = 0; q < 2; ++q) {
-      f->pipe[q] = !off && cfg[q] >= 0;
-      f->sweep_ctas[q] = f->pipe[q] ? std::min(cfg[q], num_sms()) : 0;
-    }
-    for (int q = 0; q < 2; ++q) f->sweep_steps[q] = f->pipe[q] ? win[q] : 1;
-  }
   f->C = C; f->gh = gh; f->gw = gw; f->hw = gh * gw; f->bsz = bsz; f->Lf = n_levels * FIT_F;
   f->grid.n_levels = n_levels;
   for (int l = 0; l < n_levels; ++l) {
@@ -1380,7 +1234,6 @@ int fit_init_params(Fit* f, uint64_t seed, cudaStream_t caller) {
     count_launch();
     return DVT_OK;
   };
-  f->cur_host = 0;
   f->cur_buf = 0;
   FIT_RC0(launch(f->tb.p[0], f->n_table, 0, 0, 1e-4f));
   struct { Seg* w; Seg* b; uint32_t tid; } lin[] = {{&f->W1, &f->b1, 1}, {&f->W2, &f->b2, 3}, {&f->R1, &f->rb1, 5},
@@ -1525,7 +1378,6 @@ int fit_begin(Fit* f, const float* bank, const float* coords, size_t bank_rows, 
   DVT_CUDA_OK(cudaMemsetAsync(f->losses, 0, (size_t)num_iters * 5 * 4, st));
   if (f->cur_buf)  // the schedule restarts with no sweep done: its state lives in buffer 0
     DVT_CUDA_OK(cudaMemcpyAsync(f->tb.p[0], f->tb.p[1], f->n_table * 4, cudaMemcpyDeviceToDevice, st));
-  f->cur_host = 0;
   f->cur_buf = 0;
   DVT_CUDA_OK(cudaMemsetAsync(f->tb.m[0], 0, f->n_table * 4, st));
   DVT_CUDA_OK(cudaMemsetAsync(f->tb.v[0], 0, f->n_table * 4, st));
@@ -1554,68 +1406,64 @@ struct Op {
   size_t plane;
 };
 
+// What all GEMMs of one step (or one query) share.
+struct GemmOpt {
+  int impl;
+  bool pdl;  // programmatic dependent launch
+  int wide;  // 128 x 128 tiles when N >= this (GemmShape::x3_wide_min_n)
+};
+
+static GemmShape fit_gemm_shape(int M, int N, int K, int splits, Op A, Op B, const GemmOpt& o) {
+  GemmShape s{M, N, K, splits};
+  s.x3 = 1; s.plane_a = A.plane; s.plane_b = B.plane; s.pdl = o.pdl; s.x3_wide_min_n = o.wide;
+  return s;
+}
+
 // Y = act(X W^T + b):  X [M, K] planes, W [N, K] planes.  split_out: Y is written as hi/lo planes (feeds a GEMM).
 static int fit_linear(Op X, int M, int K, Op W, int N, const float* bias, int act, float* out, int ldo, size_t out_plane,
-                      bool split_out, cudaStream_t st, int impl, bool pdl = false, int x3 = 1, int prio_drop = 0,
-                      int wide = 0) {
+                      bool split_out, cudaStream_t st, const GemmOpt& o) {
   GemmEpi e;
   e.bias = bias; e.act = act; e.out = out; e.ldo = ldo; e.out_plane = out_plane;
   e.out_mode = split_out ? OUT_F32_SPLIT : OUT_F32;
-  GemmShape s{M, N, K, 1};
-  s.x3 = x3; s.plane_a = X.plane; s.plane_b = W.plane; s.pdl = pdl; s.prio_drop = prio_drop; s.x3_wide_min_n = wide;
-  return launch_gemm_tn(X.p, X.ld, W.p, W.ld, TMAP_F32, s, e, st, impl);
+  const GemmShape s = fit_gemm_shape(M, N, K, 1, X, W, o);
+  return launch_gemm_tn(X.p, X.ld, W.p, W.ld, TMAP_F32, s, e, st, o.impl);
 }
 
 // dX = (dY . W) * (H > 0):  dY [M, Nout] K-major A; W stored [Nout, Kin] = MN-major B with N = Kin
 static int fit_dgrad(Op dY, int M, int Nout, Op W, int Kin, const float* Hmask, int ldmask, float* out, int ldo,
-                     size_t out_plane, bool split_out, cudaStream_t st, int impl, bool pdl = false, int x3 = 1,
-                     int prio_drop = 0, int wide = 0) {
+                     size_t out_plane, bool split_out, cudaStream_t st, const GemmOpt& o) {
   GemmEpi e;
   e.mask_f32 = Hmask; e.ldmask = ldmask; e.out = out; e.ldo = ldo; e.out_plane = out_plane;
   e.out_mode = split_out ? OUT_F32_SPLIT : OUT_F32;
-  GemmShape s{M, Kin, Nout, 1};
-  s.b_mn = 1; s.x3 = x3; s.plane_a = dY.plane; s.plane_b = W.plane; s.pdl = pdl; s.prio_drop = prio_drop; s.x3_wide_min_n = wide;
-  return launch_gemm_tn(dY.p, dY.ld, W.p, W.ld, TMAP_F32, s, e, st, impl);
+  GemmShape s = fit_gemm_shape(M, Kin, Nout, 1, dY, W, o);
+  s.b_mn = 1;
+  return launch_gemm_tn(dY.p, dY.ld, W.p, W.ld, TMAP_F32, s, e, st, o.impl);
 }
 
 // dW[Nout, Kin] (+ db[Nout]) += dY^T . [X | 1]:  dY stored [n, Nout] (MN-major A), X stored [n, Kin + ones] (MN-major B)
 // sem: FIT_SEM_TILES zeroed per-tile counters of this call site: the splits of a tile add their partial sums in split
-// order, so the gradient does not depend on which split finishes first.
-static int fit_wgrad(Op dY, int n, int Nout, Op X, int Kin, float* gW, float* gb, unsigned* sem, cudaStream_t st, int impl,
-                     bool pdl = false, int x3 = 1, int prio_drop = 0, int wide = 0, int sm_cap = 1 << 20) {
+// order, so the gradient does not depend on which split finishes first.  sm_cap: see Fit::wgrad_sms.
+static int fit_wgrad(Op dY, int n, int Nout, Op X, int Kin, float* gW, float* gb, unsigned* sem, int sm_cap, cudaStream_t st,
+                     const GemmOpt& o) {
   GemmEpi e;
   e.out = gW; e.ldo = Kin; e.out_mode = OUT_F32_ATOMIC; e.last_col_out = gb; e.splitk_sem = sem;
   // split-K so that (output tiles x splits) fills the SMs once: tiles are 128 x 64 or 128 x 128, k-blocks 32 samples
   const int kb = (n + 31) / 32;
-  const int bn = gemm_x3_tile_n(Kin + 1, wide);
+  const int bn = gemm_x3_tile_n(Kin + 1, o.wide);
   const int tiles = ((Nout + 127) / 128) * ((Kin + bn) / bn);
   DVT_REQUIRE(tiles <= FIT_SEM_TILES, "fit: %d weight-gradient tiles exceed the split-K counters", tiles);
-  int splits = std::max(1, std::min(std::min(num_sms(), sm_cap) / std::max(tiles, 1), kb / 4));
-  GemmShape s{Nout, Kin + 1, n, splits};
-  s.a_mn = 1; s.b_mn = 1; s.x3 = x3; s.plane_a = dY.plane; s.plane_b = X.plane; s.pdl = pdl; s.prio_drop = prio_drop;
-  s.x3_wide_min_n = wide;
-  return launch_gemm_tn(dY.p, dY.ld, X.p, X.ld, TMAP_F32, s, e, st, impl);
+  const int splits = std::max(1, std::min(std::min(num_sms(), sm_cap) / std::max(tiles, 1), kb / 4));
+  GemmShape s = fit_gemm_shape(Nout, Kin + 1, n, splits, dY, X, o);
+  s.a_mn = 1; s.b_mn = 1;
+  return launch_gemm_tn(dY.p, dY.ld, X.p, X.ld, TMAP_F32, s, e, st, o.impl);
 }
 
-// Sweep launch geometry: n > 0 persistent CTAs of 1024 threads (one per SM: the register file is full, so the GEMM
-// chain of the next steps keeps the other SMs), else 8 x #SM CTAs of 256 threads (fastest when running alone).
+// Sweep launch geometry: n > 0 persistent CTAs of FIT_SWEEP_CTA_THREADS threads (one per SM), else 8 x #SM CTAs of 256
+// threads (fastest when running alone).
 static void fit_sweep_geometry(const Fit* f, bool phase2, int* grid, int* block) {
   const int ctas = f->sweep_ctas[phase2 ? 1 : 0];
-  if (ctas > 0) { *grid = ctas; *block = f->sweep_threads; }
+  if (ctas > 0) { *grid = ctas; *block = FIT_SWEEP_CTA_THREADS; }
   else { *grid = num_sms() * 8; *block = 256; }
-}
-
-static int fit_launch_sweep_tma(Fit* f, int ctas, int step_off, int buf_off, cudaStream_t st, bool pdl) {
-  static bool prepared = false;
-  if (!prepared) {
-    DVT_CUDA_OK(cudaFuncSetAttribute(fit_adam_table_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SW_SMEM));
-    prepared = true;
-  }
-  DVT_CUDA_OK(launch_k(pdl, fit_adam_table_tma_kernel, dim3(ctas), dim3(SW_THREADS), SW_SMEM, st, f->tb,
-                       (uint32_t)(f->n_table / FIT_F), f->sc_main, f->step_base, step_off, buf_off, f->wd));
-  DVT_CUDA_OK(cudaGetLastError());
-  count_launch();
-  return DVT_OK;
 }
 
 // The sweep kernel instance with a window capacity KW >= len (the smallest one: registers).
@@ -1638,12 +1486,9 @@ static int fit_launch_sweep_kernel(Fit* f, dim3 grid, dim3 block, int step_off, 
 
 // Sweep of the window [step_off, step_off + len) from state buffer (step_base[1] + buf_off) & 1.
 static int fit_launch_sweep(Fit* f, int step_off, int len, int buf_off, bool phase2, cudaStream_t st) {
-  const bool pdl = f->pdl && f->sweep_pdl;
-  if (f->sweep_tma && f->sweep_ctas[phase2 ? 1 : 0] > 0 && len == 1)
-    return fit_launch_sweep_tma(f, f->sweep_ctas[phase2 ? 1 : 0], step_off, buf_off, st, pdl);
   int sg_ = 0, sb_ = 0;
   fit_sweep_geometry(f, phase2, &sg_, &sb_);
-  return fit_launch_sweep_kernel(f, dim3(sg_), dim3(sb_), step_off, len, buf_off, st, pdl);
+  return fit_launch_sweep_kernel(f, dim3(sg_), dim3(sb_), step_off, len, buf_off, st, f->pdl);
 }
 
 // Encodes step (*step_base + step_off) into f->enc from state S_{step - npeek} in buffer (step_base[1] + buf_off) & 1,
@@ -1700,13 +1545,12 @@ static int fit_enqueue_step(Fit* f, int step_off, bool phase2, bool epoch_end, c
   const Op dR{f->dR, C, p_nc}, dr2{f->dr2, Hr, p_nr}, dr1{f->dr1, Hr, p_nr};
   cudaStream_t sB = f->sB, sC = f->sC, sD = f->sD, sE = f->sE;
   const bool pdl = f->pdl;
-  // Kernels that only feed Adam(small) -- weight gradients, the residual MLP's backward, the dG scatter -- can be launched
-  // below the chain's priority (DVT_FIT_OFFPATH_PRIO; measured neutral, see fit_create).  What does help is keeping the
-  // weight-gradient GEMMs small (wcap): the CUPTI timeline (tools/fit_timeline.py) shows the next kernel of the critical
-  // path waiting one CTA lifetime (~12 us, twice per step) whenever a finishing data-gradient GEMM hands its SMs to the
-  // queued CTAs of a weight-gradient GEMM -- every 3xTF32 CTA fills the shared memory of its SM.
-  const int off = f->off_path_prio_drop;
-  const int wide = f->x3_wide_min_n[phase2 ? 1 : 0], wcap = f->wgrad_sms;
+  // The weight-gradient GEMMs only feed Adam(small), and are kept small (wcap): the CUPTI timeline (tools/fit_timeline.py)
+  // shows the next kernel of the critical path waiting one CTA lifetime (~12 us, twice per step) whenever a finishing
+  // data-gradient GEMM hands its SMs to the queued CTAs of a weight-gradient GEMM -- every 3xTF32 CTA fills the shared
+  // memory of its SM.
+  const int wcap = f->wgrad_sms;
+  const GemmOpt gopt{impl, pdl, f->x3_wide_min_n[phase2 ? 1 : 0]};
   auto fork = [&](cudaStream_t to, cudaEvent_t e) -> int {
     DVT_CUDA_OK(cudaEventRecord(e, st));
     DVT_CUDA_OK(cudaStreamWaitEvent(to, e, 0));
@@ -1725,12 +1569,12 @@ static int fit_enqueue_step(Fit* f, int step_off, bool phase2, bool epoch_end, c
   const bool pipe = f->pipe[phase2 ? 1 : 0];
   if (!pipe) FIT_RC(fit_enqueue_encode(f, step_off, 0, f->epoch_windows, st));  // else f->enc is already this step's (fit_run)
   if (phase2) {
-    FIT_RC(fit_linear(rawb, n, C, W(f->R1), Hr, sp + f->rb1.off, ACT_RELU, f->r1, f->ld_r, p_r, true, sB, impl, pdl, f->res_x3, 0, wide));
-    FIT_RC(fit_linear(r1, n, Hr, W(f->R2), Hr, sp + f->rb2.off, ACT_RELU, f->r2, f->ld_r, p_r, true, sB, impl, pdl, f->res_x3, 0, wide));
-    FIT_RC(fit_linear(r2, n, Hr, W(f->R3), C, sp + f->rb3.off, ACT_NONE, f->Rout, C, 0, false, sB, impl, pdl, f->res_x3, 0, wide));
+    FIT_RC(fit_linear(rawb, n, C, W(f->R1), Hr, sp + f->rb1.off, ACT_RELU, f->r1, f->ld_r, p_r, true, sB, gopt));
+    FIT_RC(fit_linear(r1, n, Hr, W(f->R2), Hr, sp + f->rb2.off, ACT_RELU, f->r2, f->ld_r, p_r, true, sB, gopt));
+    FIT_RC(fit_linear(r2, n, Hr, W(f->R3), C, sp + f->rb3.off, ACT_NONE, f->Rout, C, 0, false, sB, gopt));
   }
-  FIT_RC(fit_linear(enc, n, Lf, W(f->W1), H1, sp + f->b1.off, ACT_RELU, f->h1, f->ld_h1, p_h1, true, st, impl, pdl, 1, 0, wide));
-  FIT_RC(fit_linear(h1, n, H1, W(f->W2), C, sp + f->b2.off, ACT_NONE, f->Fout, C, 0, false, st, impl, pdl, 1, 0, wide));
+  FIT_RC(fit_linear(enc, n, Lf, W(f->W1), H1, sp + f->b1.off, ACT_RELU, f->h1, f->ld_h1, p_h1, true, st, gopt));
+  FIT_RC(fit_linear(h1, n, H1, W(f->W2), C, sp + f->b2.off, ACT_NONE, f->Fout, C, 0, false, st, gopt));
   FIT_RC(join(sB, f->ev[1]));
   // ---- loss + d pred ----
   LossArgs la;
@@ -1746,11 +1590,11 @@ static int fit_enqueue_step(Fit* f, int step_off, bool phase2, bool epoch_end, c
     FIT_RC(fork(sC, f->ev[3]));
     FIT_RC(fork(sE, f->ev[11]));
   }
-  FIT_RC(fit_wgrad(dpred, n, C, h1, H1, sg + f->W2.off, sg + f->b2.off, f->wg_sem + 0 * FIT_SEM_TILES, sB, impl, pdl, f->wgrad_x3, off, wide, wcap));   // side B
-  FIT_RC(fit_dgrad(dpred, n, C, W(f->W2), H1, f->h1, f->ld_h1, f->dh1, H1, p_nh, true, st, impl, pdl, 1, 0, wide));  // main
+  FIT_RC(fit_wgrad(dpred, n, C, h1, H1, sg + f->W2.off, sg + f->b2.off, f->wg_sem + 0 * FIT_SEM_TILES, wcap, sB, gopt));   // side B
+  FIT_RC(fit_dgrad(dpred, n, C, W(f->W2), H1, f->h1, f->ld_h1, f->dh1, H1, p_nh, true, st, gopt));  // main
   FIT_RC(fork(sB, f->ev[4]));  // dh1 ready
-  FIT_RC(fit_wgrad(dh1, n, H1, enc, Lf, sg + f->W1.off, sg + f->b1.off, f->wg_sem + 1 * FIT_SEM_TILES, sB, impl, pdl, f->wgrad_x3, off, wide, wcap));  // side B (reads enc)
-  FIT_RC(fit_dgrad(dh1, n, H1, W(f->W1), Lf, nullptr, 0, f->denc, Lf, 0, false, st, impl, pdl, 1, 0, wide));
+  FIT_RC(fit_wgrad(dh1, n, H1, enc, Lf, sg + f->W1.off, sg + f->b1.off, f->wg_sem + 1 * FIT_SEM_TILES, wcap, sB, gopt));  // side B (reads enc)
+  FIT_RC(fit_dgrad(dh1, n, H1, W(f->W1), Lf, nullptr, 0, f->denc, Lf, 0, false, st, gopt));
   if (!phase2) {
     // dG (+ grid_sample's neighbour shares) on side C, enqueued BEHIND the two data-gradient GEMMs: launched beside them, its
     // 256 small CTAs take the registers the GEMM CTAs need and delay the critical path.
@@ -1758,7 +1602,7 @@ static int fit_enqueue_step(Fit* f, int step_off, bool phase2, bool epoch_end, c
     ScatterArgs sa;
     sa.dpred = f->dpred; sa.plane = p_nc; sa.sr = sr; sa.gG = sg + f->G.off; sa.n = n; sa.C = C; sa.hw = f->hw;
     sa.gw = f->gw; sa.gh = f->gh; sa.ax_i0 = f->ax_i0; sa.ax_w0 = f->ax_w0; sa.ax_w1 = f->ax_w1;
-    DVT_CUDA_OK(launch_kx(LaunchOpt{pdl, off}, fit_g_scatter_kernel, dim3((f->hw * 32 + tb - 1) / tb), dim3(tb), 0, sC, sa));
+    DVT_CUDA_OK(launch_k(pdl, fit_g_scatter_kernel, dim3((f->hw * 32 + tb - 1) / tb), dim3(tb), 0, sC, sa));
     DVT_CUDA_OK(cudaGetLastError());
     count_launch();
   }
@@ -1773,13 +1617,13 @@ static int fit_enqueue_step(Fit* f, int step_off, bool phase2, bool epoch_end, c
   if (phase2) {
     // residual MLP backward: the data-gradient chain on side C, the weight-gradient GEMMs that do not feed it on side E
     //   side C: dr2 = dR.R3 -> dr1 = dr2.R2 -> dR1      side E: dR3 (needs dR, r2 only) -> [dr2 ready] dR2
-    FIT_RC(fit_dgrad(dR, n, C, W(f->R3), Hr, f->r2, f->ld_r, f->dr2, Hr, p_nr, true, sC, impl, pdl, f->res_x3, off, wide));
+    FIT_RC(fit_dgrad(dR, n, C, W(f->R3), Hr, f->r2, f->ld_r, f->dr2, Hr, p_nr, true, sC, gopt));
     DVT_CUDA_OK(cudaEventRecord(f->ev[12], sC));                                              // dr2 ready
-    FIT_RC(fit_dgrad(dr2, n, Hr, W(f->R2), Hr, f->r1, f->ld_r, f->dr1, Hr, p_nr, true, sC, impl, pdl, f->res_x3, off, wide));
-    FIT_RC(fit_wgrad(dr1, n, Hr, rawb, C, sg + f->R1.off, sg + f->rb1.off, f->wg_sem + 2 * FIT_SEM_TILES, sC, impl, pdl, f->res_x3, off, wide, wcap));
-    FIT_RC(fit_wgrad(dR, n, C, r2, Hr, sg + f->R3.off, sg + f->rb3.off, f->wg_sem + 3 * FIT_SEM_TILES, sE, impl, pdl, f->res_x3, off, wide, wcap));
+    FIT_RC(fit_dgrad(dr2, n, Hr, W(f->R2), Hr, f->r1, f->ld_r, f->dr1, Hr, p_nr, true, sC, gopt));
+    FIT_RC(fit_wgrad(dr1, n, Hr, rawb, C, sg + f->R1.off, sg + f->rb1.off, f->wg_sem + 2 * FIT_SEM_TILES, wcap, sC, gopt));
+    FIT_RC(fit_wgrad(dR, n, C, r2, Hr, sg + f->R3.off, sg + f->rb3.off, f->wg_sem + 3 * FIT_SEM_TILES, wcap, sE, gopt));
     DVT_CUDA_OK(cudaStreamWaitEvent(sE, f->ev[12], 0));
-    FIT_RC(fit_wgrad(dr2, n, Hr, r1, Hr, sg + f->R2.off, sg + f->rb2.off, f->wg_sem + 4 * FIT_SEM_TILES, sE, impl, pdl, f->res_x3, off, wide, wcap));
+    FIT_RC(fit_wgrad(dr2, n, Hr, r1, Hr, sg + f->R2.off, sg + f->rb2.off, f->wg_sem + 4 * FIT_SEM_TILES, wcap, sE, gopt));
     FIT_RC(join(sE, f->ev[13]));
   }
   FIT_RC(join(sC, f->ev[5]));
@@ -1934,7 +1778,6 @@ int fit_run(Fit* f, int count, int use_graphs, cudaStream_t caller, int impl) {
       cur += 1;
     }
   }
-  f->cur_host = end;
   f->cur_step = end;
   DVT_CUDA_OK(cudaEventRecord(f->ev_run_done[f->idx_slot], st));
   f->run_done_valid[f->idx_slot] = true;
@@ -1942,18 +1785,16 @@ int fit_run(Fit* f, int count, int use_graphs, cudaStream_t caller, int impl) {
 }
 
 // One dense table sweep (the Adam step of the CURRENT device step counter, state buffer ping-pong not advanced) on `st`:
-// the hook bench.py / ncu use to time the dominant HBM-bound kernel alone.  ctas: > 0 persistent 1024-thread CTAs, 0 the
-// many-small-CTA geometry.  The optimiser state is modified: call it after the fit results have been read.
+// the hook bench.py / ncu use to time the dominant HBM-bound kernel alone.  ctas: > 0 that many persistent CTAs of
+// FIT_SWEEP_CTA_THREADS threads, 0 the many-small-CTA geometry.  The optimiser state is modified: call it after the fit
+// results have been read.
 int fit_sweep_once(Fit* f, int ctas, cudaStream_t st) {
   DVT_REQUIRE(f->sc_main && f->num_iters > 0, "fit_sweep_once: call fit_begin first");
   // (no device read-back here: a blocking copy per call would put ~20 us of host latency between back-to-back launches
   //  and into every event-timed measurement; the host mirror of the step counter is enough for the bounds check)
-  DVT_REQUIRE(f->cur_host <= f->num_iters, "fit_sweep_once: step counter %d beyond the schedule", f->cur_host);
-  // ctas > 0: persistent CTAs as in the pipelined schedule (TMA-staged kernel unless DVT_FIT_SWEEP_TMA=0);
-  // ctas < 0: -ctas persistent CTAs of the plain-load kernel; 0: the many-small-CTA geometry of the sequential schedule
-  if (ctas > 0 && f->sweep_tma) return fit_launch_sweep_tma(f, std::min(ctas, num_sms()), 0, 0, st, false);
-  const int n = ctas < 0 ? -ctas : ctas;
-  const int grid = n > 0 ? std::min(n, num_sms()) : num_sms() * 8, block = n > 0 ? 1024 : 256;
+  DVT_REQUIRE(f->cur_step <= f->num_iters, "fit_sweep_once: step counter %d beyond the schedule", f->cur_step);
+  DVT_REQUIRE(ctas >= 0, "fit_sweep_once: %d persistent CTAs", ctas);
+  const int grid = ctas > 0 ? std::min(ctas, num_sms()) : num_sms() * 8, block = ctas > 0 ? FIT_SWEEP_CTA_THREADS : 256;
   return fit_launch_sweep_kernel(f, dim3(grid), dim3(block), 0, 1, 0, st, false);
 }
 
@@ -1993,15 +1834,16 @@ int fit_query(Fit* f, const float* coords, int n, float* out, cudaStream_t st, i
   FIT_RC(fit_before_caller(f, st));
   const int C = f->C, H1 = C / 2;
   const size_t cap = (size_t)f->q_cap, wp = (size_t)f->n_small;
+  const GemmOpt gopt{impl, false, 0};  // no PDL, 128 x 64 tiles
   const StepRows sr{nullptr, f->step_base, 0};
   fit_encode_kernel<2><<<(n * f->grid.n_levels * 4 + 255) / 256, 256, 0, st>>>(
       f->grid, f->tb, f->tb.p[f->cur_buf], coords, sr, n, f->q_enc, f->ld_enc, cap * f->ld_enc, nullptr, 0.f, 0, 0);
   DVT_CUDA_OK(cudaGetLastError());
   count_launch();
   FIT_RC(fit_linear(Op{f->q_enc, f->ld_enc, cap * f->ld_enc}, n, f->Lf, Op{f->wsplit + f->W1.off, f->Lf, wp}, H1,
-                    f->sp + f->b1.off, ACT_RELU, f->q_h1, f->ld_h1, cap * f->ld_h1, true, st, impl));
+                    f->sp + f->b1.off, ACT_RELU, f->q_h1, f->ld_h1, cap * f->ld_h1, true, st, gopt));
   FIT_RC(fit_linear(Op{f->q_h1, f->ld_h1, cap * f->ld_h1}, n, H1, Op{f->wsplit + f->W2.off, H1, wp}, C, f->sp + f->b2.off,
-                    ACT_NONE, out, C, 0, false, st, impl));
+                    ACT_NONE, out, C, 0, false, st, gopt));
   return DVT_OK;
 }
 
@@ -2012,16 +1854,17 @@ int fit_residual(Fit* f, const float* raw, int n, float* out, cudaStream_t st, i
   FIT_RC(fit_before_caller(f, st));
   const int C = f->C, Hr = C / 4;
   const size_t cap = (size_t)f->q_cap, wp = (size_t)f->n_small;
+  const GemmOpt gopt{impl, false, 0};  // no PDL, 128 x 64 tiles
   const StepRows sr{nullptr, f->step_base, 0};
   fit_gather_rows_kernel<<<n, 192, 0, st>>>(raw, C, sr, n, f->q_raw, f->ld_raw, cap * f->ld_raw);
   DVT_CUDA_OK(cudaGetLastError());
   count_launch();
   FIT_RC(fit_linear(Op{f->q_raw, f->ld_raw, cap * f->ld_raw}, n, C, Op{f->wsplit + f->R1.off, C, wp}, Hr, f->sp + f->rb1.off,
-                    ACT_RELU, f->q_r1, f->ld_r, cap * f->ld_r, true, st, impl));
+                    ACT_RELU, f->q_r1, f->ld_r, cap * f->ld_r, true, st, gopt));
   FIT_RC(fit_linear(Op{f->q_r1, f->ld_r, cap * f->ld_r}, n, Hr, Op{f->wsplit + f->R2.off, Hr, wp}, Hr, f->sp + f->rb2.off,
-                    ACT_RELU, f->q_r2, f->ld_r, cap * f->ld_r, true, st, impl));
+                    ACT_RELU, f->q_r2, f->ld_r, cap * f->ld_r, true, st, gopt));
   FIT_RC(fit_linear(Op{f->q_r2, f->ld_r, cap * f->ld_r}, n, Hr, Op{f->wsplit + f->R3.off, Hr, wp}, C, f->sp + f->rb3.off,
-                    ACT_NONE, out, C, 0, false, st, impl));
+                    ACT_NONE, out, C, 0, false, st, gopt));
   return DVT_OK;
 }
 

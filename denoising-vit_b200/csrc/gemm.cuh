@@ -59,11 +59,10 @@ struct GemmShape {
   // 3xTF32 ("x3"): fp32-accurate product on the tensor cores.  Each fp32 operand is stored as two planes
   // (hi = TF32-exact part at the base pointer, lo = remainder at base + plane elements) and the kernel accumulates
   // A_hi.B_hi + A_hi.B_lo + A_lo.B_hi.
-  int x3 = 0;    // 1: 3xTF32 as described; 2: same operand layout, but only A_hi.B_hi (plain TF32 accuracy)
+  int x3 = 0;    // 1: 3xTF32 as described
   size_t plane_a = 0, plane_b = 0;
   int pdl = 0;   // launch with programmatic stream serialisation (the kernel calls pdl_wait() after its set-up)
   int x3_wide_min_n = 0;  // x3: 128 x 128 tiles when N >= this (0: always 128 x 64)
-  int prio_drop = 0;  // > 0: launch that many priority levels below the highest (common.cuh LaunchOpt)
 };
 
 // FIT = true (the 3xTF32 kernels of the stage-1 fit): epilogue features only other callers use -- GELU, the bf16 mask with

@@ -206,8 +206,9 @@ int dvt_fit_query(dvt_fit_t* h, const float* coords, int n, float* out, void* st
 int dvt_fit_residual(dvt_fit_t* h, const float* raw, int n, float* out, void* stream);
 /* Measurement hook: ONE dense Adam sweep of the hash table (the dominant HBM-bound kernel of HP-2; reference: the
  * torch.optim.Adam.step() over tcnn's dense table gradient, main_img_denoising.py:88) on `stream`, outside the step
- * schedule.  ctas > 0: that many persistent 1024-thread CTAs; 0: 8 x #SM CTAs of 256 threads.  Modifies the optimiser
- * state -- call after the results of the fit have been read.  Requires dvt_fit_begin. */
+ * schedule.  ctas > 0: that many persistent 1024-thread CTAs (at most one per SM); 0: 8 x #SM CTAs of 256 threads; a
+ * negative value is an error.  Modifies the optimiser state -- call after the results of the fit have been read.
+ * Requires dvt_fit_begin. */
 int dvt_fit_sweep_once(dvt_fit_t* h, int ctas, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------

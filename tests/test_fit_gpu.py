@@ -188,7 +188,7 @@ def test_fit_matches_reference_golden(name, impl, graph_steps, pipeline, monkeyp
     encode); pipeline=0: sequential schedule.  Both must reproduce the reference run."""
     from dvt.fit import FitEngine
     monkeypatch.setenv("DVT_FIT_PIPELINE", str(pipeline))   # read by dvt_fit_create
-    monkeypatch.setenv("DVT_FIT_SWEEP_CTAS", "6,3")         # pipelined in both phases (the default is phase 1 only)
+    monkeypatch.setenv("DVT_FIT_SWEEP_CTAS", "6,3")         # few persistent sweep CTAs in both phases
     cfg, z = _golden(name)
     feats, coords, init, idx, den, field, _ = _setup(cfg)
     assert int(idx.sum()) == int(z["idx_checksum"][0])  # same sampling stream as the reference run
@@ -518,52 +518,3 @@ def test_encode_with_partial_last_warp(n_levels, n):
     torch.cuda.synchronize()
     assert (got - ref).abs().max().item() < 2e-3 * max(1.0, ref.abs().max().item())
     assert _L().device_error() == 0
-
-
-def test_sweep_kernels_agree(monkeypatch):
-    """The TMA-staged dense Adam sweep (`fit_adam_table_tma_kernel`, the default of the pipelined schedule) against the
-    plain-load kernel: (i) one sweep from the same state is BIT-identical (same adam1() arithmetic), incl. a ragged last
-    chunk; (ii) whole fits with either kernel agree within the tolerance below."""
-    import dvt.models as DVT
-    from dvt.fit import FitEngine
-    # (i) 10 levels on purpose: 1 740 464 entries = 3399 chunks of 512 + a ragged one
-    C, h, w, bsz, L, T = 64, 6, 6, 128, 10, 8
-    field = DVT.NeuralFeatureField(feat_dim=C, n_levels=L)
-    assert (field.meta.n_params // 8) % 512 != 0
-    g = torch.Generator(device="cuda").manual_seed(0)
-    bank = torch.randn(4 * h * w, C, device="cuda", generator=g)
-    co = torch.rand(4 * h * w, 2, device="cuda", generator=g)
-    idx = np.random.RandomState(0).randint(0, 4 * h * w, (T, bsz))
-    hyper = dict(lr=0.01, min_lr=0.001, warmup_iters=0, freeze_after=0.5, weight_decay=0.37, loss_scale=1024.0)
-    outs = []
-    for ctas in (7, -7, 0):          # TMA-staged on 7 CTAs, plain loads on 7 CTAs, plain loads on the full grid
-        monkeypatch.setenv("DVT_FIT_SWEEP_TMA", "1" if ctas > 0 else "0")
-        eng = FitEngine(C, h, w, bsz, field.meta)
-        eng.init_params(5)
-        eng.begin(bank, co, idx, **hyper)
-        eng.sweep_once(ctas)
-        outs.append(eng.get_param("table.next", field.neural_field.params).cpu())
-        torch.cuda.synchronize()
-        assert _L().device_error() == 0
-        start = eng.get_param("table", field.neural_field.params).cpu()
-    assert not torch.equal(outs[0], start), "the sweep must have changed the table (weight decay 0.37, lr 0.01)"
-    assert torch.equal(outs[0], outs[1]) and torch.equal(outs[1], outs[2])
-    # (ii) whole fits
-    cfg, z = _golden("hashed_L16")
-    res = []
-    for tma in ("1", "0"):
-        monkeypatch.setenv("DVT_FIT_SWEEP_TMA", tma)     # read by dvt_fit_create
-        monkeypatch.setenv("DVT_FIT_SWEEP_CTAS", "5,3")
-        feats, coords, init, idx2, den, fld, _ = _setup(cfg)
-        eng = FitEngine(cfg["C"], cfg["h"], cfg["w"], cfg["bsz"], fld.meta)
-        eng.fit(den, fld, feats.reshape(-1, cfg["C"]).cuda().contiguous(), coords.reshape(-1, 2).cuda().contiguous(), idx2,
-                graph_steps=5, lr=cfg["lr"], min_lr=cfg["min_lr"], warmup_iters=cfg["warmup_iters"],
-                freeze_after=cfg["freeze_after"], weight_decay=cfg["weight_decay"], loss_scale=cfg["loss_scale"])
-        torch.cuda.synchronize()
-        assert _L().device_error() == 0
-        res.append((eng.get_param("table", init["table"]).cpu() - init["table"], eng.losses().copy(),
-                    eng.query(coords[-1:].cuda()).cpu()))
-    (ta, la, qa), (tb, lb, qb) = res
-    assert F.cosine_similarity(ta.flatten().double(), tb.flatten().double(), dim=0).item() > 0.9999
-    assert np.allclose(la, lb, rtol=1e-3, atol=1e-5)
-    assert _min_cos(qa, torch.from_numpy(z["denoised_feats"])) > 0.999

@@ -114,6 +114,7 @@ def test_sweep_once_applies_one_step(monkeypatch):
     """The measurement hook sweeps exactly one Adam step whatever the window: from zero moments and no gradient, weight
     decay 0.37 and lr 0.01 (no warm-up) move every parameter by lr / (1 - b1) * 0.1 * sign(p) = 0.01 sign(p)."""
     import dvt.models as DVT
+    from dvt._lib import DvtError
     from dvt.fit import FitEngine
     C, h, w, bsz, L, T = 64, 6, 6, 128, 10, 8
     field = DVT.NeuralFeatureField(feat_dim=C, n_levels=L)
@@ -123,9 +124,8 @@ def test_sweep_once_applies_one_step(monkeypatch):
     idx = np.random.RandomState(0).randint(0, 4 * h * w, (T, bsz))
     hyper = dict(lr=0.01, min_lr=0.001, warmup_iters=0, freeze_after=0.5, weight_decay=0.37, loss_scale=1024.0)
     outs = []
-    for k, ctas in (("1", -7), ("4", -7), ("8", 0)):
+    for k, ctas in (("1", 7), ("4", 7), ("8", 0)):
         monkeypatch.setenv("DVT_FIT_SWEEP_STEPS", k)
-        monkeypatch.setenv("DVT_FIT_SWEEP_TMA", "0")
         eng = FitEngine(C, h, w, bsz, field.meta)
         eng.init_params(5)
         eng.begin(bank, co, idx, **hyper)
@@ -136,6 +136,8 @@ def test_sweep_once_applies_one_step(monkeypatch):
     assert torch.equal(outs[0], outs[1]) and torch.equal(outs[1], outs[2])
     # (approximate sqrt / division inside adam1(); a second step would move every parameter by another 0.01)
     assert (outs[0] - (start - 0.01 * start.sign())).abs().max().item() < 1e-4
+    with pytest.raises(DvtError):
+        eng.sweep_once(-7)
 
 
 def test_windowed_sweep_full_size(monkeypatch):

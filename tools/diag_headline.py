@@ -18,7 +18,7 @@ from dvt.fit import FitEngine  # noqa: E402
 
 
 def run(tag, env, impl=-1, graph_steps=20):
-    for k in ("DVT_FIT_PIPELINE", "DVT_FIT_SWEEP_CTAS", "DVT_FIT_SWEEP_TMA", "DVT_FIT_PDL"):
+    for k in ("DVT_FIT_PIPELINE", "DVT_FIT_SWEEP_CTAS", "DVT_FIT_PDL"):
         os.environ.pop(k, None)
     os.environ.update(env)
     cfg, z = T._golden("headline_2000")
@@ -51,7 +51,6 @@ if __name__ == "__main__":
     b, lb = run("same again (run-to-run noise)", {})
     c, lc = run("sequential schedule", {"DVT_FIT_PIPELINE": "0"})
     d, ld = run("sequential, no graphs", {"DVT_FIT_PIPELINE": "0"}, graph_steps=0)
-    e, le = run("sequential, plain-load sweep", {"DVT_FIT_PIPELINE": "0", "DVT_FIT_SWEEP_TMA": "0"})
     cs = lambda x, y: F.cosine_similarity(x.reshape(-1, 768), y.reshape(-1, 768), dim=-1).min().item()  # noqa: E731
     print(f"run-to-run min cos {cs(a, b):.6f}; pipelined vs sequential {cs(a, c):.6f}; graphs vs none {cs(c, d):.6f}")
     if len(sys.argv) > 1 and sys.argv[1] == "simt":

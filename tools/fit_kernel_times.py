@@ -42,8 +42,8 @@ def main():
         torch.cuda.synchronize()
     tot, cnt = defaultdict(float), defaultdict(int)
     for e in prof.events():
-        for key in ("fit_encode_kernel", "fit_adam_table_kernel", "fit_adam_table_tma_kernel"):
-            if key in e.name and (key != "fit_adam_table_kernel" or "tma" not in e.name):
+        for key in ("fit_encode_kernel", "fit_adam_table_kernel"):
+            if key in e.name:
                 tot[key] += e.device_time_total
                 cnt[key] += 1
     for key in sorted(tot):

@@ -13,7 +13,7 @@ int vit_load(Vit* v, const char* name, const float* src, size_t numel);
 int vit_reserve(Vit* v, size_t tokens, size_t patches);
 int vit_forward(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int stride, const float* pos_patch,
                 const float* prefix_rows, int layer_index, int apply_norm, float* out, int out_all_tokens,
-                cudaStream_t stream, int impl);
+                cudaStream_t stream);
 int vit_patch(const Vit* v);
 int vit_prefix(const Vit* v);
 struct Fit;
@@ -28,11 +28,11 @@ int fit_begin(Fit* f, const float* bank, const float* coords, size_t bank_rows, 
               int validate, cudaStream_t caller);
 int fit_check(Fit* f);
 int fit_set_artifact_grid(Fit* f, const int* i0, const float* w0, const float* w1);
-int fit_run(Fit* f, int count, int use_graphs, cudaStream_t st, int impl);
+int fit_run(Fit* f, int count, int use_graphs, cudaStream_t st);
 int fit_losses(Fit* f, float* dst_host, int num_iters);
 int fit_losses_async(Fit* f, float* dst, int num_iters, cudaStream_t caller);
-int fit_query(Fit* f, const float* coords, int n, float* out, cudaStream_t st, int impl);
-int fit_residual(Fit* f, const float* raw, int n, float* out, cudaStream_t st, int impl);
+int fit_query(Fit* f, const float* coords, int n, float* out, cudaStream_t st);
+int fit_residual(Fit* f, const float* raw, int n, float* out, cudaStream_t st);
 int fit_sweep_once(Fit* f, int ctas, cudaStream_t st);
 int view_crops(const float* image, int H, int W, const int* boxes_host, const int* flips_host, int V, void* out, bool out_bf16,
                int OH, int OW, float* coords_out, int hp, int wp, cudaStream_t st);
@@ -62,7 +62,7 @@ int launch_layernorm_bwd_grouped(const float* x, const float* gamma, const float
                                  float* dbeta, float* workspace, int rows, int C, float eps, int in_group, int skip,
                                  cudaStream_t st);
 int launch_vit_embed_fwd(const __nv_bfloat16* patches, int Kp, const __nv_bfloat16* w, const float* bias, const float* pos_patch,
-                         const float* prefix_rows, int B, int np, int prefix, int C, float* out, cudaStream_t st, int impl);
+                         const float* prefix_rows, int B, int np, int prefix, int C, float* out, cudaStream_t st);
 int launch_attention_bwd_det(const __nv_bfloat16* qkv, const __nv_bfloat16* out, const __nv_bfloat16* dout, const float* lse,
                              __nv_bfloat16* dqkv, float* delta, int B, int N, int heads, cudaStream_t stream, int head_dim);
 int launch_colsum_ordered(const void* in, bool bf16, int ld, int rows, int cols, float* out, float* workspace, cudaStream_t st);
@@ -77,17 +77,13 @@ int launch_seg_slide_accumulate(const float* logits, int h, int w, int K, int y1
 int launch_seg_predict_hist(float* acc, const float* count, int K, int Hc, int Wc, const uint8_t* labels, int Ho, int Wo,
                             unsigned long long* hist, cudaStream_t st);
 const char* last_error();
-extern int g_debug_impl_override;
-int g_debug_impl_override = -1;
 }  // namespace dvt
 
 using namespace dvt;
 
-static inline int eff_impl() { return dvt::g_debug_impl_override >= 0 ? dvt::g_debug_impl_override : -1; }
-
 extern "C" {
 
-int dvt_version(void) { return 100; }
+int dvt_version(void) { return 101; }
 
 const char* dvt_last_error(void) { return dvt::last_error(); }
 
@@ -107,7 +103,7 @@ int dvt_set_debug_impl(int impl) {
     dvt::set_last_error("dvt_set_debug_impl: impl must be -1, 0 or 1");
     return DVT_ERR_INVALID;
   }
-  dvt::g_debug_impl_override = impl;
+  dvt::set_debug_impl(impl);
   return DVT_OK;
 }
 
@@ -129,31 +125,16 @@ int dvt_gemm_tn(const void* A, int lda, const void* B, int ldb, int dtype, int M
   }
   GemmShape s{M, N, K, splits < 1 ? 1 : splits};
   return launch_gemm_tn(A, lda, B, ldb, dtype == DVT_DTYPE_BF16 ? TMAP_BF16 : TMAP_F32, s, e,
-                        reinterpret_cast<cudaStream_t>(stream), eff_impl());
+                        reinterpret_cast<cudaStream_t>(stream));
 }
 
 int dvt_gemm_tn_residual(const void* A, int lda, const void* B, int ldb, int dtype, int M, int N, int K,
-                         const float* bias, const float* gamma, float* x_inout, int ldx, void* stream) {
+                         const float* bias, const float* gamma, float* x_inout, int ldx, void* branch_out_bf16,
+                         int ld_branch, void* stream) {
   DVT_REQUIRE(dtype == DVT_DTYPE_BF16 || dtype == DVT_DTYPE_F32, "dvt_gemm_tn_residual: bad dtype %d", dtype);
   DVT_REQUIRE(A && B && x_inout, "dvt_gemm_tn_residual: null pointer");
-  GemmEpi e;
-  e.bias = bias;
-  e.gamma = gamma;
-  e.out = x_inout;
-  e.ldo = ldx;
-  e.out_mode = OUT_F32_RESID;
-  GemmShape s{M, N, K, 1};
-  return launch_gemm_tn(A, lda, B, ldb, dtype == DVT_DTYPE_BF16 ? TMAP_BF16 : TMAP_F32, s, e,
-                        reinterpret_cast<cudaStream_t>(stream), eff_impl());
-}
-
-int dvt_gemm_tn_residual_ex(const void* A, int lda, const void* B, int ldb, int dtype, int M, int N, int K,
-                            const float* bias, const float* gamma, float* x_inout, int ldx, void* branch_out_bf16,
-                            int ld_branch, void* stream) {
-  DVT_REQUIRE(dtype == DVT_DTYPE_BF16 || dtype == DVT_DTYPE_F32, "dvt_gemm_tn_residual_ex: bad dtype %d", dtype);
-  DVT_REQUIRE(A && B && x_inout, "dvt_gemm_tn_residual_ex: null pointer");
   DVT_REQUIRE(!branch_out_bf16 || (ld_branch >= N && ld_branch % 4 == 0),
-              "dvt_gemm_tn_residual_ex: ld_branch=%d must be >= N=%d and a multiple of 4", ld_branch, N);
+              "dvt_gemm_tn_residual: ld_branch=%d must be >= N=%d and a multiple of 4", ld_branch, N);
   GemmEpi e;
   e.bias = bias;
   e.gamma = gamma;
@@ -164,7 +145,7 @@ int dvt_gemm_tn_residual_ex(const void* A, int lda, const void* B, int ldb, int 
   e.ld_branch = ld_branch;
   GemmShape s{M, N, K, 1};
   return launch_gemm_tn(A, lda, B, ldb, dtype == DVT_DTYPE_BF16 ? TMAP_BF16 : TMAP_F32, s, e,
-                        reinterpret_cast<cudaStream_t>(stream), eff_impl());
+                        reinterpret_cast<cudaStream_t>(stream));
 }
 
 int dvt_layernorm(const float* x, int ldx, const float* gamma, const float* beta, void* y, int ldy, int y_dtype,
@@ -175,43 +156,16 @@ int dvt_layernorm(const float* x, int ldx, const float* gamma, const float* beta
                           reinterpret_cast<cudaStream_t>(stream));
 }
 
-int dvt_attention_fwd(const void* qkv_bf16, void* out_bf16, int B, int N, int heads, void* stream) {
+int dvt_attention_fwd(const void* qkv_bf16, void* out_bf16, float* lse, int B, int N, int heads, int head_dim,
+                      void* stream) {
   DVT_REQUIRE(qkv_bf16 && out_bf16, "dvt_attention_fwd: null pointer");
-  int impl = eff_impl();
-  if (impl < 0) impl = default_gemm_impl();
   return launch_attention(reinterpret_cast<const __nv_bfloat16*>(qkv_bf16), reinterpret_cast<__nv_bfloat16*>(out_bf16),
-                          B, N, heads, reinterpret_cast<cudaStream_t>(stream), impl);
-}
-
-int dvt_attention_fwd_hd(const void* qkv_bf16, void* out_bf16, int B, int N, int heads, int head_dim, void* stream) {
-  DVT_REQUIRE(qkv_bf16 && out_bf16, "dvt_attention_fwd_hd: null pointer");
-  int impl = eff_impl();
-  if (impl < 0) impl = default_gemm_impl();
-  return launch_attention(reinterpret_cast<const __nv_bfloat16*>(qkv_bf16), reinterpret_cast<__nv_bfloat16*>(out_bf16),
-                          B, N, heads, reinterpret_cast<cudaStream_t>(stream), impl, nullptr, head_dim);
+                          B, N, heads, reinterpret_cast<cudaStream_t>(stream), lse, head_dim);
 }
 
 /* ---- stage-2 training operators (SURVEY.md 8(f-2)) ---- */
-int dvt_attention_fwd_lse(const void* qkv_bf16, void* out_bf16, float* lse, int B, int N, int heads, void* stream) {
-  DVT_REQUIRE(qkv_bf16 && out_bf16 && lse, "dvt_attention_fwd_lse: null pointer");
-  return launch_attention(reinterpret_cast<const __nv_bfloat16*>(qkv_bf16), reinterpret_cast<__nv_bfloat16*>(out_bf16),
-                          B, N, heads, reinterpret_cast<cudaStream_t>(stream), 0, lse);
-}
 int dvt_attention_bwd(const void* qkv_bf16, const void* out_bf16, const void* dout_bf16, const float* lse, void* dqkv_bf16,
-                      float* dq_workspace, float* delta_workspace, int B, int N, int heads, void* stream) {
-  return launch_attention_bwd(reinterpret_cast<const __nv_bfloat16*>(qkv_bf16), reinterpret_cast<const __nv_bfloat16*>(out_bf16),
-                              reinterpret_cast<const __nv_bfloat16*>(dout_bf16), lse, reinterpret_cast<__nv_bfloat16*>(dqkv_bf16),
-                              dq_workspace, delta_workspace, B, N, heads, reinterpret_cast<cudaStream_t>(stream), 64);
-}
-int dvt_attention_fwd_lse_hd(const void* qkv_bf16, void* out_bf16, float* lse, int B, int N, int heads, int head_dim,
-                             void* stream) {
-  DVT_REQUIRE(qkv_bf16 && out_bf16 && lse, "dvt_attention_fwd_lse_hd: null pointer");
-  return launch_attention(reinterpret_cast<const __nv_bfloat16*>(qkv_bf16), reinterpret_cast<__nv_bfloat16*>(out_bf16),
-                          B, N, heads, reinterpret_cast<cudaStream_t>(stream), 0, lse, head_dim);
-}
-int dvt_attention_bwd_hd(const void* qkv_bf16, const void* out_bf16, const void* dout_bf16, const float* lse,
-                         void* dqkv_bf16, float* dq_workspace, float* delta_workspace, int B, int N, int heads, int head_dim,
-                         void* stream) {
+                      float* dq_workspace, float* delta_workspace, int B, int N, int heads, int head_dim, void* stream) {
   return launch_attention_bwd(reinterpret_cast<const __nv_bfloat16*>(qkv_bf16), reinterpret_cast<const __nv_bfloat16*>(out_bf16),
                               reinterpret_cast<const __nv_bfloat16*>(dout_bf16), lse, reinterpret_cast<__nv_bfloat16*>(dqkv_bf16),
                               dq_workspace, delta_workspace, B, N, heads, reinterpret_cast<cudaStream_t>(stream), head_dim);
@@ -227,15 +181,18 @@ int dvt_gelu(const void* in_bf16, void* out_bf16, size_t n, void* stream) {
   return launch_gelu(reinterpret_cast<const __nv_bfloat16*>(in_bf16), reinterpret_cast<__nv_bfloat16*>(out_bf16), n,
                      reinterpret_cast<cudaStream_t>(stream));
 }
-int dvt_gemm_bf16_bwd(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, int M, int N, int K, void* out,
-                      int ldo, int out_dtype, int splits, const void* gelu_preact_bf16, int ld_preact, void* stream) {
-  DVT_REQUIRE(A && B && out, "dvt_gemm_bf16_bwd: null pointer");
+int dvt_gemm_bf16(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, int M, int N, int K, void* out,
+                  int ldo, int out_dtype, int splits, const void* gelu_preact_bf16, int ld_preact, float* last_col_out,
+                  void* stream) {
+  DVT_REQUIRE(A && B && out, "dvt_gemm_bf16: null pointer");
   GemmEpi e;
   e.out = out;
   e.ldo = ldo;
-  if (splits > 1) {
-    DVT_REQUIRE(out_dtype == DVT_DTYPE_F32 && !gelu_preact_bf16, "dvt_gemm_bf16_bwd: split-K needs plain fp32 output");
+  if (splits > 1 || last_col_out) {
+    DVT_REQUIRE(out_dtype == DVT_DTYPE_F32 && !gelu_preact_bf16,
+                "dvt_gemm_bf16: split-K / last_col_out need plain fp32 output");
     e.out_mode = OUT_F32_ATOMIC;
+    e.last_col_out = last_col_out;
   } else {
     e.out_mode = out_dtype == DVT_DTYPE_BF16 ? OUT_BF16 : OUT_F32;
   }
@@ -247,7 +204,7 @@ int dvt_gemm_bf16_bwd(const void* A, int lda, int a_mn, const void* B, int ldb, 
   GemmShape s{M, N, K, splits < 1 ? 1 : splits};
   s.a_mn = a_mn;
   s.b_mn = b_mn;
-  return launch_gemm_tn(A, lda, B, ldb, TMAP_BF16, s, e, reinterpret_cast<cudaStream_t>(stream), eff_impl());
+  return launch_gemm_tn(A, lda, B, ldb, TMAP_BF16, s, e, reinterpret_cast<cudaStream_t>(stream));
 }
 /* ---- stage-3 (distillation) operators ---- */
 int dvt_swiglu(const void* hpre_bf16, void* out_bf16, size_t M, int Hh, void* stream) {
@@ -266,7 +223,7 @@ int dvt_gemm_bf16_dgrad_swiglu(const void* dy_bf16, int ld_dy, const void* w_bf1
   e.mask_mode = 2;
   GemmShape s{M, Hh, K, 1};
   s.b_mn = 1;
-  return launch_gemm_tn(dy_bf16, ld_dy, w_bf16, ldw, TMAP_BF16, s, e, reinterpret_cast<cudaStream_t>(stream), eff_impl());
+  return launch_gemm_tn(dy_bf16, ld_dy, w_bf16, ldw, TMAP_BF16, s, e, reinterpret_cast<cudaStream_t>(stream));
 }
 int dvt_layerscale_bwd(const float* dx, int ldx, const void* branch_bf16, const float* gamma, void* dbranch_bf16, float* dbias,
                        float* dgamma, float* workspace, int rows, int C, void* stream) {
@@ -278,7 +235,7 @@ int dvt_vit_embed_fwd(const void* patches_bf16, int Kp, const void* w_bf16, cons
                       const float* prefix_rows, int B, int np, int prefix, int C, float* out, void* stream) {
   return launch_vit_embed_fwd(reinterpret_cast<const __nv_bfloat16*>(patches_bf16), Kp,
                               reinterpret_cast<const __nv_bfloat16*>(w_bf16), bias, pos_patch, prefix_rows, B, np, prefix, C,
-                              out, reinterpret_cast<cudaStream_t>(stream), eff_impl());
+                              out, reinterpret_cast<cudaStream_t>(stream));
 }
 int dvt_vit_embed_bwd(const float* dx0, int B, int ntok, int prefix, int C, void* dpatch_bf16, float* dpos, float* dprefix,
                       float* dbias, float* workspace, void* stream) {
@@ -319,12 +276,12 @@ int dvt_gemm_bf16_wgrad_ordered(const void* dy_bf16, int ld_dy, const void* x_bf
   if (s.splits == 1) {
     e.out = out;
     e.out_mode = OUT_F32;
-    return launch_gemm_tn(dy_bf16, ld_dy, x_bf16, ldx, TMAP_BF16, s, e, st, eff_impl());
+    return launch_gemm_tn(dy_bf16, ld_dy, x_bf16, ldx, TMAP_BF16, s, e, st);
   }
   e.out = workspace;
   e.out_mode = OUT_F32_PLANES;
   e.out_plane = (size_t)M * ldo;
-  int rc = launch_gemm_tn(dy_bf16, ld_dy, x_bf16, ldx, TMAP_BF16, s, e, st, eff_impl());
+  int rc = launch_gemm_tn(dy_bf16, ld_dy, x_bf16, ldx, TMAP_BF16, s, e, st);
   if (rc) return rc;
   return launch_splitk_planes_sum(workspace, s.splits, (size_t)M * ldo, M, N, ldo, out, st);
 }
@@ -349,14 +306,8 @@ int dvt_im2col(const void* x, int x_dtype, void* out_bf16, int B, int H, int W, 
 }
 
 int dvt_vit_create(dvt_vit_t** out, int embed, int depth, int heads, int patch, int mlp_hidden, int swiglu,
-                   int layerscale, int prefix_tokens, float ln_eps) {
+                   int layerscale, int prefix_tokens, float ln_eps, int pre_norm, int patch_bias) {
   DVT_REQUIRE(out, "dvt_vit_create: null out");
-  return vit_create(reinterpret_cast<Vit**>(out), embed, depth, heads, patch, mlp_hidden, swiglu, layerscale,
-                    prefix_tokens, ln_eps, 0, 1);
-}
-int dvt_vit_create_ex(dvt_vit_t** out, int embed, int depth, int heads, int patch, int mlp_hidden, int swiglu,
-                      int layerscale, int prefix_tokens, float ln_eps, int pre_norm, int patch_bias) {
-  DVT_REQUIRE(out, "dvt_vit_create_ex: null out");
   return vit_create(reinterpret_cast<Vit**>(out), embed, depth, heads, patch, mlp_hidden, swiglu, layerscale,
                     prefix_tokens, ln_eps, pre_norm, patch_bias);
 }
@@ -378,39 +329,13 @@ int dvt_vit_forward(dvt_vit_t* h, const void* x, int x_dtype, int B, int H, int 
                     int all_tokens, void* stream) {
   DVT_REQUIRE(h, "dvt_vit_forward: null handle");
   return vit_forward(reinterpret_cast<Vit*>(h), x, x_dtype == DVT_DTYPE_BF16, B, H, W, stride, pos_patch, prefix_rows,
-                     layer_index, norm, out, all_tokens, reinterpret_cast<cudaStream_t>(stream), eff_impl());
-}
-
-int dvt_gemm_bf16_ex(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, int M, int N, int K,
-                     void* out, int ldo, int out_dtype, int splits, float* last_col_out, void* stream) {
-  DVT_REQUIRE(A && B && out, "dvt_gemm_bf16_ex: null pointer");
-  GemmEpi e;
-  e.out = out;
-  e.ldo = ldo;
-  if (splits > 1 || last_col_out) {
-    DVT_REQUIRE(out_dtype == DVT_DTYPE_F32, "dvt_gemm_bf16_ex: split-K / last_col_out need fp32 output");
-    e.out_mode = OUT_F32_ATOMIC;
-    e.last_col_out = last_col_out;
-  } else {
-    e.out_mode = out_dtype == DVT_DTYPE_BF16 ? OUT_BF16 : OUT_F32;
-  }
-  GemmShape s{M, N, K, splits < 1 ? 1 : splits};
-  s.a_mn = a_mn;
-  s.b_mn = b_mn;
-  return launch_gemm_tn(A, lda, B, ldb, TMAP_BF16, s, e, reinterpret_cast<cudaStream_t>(stream), eff_impl());
-}
-
-static unsigned long long* g_debug_ts = nullptr;
-int dvt_debug_set_timestamp_buffer(unsigned long long* dev_buf16) {
-  g_debug_ts = dev_buf16;
-  return DVT_OK;
+                     layer_index, norm, out, all_tokens, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int dvt_gemm_f32x3(const float* A, int lda, size_t plane_a, int a_mn, const float* B, int ldb, size_t plane_b, int b_mn,
                    int M, int N, int K, float* out, int ldo, int splits, float* last_col_out, void* stream) {
   DVT_REQUIRE(A && B && out, "dvt_gemm_f32x3: null pointer");
   GemmEpi e;
-  e.debug_ts = g_debug_ts;
   e.out = out;
   e.ldo = ldo;
   if (splits > 1 || last_col_out) {
@@ -421,7 +346,7 @@ int dvt_gemm_f32x3(const float* A, int lda, size_t plane_a, int a_mn, const floa
   }
   GemmShape s{M, N, K, splits < 1 ? 1 : splits};
   s.a_mn = a_mn; s.b_mn = b_mn; s.x3 = 1; s.plane_a = plane_a; s.plane_b = plane_b;
-  return launch_gemm_tn(A, lda, B, ldb, TMAP_F32, s, e, reinterpret_cast<cudaStream_t>(stream), eff_impl());
+  return launch_gemm_tn(A, lda, B, ldb, TMAP_F32, s, e, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int dvt_hashgrid_corners(int n_levels, const float* scale_host, const uint32_t* res_host, const uint32_t* size_host,
@@ -486,7 +411,7 @@ int dvt_fit_check(dvt_fit_t* h) {
 }
 int dvt_fit_run(dvt_fit_t* h, int count, int graph_steps, void* stream) {
   DVT_REQUIRE(h, "dvt_fit_run: null handle");
-  return fit_run(reinterpret_cast<Fit*>(h), count, graph_steps, reinterpret_cast<cudaStream_t>(stream), eff_impl());
+  return fit_run(reinterpret_cast<Fit*>(h), count, graph_steps, reinterpret_cast<cudaStream_t>(stream));
 }
 int dvt_fit_losses(dvt_fit_t* h, float* dst_host, int num_iters) {
   DVT_REQUIRE(h && dst_host, "dvt_fit_losses: null argument");
@@ -498,11 +423,11 @@ int dvt_fit_losses_async(dvt_fit_t* h, float* dst, int num_iters, void* stream) 
 }
 int dvt_fit_query(dvt_fit_t* h, const float* coords, int n, float* out, void* stream) {
   DVT_REQUIRE(h, "dvt_fit_query: null handle");
-  return fit_query(reinterpret_cast<Fit*>(h), coords, n, out, reinterpret_cast<cudaStream_t>(stream), eff_impl());
+  return fit_query(reinterpret_cast<Fit*>(h), coords, n, out, reinterpret_cast<cudaStream_t>(stream));
 }
 int dvt_fit_residual(dvt_fit_t* h, const float* raw, int n, float* out, void* stream) {
   DVT_REQUIRE(h, "dvt_fit_residual: null handle");
-  return fit_residual(reinterpret_cast<Fit*>(h), raw, n, out, reinterpret_cast<cudaStream_t>(stream), eff_impl());
+  return fit_residual(reinterpret_cast<Fit*>(h), raw, n, out, reinterpret_cast<cudaStream_t>(stream));
 }
 int dvt_fit_sweep_once(dvt_fit_t* h, int ctas, void* stream) {
   DVT_REQUIRE(h, "dvt_fit_sweep_once: null handle");

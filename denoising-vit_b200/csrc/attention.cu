@@ -301,8 +301,7 @@ int launch_attention_d(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int 
   const int C = heads * D;
   // D^-0.5: 0.125 for 64 (exact, the historical literal); rounded to fp32 for 80
   const float scale = D == 64 ? 0.125f : (float)(1.0 / 8.94427190999915878564);
-  if (impl == 1) {
-    DVT_REQUIRE(lse == nullptr, "attention (simt debug): the log-sum-exp output needs the tensor-core kernel");
+  if (impl == GEMM_SIMT_DEBUG) {
     DVT_REQUIRE(N <= 12000, "attention (simt debug): N=%d too large", N);
     dim3 grid(N, heads, B);
     attention_simt_kernel<D><<<grid, 32, N * sizeof(float), stream>>>(qkv, out, N, C, scale);
@@ -328,7 +327,7 @@ int launch_attention_d(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int 
   }
   dim3 grid((N + ATT_BQ - 1) / ATT_BQ, heads, B);
   const float sl2 = scale * 1.4426950408889634f;
-  DVT_CUDA_OK(launch_k(g_vit_pdl, attention_tc_kernel<D>, grid, dim3(ATT_THREADS), (size_t)Cfg::SMEM, stream, tm, tm_tail,
+  DVT_CUDA_OK(launch_k(false, attention_tc_kernel<D>, grid, dim3(ATT_THREADS), (size_t)Cfg::SMEM, stream, tm, tm_tail,
                        out, N, C, sl2, lse));
   DVT_CUDA_OK(cudaGetLastError());
   count_launch();
@@ -337,11 +336,13 @@ int launch_attention_d(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int 
 
 }  // namespace
 
-// head_dim: 64 or 80 (C = heads * head_dim).
+// head_dim: 64 or 80 (C = heads * head_dim).  Without lse: the kernel debug_impl() selects.  With lse (training): always
+// the tensor-core kernel, the SIMT kernel does not produce the log-sum-exp.
 int launch_attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int N, int heads, cudaStream_t stream,
-                     int impl, float* lse, int head_dim) {
+                     float* lse, int head_dim) {
   DVT_REQUIRE(B > 0 && N > 0 && heads > 0, "attention: bad shape B=%d N=%d heads=%d", B, N, heads);
   DVT_REQUIRE(head_dim == 64 || head_dim == 80, "attention: head_dim %d is not supported (64 or 80)", head_dim);
+  const int impl = lse ? GEMM_TC : debug_impl();
   return head_dim == 64 ? launch_attention_d<64>(qkv, out, B, N, heads, stream, impl, lse)
                         : launch_attention_d<80>(qkv, out, B, N, heads, stream, impl, lse);
 }

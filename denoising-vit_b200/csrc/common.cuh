@@ -416,9 +416,14 @@ int num_sms();
 
 // host-side tally of kernels launched by this library (graph replays add the node count of the graph)
 void count_launch(long long n = 1);
-// Set by vit_forward around its block loop: LayerNorm / attention launches then use programmatic dependent launch (each
-// process drives one GPU from one thread, see INTEGRATION.md).
-extern bool g_vit_pdl;
 long long launch_count();
+
+// Kernel implementation of every GEMM and of the inference attention, one choice per process: the tensor-core kernels, or
+// the plain SIMT kernels (same semantics, slow) that tell a broken tensor-core kernel apart from a broken caller.
+// debug_impl() is DVT_GEMM_IMPL (a value starting with 's': SIMT) read on first use, unless set_debug_impl(0 or 1)
+// overrides it; set_debug_impl(-1) returns to DVT_GEMM_IMPL.  Read when a kernel is enqueued.
+enum GemmImpl { GEMM_TC = 0 /* tensor cores: wgmma, mma.sync for 3xTF32 */, GEMM_SIMT_DEBUG = 1 };
+int debug_impl();
+void set_debug_impl(int impl);
 
 }  // namespace dvt

@@ -303,7 +303,7 @@ int launch_layernorm_bwd_grouped(const float* x, const float* gamma, const float
 // token rows, then the prefix rows -- the first two steps of vit_forward (vit.cu) on caller-owned tensors.
 // ----------------------------------------------------------------------------------------------------
 int launch_vit_embed_fwd(const __nv_bfloat16* patches, int Kp, const __nv_bfloat16* w, const float* bias, const float* pos_patch,
-                         const float* prefix_rows, int B, int np, int prefix, int C, float* out, cudaStream_t st, int impl) {
+                         const float* prefix_rows, int B, int np, int prefix, int C, float* out, cudaStream_t st) {
   DVT_REQUIRE(patches && w && pos_patch && prefix_rows && out, "vit_embed_fwd: null argument");  // bias may be null
   DVT_REQUIRE(B > 0 && np > 0 && prefix >= 1 && C % 4 == 0 && Kp % 8 == 0, "vit_embed_fwd: bad shape");
   const int ntok = np + prefix;
@@ -311,7 +311,7 @@ int launch_vit_embed_fwd(const __nv_bfloat16* patches, int Kp, const __nv_bfloat
   e.bias = bias; e.out_mode = OUT_F32_REMAP; e.out = out; e.ldo = C; e.addend = pos_patch;
   e.rows_per_group = np; e.group_stride = ntok; e.row_offset = prefix;
   GemmShape s{B * np, C, Kp, 1};
-  int rc = launch_gemm_tn(patches, Kp, w, Kp, TMAP_BF16, s, e, st, impl);
+  int rc = launch_gemm_tn(patches, Kp, w, Kp, TMAP_BF16, s, e, st);
   if (rc) return rc;
   prefix_rows_kernel<<<B * prefix, 256, 0, st>>>(prefix_rows, out, B, prefix, ntok, C);
   DVT_CUDA_OK(cudaGetLastError());

@@ -1408,7 +1408,6 @@ struct Op {
 
 // What all GEMMs of one step (or one query) share.
 struct GemmOpt {
-  int impl;
   bool pdl;  // programmatic dependent launch
   int wide;  // 128 x 128 tiles when N >= this (GemmShape::x3_wide_min_n)
 };
@@ -1426,7 +1425,7 @@ static int fit_linear(Op X, int M, int K, Op W, int N, const float* bias, int ac
   e.bias = bias; e.act = act; e.out = out; e.ldo = ldo; e.out_plane = out_plane;
   e.out_mode = split_out ? OUT_F32_SPLIT : OUT_F32;
   const GemmShape s = fit_gemm_shape(M, N, K, 1, X, W, o);
-  return launch_gemm_tn(X.p, X.ld, W.p, W.ld, TMAP_F32, s, e, st, o.impl);
+  return launch_gemm_tn(X.p, X.ld, W.p, W.ld, TMAP_F32, s, e, st);
 }
 
 // dX = (dY . W) * (H > 0):  dY [M, Nout] K-major A; W stored [Nout, Kin] = MN-major B with N = Kin
@@ -1437,7 +1436,7 @@ static int fit_dgrad(Op dY, int M, int Nout, Op W, int Kin, const float* Hmask, 
   e.out_mode = split_out ? OUT_F32_SPLIT : OUT_F32;
   GemmShape s = fit_gemm_shape(M, Kin, Nout, 1, dY, W, o);
   s.b_mn = 1;
-  return launch_gemm_tn(dY.p, dY.ld, W.p, W.ld, TMAP_F32, s, e, st, o.impl);
+  return launch_gemm_tn(dY.p, dY.ld, W.p, W.ld, TMAP_F32, s, e, st);
 }
 
 // dW[Nout, Kin] (+ db[Nout]) += dY^T . [X | 1]:  dY stored [n, Nout] (MN-major A), X stored [n, Kin + ones] (MN-major B)
@@ -1455,7 +1454,7 @@ static int fit_wgrad(Op dY, int n, int Nout, Op X, int Kin, float* gW, float* gb
   const int splits = std::max(1, std::min(std::min(num_sms(), sm_cap) / std::max(tiles, 1), kb / 4));
   GemmShape s = fit_gemm_shape(Nout, Kin + 1, n, splits, dY, X, o);
   s.a_mn = 1; s.b_mn = 1;
-  return launch_gemm_tn(dY.p, dY.ld, X.p, X.ld, TMAP_F32, s, e, st, o.impl);
+  return launch_gemm_tn(dY.p, dY.ld, X.p, X.ld, TMAP_F32, s, e, st);
 }
 
 // Sweep launch geometry: n > 0 persistent CTAs of FIT_SWEEP_CTA_THREADS threads (one per SM), else 8 x #SM CTAs of 256
@@ -1530,7 +1529,7 @@ static int fit_enqueue_encode(Fit* f, int step_off, int npeek, int buf_off, cuda
 // before window w-1 (see fit_create).  With k = 1 this is the two-step-deep pipeline: one sweep per step, encodes with
 // two pending steps.  Precondition: f->enc holds the encoding of step t.
 // Sequential schedule (f->pipe[phase] == false): encode(t) at the head of the step, sweep(t) on the main stream at its tail.
-static int fit_enqueue_step(Fit* f, int step_off, bool phase2, bool epoch_end, cudaStream_t st, int impl) {
+static int fit_enqueue_step(Fit* f, int step_off, bool phase2, bool epoch_end, cudaStream_t st) {
   const int n = f->bsz, C = f->C, H1 = C / 2, Hr = C / 4, Lf = f->Lf;
   const StepRows sr{nullptr, f->step_base, step_off, f->inputs_dev};
   const int tb = 256;
@@ -1550,7 +1549,7 @@ static int fit_enqueue_step(Fit* f, int step_off, bool phase2, bool epoch_end, c
   // data-gradient GEMM hands its SMs to the queued CTAs of a weight-gradient GEMM -- every 3xTF32 CTA fills the shared
   // memory of its SM.
   const int wcap = f->wgrad_sms;
-  const GemmOpt gopt{impl, pdl, f->x3_wide_min_n[phase2 ? 1 : 0]};
+  const GemmOpt gopt{pdl, f->x3_wide_min_n[phase2 ? 1 : 0]};
   auto fork = [&](cudaStream_t to, cudaEvent_t e) -> int {
     DVT_CUDA_OK(cudaEventRecord(e, st));
     DVT_CUDA_OK(cudaStreamWaitEvent(to, e, 0));
@@ -1677,7 +1676,7 @@ static int fit_sync_sweep(Fit* f, cudaStream_t st, int* sweeps) {
   return DVT_OK;
 }
 
-static int fit_capture(Fit* f, bool phase2, int steps, cudaStream_t st, int impl, cudaGraphExec_t* out, long long* nodes,
+static int fit_capture(Fit* f, bool phase2, int steps, cudaStream_t st, cudaGraphExec_t* out, long long* nodes,
                        int* sweeps) {
   cudaGraph_t graph = nullptr;
   const long long before = launch_count();
@@ -1686,7 +1685,7 @@ static int fit_capture(Fit* f, bool phase2, int steps, cudaStream_t st, int impl
   // graphs start and end with the sweeps joined
   f->epoch_steps = f->epoch_windows = f->win_first = f->prev_first = 0;
   f->epoch_forked = false;
-  for (int i = 0; i < steps && rc == DVT_OK; ++i) rc = fit_enqueue_step(f, i, phase2, i + 1 == steps, st, impl);
+  for (int i = 0; i < steps && rc == DVT_OK; ++i) rc = fit_enqueue_step(f, i, phase2, i + 1 == steps, st);
   if (rc == DVT_OK) rc = fit_sync_sweep(f, st, sweeps);  // a capture must join every forked stream
   if (rc == DVT_OK) {
     fit_advance_kernel<<<1, 1, 0, st>>>(f->step_base, steps, *sweeps);
@@ -1733,7 +1732,7 @@ static int fit_capture(Fit* f, bool phase2, int steps, cudaStream_t st, int impl
 
 // Runs steps [cur, cur + count) of the schedule installed by fit_begin.  use_graphs: 0 = plain launches,
 // k > 0 = CUDA graphs of k steps each (remainders and the phase boundary fall back to plain launches).
-int fit_run(Fit* f, int count, int use_graphs, cudaStream_t caller, int impl) {
+int fit_run(Fit* f, int count, int use_graphs, cudaStream_t caller) {
   DVT_REQUIRE(f->bank && f->idx[0], "fit_run: call fit_begin first");
   int cur = f->cur_step;  // host mirror of the device step counter: no read-back, no host synchronisation
   // order the engine's stream after everything already enqueued on the caller's stream (the bank is produced there)
@@ -1760,14 +1759,14 @@ int fit_run(Fit* f, int count, int use_graphs, cudaStream_t caller, int impl) {
       cudaGraphExec_t* g = phase2 ? &f->graph2 : &f->graph1;
       long long* nodes = phase2 ? &f->graph2_nodes : &f->graph1_nodes;
       int* sweeps = phase2 ? &f->graph2_sweeps : &f->graph1_sweeps;
-      if (!*g) FIT_RC(fit_capture(f, phase2, use_graphs, st, impl, g, nodes, sweeps));
+      if (!*g) FIT_RC(fit_capture(f, phase2, use_graphs, st, g, nodes, sweeps));
       DVT_CUDA_OK(cudaGraphLaunch(*g, st));
       count_launch(*nodes);
       f->cur_buf ^= *sweeps & 1;
       f->enc_ready = f->pipe[phase2 ? 1 : 0];  // what the captured steps leave behind
       cur += use_graphs;
     } else {
-      FIT_RC(fit_enqueue_step(f, 0, phase2, true, st, impl));
+      FIT_RC(fit_enqueue_step(f, 0, phase2, true, st));
       // the sweep reads the device step counter: it must finish before the counter advances
       int sweeps = 0;
       FIT_RC(fit_sync_sweep(f, st, &sweeps));
@@ -1828,13 +1827,13 @@ static int fit_query_reserve(Fit* f, int n) {
 }
 
 // denoised_feats = field(coords): NeuralFeatureField.forward on n points (final query, main_img_denoising.py:121-130)
-int fit_query(Fit* f, const float* coords, int n, float* out, cudaStream_t st, int impl) {
+int fit_query(Fit* f, const float* coords, int n, float* out, cudaStream_t st) {
   DVT_REQUIRE(coords && out && n > 0, "fit_query: bad arguments");
   FIT_RC(fit_query_reserve(f, n));
   FIT_RC(fit_before_caller(f, st));
   const int C = f->C, H1 = C / 2;
   const size_t cap = (size_t)f->q_cap, wp = (size_t)f->n_small;
-  const GemmOpt gopt{impl, false, 0};  // no PDL, 128 x 64 tiles
+  const GemmOpt gopt{false, 0};  // no PDL, 128 x 64 tiles
   const StepRows sr{nullptr, f->step_base, 0};
   fit_encode_kernel<2><<<(n * f->grid.n_levels * 4 + 255) / 256, 256, 0, st>>>(
       f->grid, f->tb, f->tb.p[f->cur_buf], coords, sr, n, f->q_enc, f->ld_enc, cap * f->ld_enc, nullptr, 0.f, 0, 0);
@@ -1848,13 +1847,13 @@ int fit_query(Fit* f, const float* coords, int n, float* out, cudaStream_t st, i
 }
 
 // pred_residual = residual_predictor(raw) on n rows (offline_denoiser.py:40-46,105)
-int fit_residual(Fit* f, const float* raw, int n, float* out, cudaStream_t st, int impl) {
+int fit_residual(Fit* f, const float* raw, int n, float* out, cudaStream_t st) {
   DVT_REQUIRE(raw && out && n > 0, "fit_residual: bad arguments");
   FIT_RC(fit_query_reserve(f, n));
   FIT_RC(fit_before_caller(f, st));
   const int C = f->C, Hr = C / 4;
   const size_t cap = (size_t)f->q_cap, wp = (size_t)f->n_small;
-  const GemmOpt gopt{impl, false, 0};  // no PDL, 128 x 64 tiles
+  const GemmOpt gopt{false, 0};  // no PDL, 128 x 64 tiles
   const StepRows sr{nullptr, f->step_base, 0};
   fit_gather_rows_kernel<<<n, 192, 0, st>>>(raw, C, sr, n, f->q_raw, f->ld_raw, cap * f->ld_raw);
   DVT_CUDA_OK(cudaGetLastError());

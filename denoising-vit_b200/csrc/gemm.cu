@@ -18,7 +18,6 @@
 #include "gemm.cuh"
 
 #include <algorithm>
-#include <cstdlib>
 
 namespace dvt {
 
@@ -52,12 +51,13 @@ struct X3Smem {
   static_assert(BM * PITCH * 4 <= OFF_BAR, "staged accumulators must fit in the operand ring");
 };
 
-__device__ __forceinline__ void stamp_ts(const GemmEpi& e, int slot) {
-  if (e.debug_ts && blockIdx.x == 0) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    e.debug_ts[slot] = t;
-  }
+// A never-taken branch at the entry of the wgmma and 3xTF32 kernels (GemmEpi::entry_guard is always null).  It does nothing
+// at run time, but nvcc 12.9 allocates registers for these kernels better with it.  Without it the three 128-wide
+// gemm_x3_kernel instantiations go from 244 / 244 / 246 registers to 255 with 12-20 bytes of spill stores, the 64-wide ones
+// from 222 / 230 / 232 to 226 / 254 / 240, the gemm_wgmma_kernel ones from 90 to 92, and gemm_wgmma_swiglu_bwd_kernel
+// spills 4 bytes.  An empty asm statement or moving tile_of() does not have the same effect.
+__device__ __forceinline__ void gemm_entry_guard(const GemmEpi& e) {
+  if (threadIdx.x == 0 && e.entry_guard && blockIdx.x == 0) e.entry_guard[0] = 0;
 }
 
 template <bool FIT>
@@ -331,7 +331,7 @@ __device__ __forceinline__ void wgmma_gemm_body(const CUtensorMap& tmA, const CU
   uint64_t* empty = full + WG_STAGES;
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) stamp_ts(e, 0);
+  gemm_entry_guard(e);
   const TileIdx ti = tile_of(s, WG_BN, BK);
 
   if (warp == 8 && lane == 0) {
@@ -428,7 +428,6 @@ __device__ __forceinline__ void wgmma_gemm_body(const CUtensorMap& tmA, const CU
   } else {
     epi_tile<false, WG_BN, GLU>(e, s, tile, EPI_PITCH, warp, 8, lane, ti.tm, ti.tn, ti.kb0 < ti.kb_total);
   }
-  if (threadIdx.x == 0) stamp_ts(e, 6);
 }
 
 template <bool TF32, bool A_MN, bool B_MN>
@@ -486,7 +485,7 @@ gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
   const int wm = warp & 3, wn = warp >> 2;
-  if (threadIdx.x == 0) stamp_ts(e, 0);
+  gemm_entry_guard(e);
   const TileIdx ti = tile_of(s, BN, BK);
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
@@ -599,12 +598,11 @@ gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     __syncthreads();
     if (threadIdx.x == 0) st_release_u32(sem, split + 1 == (unsigned)s.splits ? 0u : split + 1);
   }
-  if (threadIdx.x == 0) stamp_ts(e, 6);
 }
 
 // ----------------------------------------------------------------------------------------------------
-// SIMT debug GEMM (fp32 FMA, 16x16 tiles).  Same epilogue semantics; selected with DVT_GEMM_IMPL=simt or the
-// `impl` argument.  It exists so that a broken tensor-core path can be told apart from a broken caller in
+// SIMT debug GEMM (fp32 FMA, 16x16 tiles).  Same epilogue semantics; selected with DVT_GEMM_IMPL=simt or
+// dvt_set_debug_impl(1).  It exists so that a broken tensor-core path can be told apart from a broken caller in
 // one GPU session; it is never the default.
 // ----------------------------------------------------------------------------------------------------
 template <typename T>
@@ -734,18 +732,9 @@ int gemm_prepare() {
 // shorter epilogue.  The caller chooses per call (GemmShape::x3_wide_min_n; 0 = always 128 x 64).
 int gemm_x3_tile_n(int N, int wide_min_n) { return (wide_min_n > 0 && N >= wide_min_n) ? 128 : 64; }
 
-int default_gemm_impl() {
-  static int impl = -1;
-  if (impl < 0) {
-    const char* v = getenv("DVT_GEMM_IMPL");
-    impl = (v && v[0] == 's') ? GEMM_SIMT_DEBUG : GEMM_TC;
-  }
-  return impl;
-}
-
 int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dtype, const GemmShape& shape,
-                   const GemmEpi& epi_in, cudaStream_t stream, int impl) {
-  if (impl < 0) impl = default_gemm_impl();
+                   const GemmEpi& epi_in, cudaStream_t stream) {
+  const int impl = debug_impl();
   GemmShape s = shape;
   GemmEpi epi = epi_in;
   if (s.splits < 1) s.splits = 1;

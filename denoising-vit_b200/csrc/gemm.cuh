@@ -36,7 +36,7 @@ struct GemmEpi {
   void* out = nullptr;
   int ldo = 0;
   size_t out_plane = 0;               // OUT_F32_SPLIT: element offset of the lo plane; OUT_F32_PLANES: between split planes
-  unsigned long long* debug_ts = nullptr;  // optional [8]: globaltimer (ns) milestones of CTA 0 (profiling aid)
+  unsigned long long* entry_guard = nullptr;  // always null: register allocation aid, see gemm_entry_guard (gemm.cu)
   int last_col_n = -1;                // = N-1 when last_col_out is set (filled in by launch_gemm)
   float* last_col_out = nullptr;      // OUT_F32_ATOMIC only: column N-1 is accumulated into last_col_out[m] instead
                                       // (bias gradient through a ones column in the B operand)
@@ -201,17 +201,15 @@ __device__ __forceinline__ void epi_post4(const GemmEpi& e, int m, int n, float4
   }
 }
 
-enum GemmImpl { GEMM_TC = 0 /* tensor cores: wgmma, mma.sync for 3xTF32 */, GEMM_SIMT_DEBUG = 1 };
-
 // dtype: TMAP_BF16 (bf16 operands) or TMAP_F32 (TF32 products of fp32 operands; K-major only unless x3).
 // lda / ldb: row pitch in elements of the stored matrix ([M,K] / [N,K], or [K,M] / [K,N] for MN-major operands).
+// Runs the kernels debug_impl() selects.
 int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dtype, const GemmShape& shape,
-                   const GemmEpi& epi, cudaStream_t stream, int impl = -1 /* -1: process default */);
+                   const GemmEpi& epi, cudaStream_t stream);
 
 // out [M, N] (row pitch ldo) = the `splits` fp32 planes of an OUT_F32_PLANES GEMM summed in split order
 int launch_splitk_planes_sum(const float* planes, int splits, size_t plane, int M, int N, int ldo, float* out,
                              cudaStream_t st);
-int default_gemm_impl();
 int gemm_prepare();
 int gemm_x3_tile_n(int N, int wide_min_n);  // 64 or 128: tile width launch_gemm_tn picks for a 3xTF32 product
 

@@ -1,20 +1,31 @@
-// Host runtime pieces shared by every entry point: error strings, device error word, SM count and TMA
+// Host runtime pieces shared by every entry point: error strings, debug implementation switch, SM count and TMA
 // descriptor encoding (cuTensorMapEncodeTiled resolved through the runtime so that the library does not link
 // against libcuda and can be dlopen'ed on a machine without a driver).
 #include "common.cuh"
 
 #include <cstdarg>
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <mutex>
 
 namespace dvt {
 
-bool g_vit_pdl = false;
-
 namespace {
 thread_local char g_err[1024] = "";
+int g_debug_impl_set = -1;  // dvt_set_debug_impl; -1: DVT_GEMM_IMPL decides
 }
+
+int debug_impl() {
+  if (g_debug_impl_set >= 0) return g_debug_impl_set;
+  static const int from_env = [] {
+    const char* v = getenv("DVT_GEMM_IMPL");
+    return (v && v[0] == 's') ? GEMM_SIMT_DEBUG : GEMM_TC;
+  }();
+  return from_env;
+}
+
+void set_debug_impl(int impl) { g_debug_impl_set = impl; }
 
 void set_last_error(const char* fmt, ...) {
   va_list ap;

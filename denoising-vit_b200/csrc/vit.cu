@@ -25,7 +25,7 @@ int launch_layernorm(const float* x, int ldx, const float* gamma, const float* b
 int launch_im2col(const void* x, bool x_bf16, __nv_bfloat16* out, int B, int H, int W, int P, int S, int h, int w,
                   int Kp, cudaStream_t stream);
 int launch_attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int B, int N, int heads, cudaStream_t stream,
-                     int impl, float* lse = nullptr, int head_dim = 64);
+                     float* lse, int head_dim);
 __global__ void strip_copy_kernel(const float*, int, float*, int, int, int, int, int);
 __global__ void prefix_rows_kernel(const float*, float*, int, int, int, int);
 __global__ void swiglu_kernel(const __nv_bfloat16*, __nv_bfloat16*, size_t, int);
@@ -194,7 +194,7 @@ int vit_reserve(Vit* v, size_t tokens, size_t patches) {
 
 int vit_forward(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int stride, const float* pos_patch,
                 const float* prefix_rows, int layer_index, int apply_norm, float* out, int out_all_tokens,
-                cudaStream_t stream, int impl) {
+                cudaStream_t stream) {
   const int C = v->embed, P = v->patch;
   DVT_REQUIRE(B > 0 && H >= P && W >= P && stride > 0, "vit_forward: bad input shape B=%d H=%d W=%d stride=%d", B, H, W, stride);
   DVT_REQUIRE(layer_index >= 0 && layer_index < v->depth, "vit_forward: layer_index %d out of range", layer_index);
@@ -205,7 +205,6 @@ int vit_forward(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int 
   DVT_REQUIRE(M < (size_t)1 << 30, "vit_forward: too many tokens");
   int rc = vit_reserve(v, M, (size_t)B * np);
   if (rc) return rc;
-  const int gi = impl;  // gemm / attention implementation selector (-1 default)
 
   rc = launch_im2col(x_in, x_bf16, v->patches, B, H, W, P, stride, h, w, v->Kp, stream);
   if (rc) return rc;
@@ -215,7 +214,7 @@ int vit_forward(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int 
     e.bias = v->patch_bias ? v->pe_b : nullptr; e.out_mode = OUT_F32_REMAP; e.out = x_tok; e.ldo = C; e.addend = pos_patch;
     e.rows_per_group = np; e.group_stride = ntok; e.row_offset = v->prefix;
     GemmShape s{B * np, C, v->Kp, 1};
-    rc = launch_gemm_tn(v->patches, v->Kp, v->pe_w, v->Kp, TMAP_BF16, s, e, stream, gi);
+    rc = launch_gemm_tn(v->patches, v->Kp, v->pe_w, v->Kp, TMAP_BF16, s, e, stream);
     if (rc) return rc;
   }
   prefix_rows_kernel<<<B * v->prefix, 256, 0, stream>>>(prefix_rows, x_tok, B, v->prefix, ntok, C);
@@ -227,19 +226,9 @@ int vit_forward(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int 
   }
 
   const int Mi = (int)M;
-  // Programmatic dependent launch along the block stack is available (DVT_VIT_PDL=1) but OFF by default: these kernels
-  // are long, so the hidden launch latency is worth little, and CTAs that are resident early but blocked in
-  // griddepcontrol.wait take SM slots from the fit running beside the forwards.  The fit's short kernels are where PDL
-  // pays (fit.cu).
-  static int vit_pdl = -1;
-  if (vit_pdl < 0) {
-    const char* pv = getenv("DVT_VIT_PDL");
-    vit_pdl = (pv && pv[0] == '1') ? 1 : 0;
-  }
-  struct PdlScope {
-    PdlScope(bool on) { g_vit_pdl = on; }
-    ~PdlScope() { g_vit_pdl = false; }
-  } pdl_scope(vit_pdl != 0);
+  // No programmatic dependent launch along the block stack: these kernels are long, so the hidden launch latency is worth
+  // little, and CTAs that are resident early but blocked in griddepcontrol.wait take SM slots from the fit running beside
+  // the forwards.  The fit's short kernels are where PDL pays (fit.cu).
   for (int i = 0; i <= layer_index; ++i) {
     const VitBlock& b = v->blocks[i];
     rc = launch_layernorm(v->x, C, b.n1w, b.n1b, v->xn, C, true, Mi, C, v->ln_eps, 1, 0, stream);
@@ -247,19 +236,16 @@ int vit_forward(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int 
     {
       GemmEpi e; e.bias = b.qkv_b; e.out_mode = OUT_BF16; e.out = v->qkv; e.ldo = 3 * C;
       GemmShape s{Mi, 3 * C, C, 1};
-      s.pdl = vit_pdl;
-      rc = launch_gemm_tn(v->xn, C, b.qkv_w, C, TMAP_BF16, s, e, stream, gi);
+      rc = launch_gemm_tn(v->xn, C, b.qkv_w, C, TMAP_BF16, s, e, stream);
       if (rc) return rc;
     }
-    rc = launch_attention(v->qkv, v->attn, B, ntok, v->heads, stream, gi < 0 ? default_gemm_impl() : gi, nullptr,
-                          v->head_dim);
+    rc = launch_attention(v->qkv, v->attn, B, ntok, v->heads, stream, nullptr, v->head_dim);
     if (rc) return rc;
     {
       GemmEpi e; e.bias = b.proj_b; e.out_mode = OUT_F32_RESID; e.out = v->x; e.ldo = C;
       e.gamma = v->layerscale ? b.ls1 : nullptr;
       GemmShape s{Mi, C, C, 1};
-      s.pdl = vit_pdl;
-      rc = launch_gemm_tn(v->attn, C, b.proj_w, C, TMAP_BF16, s, e, stream, gi);
+      rc = launch_gemm_tn(v->attn, C, b.proj_w, C, TMAP_BF16, s, e, stream);
       if (rc) return rc;
     }
     rc = launch_layernorm(v->x, C, b.n2w, b.n2b, v->xn, C, true, Mi, C, v->ln_eps, 1, 0, stream);
@@ -270,8 +256,7 @@ int vit_forward(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int 
       GemmEpi e; e.bias = b.fc1_b; e.act = v->swiglu ? ACT_NONE : ACT_GELU; e.out_mode = OUT_BF16; e.out = v->hid;
       e.ldo = v->mlp_hidden;
       GemmShape s{Mi, v->mlp_hidden, C, 1};
-      s.pdl = vit_pdl;
-      rc = launch_gemm_tn(v->xn, C, b.fc1_w, C, TMAP_BF16, s, e, stream, gi);
+      rc = launch_gemm_tn(v->xn, C, b.fc1_w, C, TMAP_BF16, s, e, stream);
       if (rc) return rc;
     }
     if (v->swiglu) {
@@ -285,8 +270,7 @@ int vit_forward(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int 
       GemmEpi e; e.bias = b.fc2_b; e.out_mode = OUT_F32_RESID; e.out = v->x; e.ldo = C;
       e.gamma = v->layerscale ? b.ls2 : nullptr;
       GemmShape s{Mi, C, fc2_k, 1};
-      s.pdl = vit_pdl;
-      rc = launch_gemm_tn(fc2_in, fc2_k, b.fc2_w, fc2_k, TMAP_BF16, s, e, stream, gi);
+      rc = launch_gemm_tn(fc2_in, fc2_k, b.fc2_w, fc2_k, TMAP_BF16, s, e, stream);
       if (rc) return rc;
     }
   }

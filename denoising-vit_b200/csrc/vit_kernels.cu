@@ -88,7 +88,7 @@ static void launch_ln_one(int want_blocks, int threads, cudaStream_t stream, con
     wave = occ * num_sms();
   }
   const int blocks = want_blocks < wave ? want_blocks : wave;
-  launch_k(g_vit_pdl, layernorm_kernel<OutT, NV>, dim3(blocks), dim3(threads), 0, stream, x, ldx, gamma, beta, y, ldy, rows, C,
+  launch_k(false, layernorm_kernel<OutT, NV>, dim3(blocks), dim3(threads), 0, stream, x, ldx, gamma, beta, y, ldy, rows, C,
            eps, in_group, skip);
 }
 

@@ -9,6 +9,9 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # DVT_LIB_PATH: load another build of the library (A/B measurements of two source revisions on one GPU box; symbols the
 # other build lacks are skipped)
 LIB_PATH = os.environ.get("DVT_LIB_PATH") or os.path.join(os.path.dirname(_HERE), "libdvt_b200.so")
+# dvt_version() of the library SIGNATURES describes.  A library with another version is refused: an entry point may keep
+# its name across versions but take other arguments, and calling it through these argtypes would pass garbage pointers.
+ABI_VERSION = 101
 
 
 class DvtError(RuntimeError):
@@ -24,13 +27,10 @@ SIGNATURES = {
     "dvt_device_error": (c_int, [POINTER(c_uint)]),
     "dvt_set_debug_impl": (c_int, [c_int]),
     "dvt_launch_count": (ctypes.c_longlong, []),
-    "dvt_debug_set_timestamp_buffer": (c_int, [c_void_p]),
     "dvt_gemm_tn": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p,
                             c_int, c_int, c_int, c_void_p]),
     "dvt_gemm_tn_residual": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
-                                     c_void_p, c_int, c_void_p]),
-    "dvt_gemm_tn_residual_ex": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
-                                        c_void_p, c_int, c_void_p, c_int, c_void_p]),
+                                     c_void_p, c_int, c_void_p, c_int, c_void_p]),
     "dvt_layerscale_bwd": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                    c_void_p]),
     "dvt_vit_embed_fwd": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
@@ -51,25 +51,18 @@ SIGNATURES = {
     "dvt_resample_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "dvt_layernorm": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_int,
                               c_int, c_void_p]),
-    "dvt_attention_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
-    "dvt_attention_fwd_hd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
-    "dvt_attention_fwd_lse_hd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
-    "dvt_attention_bwd_hd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
-                                     c_int, c_void_p]),
-    "dvt_attention_fwd_lse": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "dvt_attention_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "dvt_attention_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
-                                  c_void_p]),
+                                  c_int, c_void_p]),
     "dvt_layernorm_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
     "dvt_colsum": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "dvt_gelu": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p]),
-    "dvt_gemm_bf16_bwd": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int,
-                                  c_int, c_void_p, c_int, c_void_p]),
+    "dvt_gemm_bf16": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int,
+                              c_int, c_void_p, c_int, c_void_p, c_void_p]),
     "dvt_denoise_loss": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
     "dvt_adamw": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_double, c_double, c_double, c_double, c_double,
                           ctypes.c_longlong, c_void_p]),
     "dvt_im2col": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
-    "dvt_gemm_bf16_ex": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int,
-                                 c_int, c_int, c_void_p, c_void_p]),
     "dvt_gemm_f32x3": (c_int, [c_void_p, c_int, c_size_t, c_int, c_void_p, c_int, c_size_t, c_int, c_int, c_int, c_int,
                                c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "dvt_hashgrid_corners": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
@@ -101,9 +94,8 @@ SIGNATURES = {
     "dvt_seg_slide_accumulate": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
                                          c_int, c_void_p]),
     "dvt_seg_predict_hist": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p]),
-    "dvt_vit_create": (c_int, [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float]),
-    "dvt_vit_create_ex": (c_int, [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_int,
-                                  c_int]),
+    "dvt_vit_create": (c_int, [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_int,
+                               c_int]),
     "dvt_vit_destroy": (None, [c_void_p]),
     "dvt_vit_load": (c_int, [c_void_p, c_char_p, c_void_p, c_size_t]),
     "dvt_vit_reserve": (c_int, [c_void_p, c_int, c_int, c_int, c_int]),
@@ -120,6 +112,10 @@ def lib():
                 f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
                 "(there is no CPU fallback)")
         l = ctypes.CDLL(LIB_PATH)
+        l.dvt_version.restype = c_int
+        l.dvt_version.argtypes = []
+        if l.dvt_version() != ABI_VERSION:
+            raise DvtError(f"{LIB_PATH} has ABI version {l.dvt_version()}, this binding needs {ABI_VERSION}: rebuild it")
         for name, (res, args) in SIGNATURES.items():
             if not hasattr(l, name) and os.environ.get("DVT_LIB_PATH"):
                 continue

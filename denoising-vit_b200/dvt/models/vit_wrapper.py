@@ -215,9 +215,9 @@ class B200VisionTransformer(nn.Module):
             self._pos_cache = {}
         if self._handle is None:
             h = c_void_p()
-            check(lib().dvt_vit_create_ex(byref(h), a["embed"], a["depth"], a["heads"], self.patch_embed.patch_size[0],
-                                          a["mlp"], int(a["swiglu"]), int(a["ls"]), self.num_prefix_tokens, a["ln_eps"],
-                                          int(a["pre_norm"]), int(a["patch_bias"])), "dvt_vit_create_ex")
+            check(lib().dvt_vit_create(byref(h), a["embed"], a["depth"], a["heads"], self.patch_embed.patch_size[0],
+                                       a["mlp"], int(a["swiglu"]), int(a["ls"]), self.num_prefix_tokens, a["ln_eps"],
+                                       int(a["pre_norm"]), int(a["patch_bias"])), "dvt_vit_create")
             self._handle = h
         if not self._dirty:
             return

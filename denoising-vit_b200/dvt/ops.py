@@ -41,14 +41,17 @@ def gemm_tn(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None, 
 
 
 def gemm_tn_residual_(x: torch.Tensor, a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None,
-                      gamma: torch.Tensor | None) -> torch.Tensor:
-    """x += gamma * (a @ w.T + bias), x fp32 [M,N] in place."""
-    _need_cuda(x, a, w, bias, gamma)
+                      gamma: torch.Tensor | None, branch: torch.Tensor | None = None) -> torch.Tensor:
+    """x += gamma * (a @ w.T + bias), x fp32 [M,N] in place; when `branch` (bf16 [M, N]) is given, it receives
+    a @ w.T + bias (what the LayerScale backward needs)."""
+    _need_cuda(x, a, w, bias, gamma, branch)
     assert x.dtype == torch.float32 and x.stride(1) == 1
     M, K = a.shape
     N = w.shape[0]
+    if branch is not None:
+        assert branch.dtype == torch.bfloat16 and branch.shape == (M, N) and branch.is_contiguous()
     check(lib().dvt_gemm_tn_residual(ptr(a), a.stride(0), ptr(w), w.stride(0), _dt(a), M, N, K, ptr(bias), ptr(gamma),
-                                     ptr(x), x.stride(0), cur_stream()), "dvt_gemm_tn_residual")
+                                     ptr(x), x.stride(0), ptr(branch), N, cur_stream()), "dvt_gemm_tn_residual")
     return x
 
 
@@ -71,10 +74,7 @@ def attention(qkv: torch.Tensor, heads: int, head_dim: int = 64) -> torch.Tensor
     assert qkv.dtype == torch.bfloat16 and qkv.is_contiguous() and qkv.shape[2] == 3 * heads * head_dim
     B, N, _ = qkv.shape
     out = torch.empty((B, N, heads * head_dim), device=qkv.device, dtype=torch.bfloat16)
-    if head_dim == 64:
-        check(lib().dvt_attention_fwd(ptr(qkv), ptr(out), B, N, heads, cur_stream()), "dvt_attention_fwd")
-    else:
-        check(lib().dvt_attention_fwd_hd(ptr(qkv), ptr(out), B, N, heads, head_dim, cur_stream()), "dvt_attention_fwd_hd")
+    check(lib().dvt_attention_fwd(ptr(qkv), ptr(out), None, B, N, heads, head_dim, cur_stream()), "dvt_attention_fwd")
     return out
 
 
@@ -90,8 +90,8 @@ def im2col(x: torch.Tensor, patch: int, stride: int) -> torch.Tensor:
     return out
 
 
-def gemm_bf16_ex(a: torch.Tensor, b: torch.Tensor, M: int, N: int, K: int, a_mn: bool = False, b_mn: bool = False,
-                 out_dtype: torch.dtype = torch.float32, splits: int = 1, last_col: bool = False):
+def gemm_bf16(a: torch.Tensor, b: torch.Tensor, M: int, N: int, K: int, a_mn: bool = False, b_mn: bool = False,
+              out_dtype: torch.dtype = torch.float32, splits: int = 1, last_col: bool = False):
     """out[M,N] = A . B^T with A given as [M,K] (a_mn False) or [K,M] (a_mn True); B as [N,K] or [K,N]."""
     _need_cuda(a, b)
     assert a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16 and a.stride(1) == 1 and b.stride(1) == 1
@@ -100,8 +100,8 @@ def gemm_bf16_ex(a: torch.Tensor, b: torch.Tensor, M: int, N: int, K: int, a_mn:
     ldo = (n_out + 3) // 4 * 4
     out = (torch.zeros if atomic else torch.empty)((M, ldo), device=a.device, dtype=out_dtype)
     lc = torch.zeros(M, device=a.device, dtype=torch.float32) if last_col else None
-    check(lib().dvt_gemm_bf16_ex(ptr(a), a.stride(0), int(a_mn), ptr(b), b.stride(0), int(b_mn), M, N, K, ptr(out),
-                                 out.stride(0), _dt(out), splits, ptr(lc), cur_stream()), "dvt_gemm_bf16_ex")
+    check(lib().dvt_gemm_bf16(ptr(a), a.stride(0), int(a_mn), ptr(b), b.stride(0), int(b_mn), M, N, K, ptr(out),
+                              out.stride(0), _dt(out), splits, None, 0, ptr(lc), cur_stream()), "dvt_gemm_bf16")
     return (out[:, :n_out], lc) if last_col else out[:, :n_out]
 
 

@@ -35,11 +35,7 @@ def attention_fwd_lse(qkv: torch.Tensor, heads: int, head_dim: int = 64) -> Tupl
     B, N, _ = qkv.shape
     out = torch.empty((B, N, heads * head_dim), device=qkv.device, dtype=torch.bfloat16)
     lse = torch.empty((B, heads, N), device=qkv.device, dtype=torch.float32)
-    if head_dim == 64:
-        check(lib().dvt_attention_fwd_lse(ptr(qkv), ptr(out), ptr(lse), B, N, heads, cur_stream()), "dvt_attention_fwd_lse")
-    else:
-        check(lib().dvt_attention_fwd_lse_hd(ptr(qkv), ptr(out), ptr(lse), B, N, heads, head_dim, cur_stream()),
-              "dvt_attention_fwd_lse_hd")
+    check(lib().dvt_attention_fwd(ptr(qkv), ptr(out), ptr(lse), B, N, heads, head_dim, cur_stream()), "dvt_attention_fwd")
     return out, lse
 
 
@@ -56,12 +52,8 @@ def attention_bwd(qkv: torch.Tensor, out: torch.Tensor, dout: torch.Tensor, lse:
                                           cur_stream()), "dvt_attention_bwd_det")
         return dqkv
     dq_ws = torch.empty((B, N, heads * head_dim), device=qkv.device, dtype=torch.float32)
-    if head_dim == 64:
-        check(lib().dvt_attention_bwd(ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(dqkv), ptr(dq_ws), ptr(delta), B, N, heads,
-                                      cur_stream()), "dvt_attention_bwd")
-    else:
-        check(lib().dvt_attention_bwd_hd(ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(dqkv), ptr(dq_ws), ptr(delta), B, N,
-                                         heads, head_dim, cur_stream()), "dvt_attention_bwd_hd")
+    check(lib().dvt_attention_bwd(ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(dqkv), ptr(dq_ws), ptr(delta), B, N, heads,
+                                  head_dim, cur_stream()), "dvt_attention_bwd")
     return dqkv
 
 
@@ -135,8 +127,8 @@ def dgrad(dy: torch.Tensor, w: torch.Tensor, out_dtype: torch.dtype, gelu_preact
     n_in = w.shape[1]
     out = torch.empty((rows, n_in), device=dy.device, dtype=out_dtype)
     pre, ldp = (ptr(gelu_preact), gelu_preact.stride(0)) if gelu_preact is not None else (None, 0)
-    check(lib().dvt_gemm_bf16_bwd(ptr(dy), n_out, 0, ptr(w), n_in, 1, rows, n_in, n_out, ptr(out), n_in, _dt(out), 1, pre, ldp,
-                                  cur_stream()), "dvt_gemm_bf16_bwd(dgrad)")
+    check(lib().dvt_gemm_bf16(ptr(dy), n_out, 0, ptr(w), n_in, 1, rows, n_in, n_out, ptr(out), n_in, _dt(out), 1, pre, ldp,
+                              None, cur_stream()), "dvt_gemm_bf16(dgrad)")
     return out
 
 
@@ -162,8 +154,8 @@ def wgrad(dy: torch.Tensor, x: torch.Tensor) -> torch.Tensor:
                                                 cur_stream()), "dvt_gemm_bf16_wgrad_ordered")
         return out
     out = (torch.zeros if splits > 1 else torch.empty)((n_out, n_in), device=dy.device, dtype=torch.float32)
-    check(lib().dvt_gemm_bf16_bwd(ptr(dy), n_out, 1, ptr(x), n_in, 1, n_out, n_in, rows, ptr(out), n_in, DT_F32, splits, None, 0,
-                                  cur_stream()), "dvt_gemm_bf16_bwd(wgrad)")
+    check(lib().dvt_gemm_bf16(ptr(dy), n_out, 1, ptr(x), n_in, 1, n_out, n_in, rows, ptr(out), n_in, DT_F32, splits, None, 0,
+                              None, cur_stream()), "dvt_gemm_bf16(wgrad)")
     return out
 
 
@@ -345,19 +337,6 @@ def _workspace(C: int, device) -> torch.Tensor:
     return torch.empty(_WS_ROWS * C, device=device, dtype=torch.float32)
 
 
-def gemm_tn_residual_ex_(x: torch.Tensor, a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None,
-                         gamma: torch.Tensor | None, branch: torch.Tensor | None) -> torch.Tensor:
-    """x += gamma * (a @ w.T + bias) in place (fp32 x); when `branch` (bf16 [M, N]) is given, it receives a @ w.T + bias."""
-    assert x.is_cuda and x.dtype == torch.float32 and x.stride(1) == 1
-    M, K = a.shape
-    N = w.shape[0]
-    if branch is not None:
-        assert branch.dtype == torch.bfloat16 and branch.shape == (M, N) and branch.is_contiguous()
-    check(lib().dvt_gemm_tn_residual_ex(ptr(a), a.stride(0), ptr(w), w.stride(0), _dt(a), M, N, K, ptr(bias), ptr(gamma), ptr(x),
-                                        x.stride(0), ptr(branch), N, cur_stream()), "dvt_gemm_tn_residual_ex")
-    return x
-
-
 def layerscale_bwd(dx: torch.Tensor, branch: torch.Tensor | None, gamma: torch.Tensor | None, want_dbranch: bool = True):
     """Backward of x += gamma * branch: (dbranch bf16 = gamma * dx, dbias = sum_rows gamma * dx, dgamma = sum_rows dx *
     branch or None).  gamma None: no LayerScale (cast + column sum).  Fixed-order sums: bit-identical across calls."""
@@ -498,13 +477,13 @@ def _vit_block_fwd(x0, wts, heads: int, batch: int, keep: bool, eps: float = 1e-
     branch = lambda g: torch.empty((M, C), device=x0.device, dtype=torch.bfloat16) if (keep and g is not None) else None  # noqa
     x1 = x0.clone()
     br1 = branch(ls1)
-    gemm_tn_residual_ex_(x1, att, wp, projb, ls1, br1)
+    ops.gemm_tn_residual_(x1, att, wp, projb, ls1, br1)
     xn2 = ops.layernorm(x1, n2w, n2b, eps, out_dtype=torch.bfloat16)
     hpre = ops.gemm_tn(xn2, w1, fc1b, None, torch.bfloat16)
     hid = swiglu(hpre) if _is_swiglu(w1, w2) else gelu(hpre)
     x2 = x1.clone()
     br2 = branch(ls2)
-    gemm_tn_residual_ex_(x2, hid, w2, fc2b, ls2, br2)
+    ops.gemm_tn_residual_(x2, hid, w2, fc2b, ls2, br2)
     return x2, ((x1, xn1, qkv, att, lse, br1, xn2, hpre, hid, br2) if keep else None)
 
 

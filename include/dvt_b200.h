@@ -42,11 +42,10 @@ const char* dvt_last_error(void);
 int dvt_device_error(unsigned int* code_out);
 /* Number of kernels this library has launched in the calling process (CUDA-graph replays count their nodes). */
 long long dvt_launch_count(void);
-/* Profiling aid: when set (device pointer to 16 x u64, or NULL to disable), dvt_gemm_f32x3 launches record %globaltimer
- * milestones of CTA 0: slot 0 at entry, slot 6 at exit. */
-int dvt_debug_set_timestamp_buffer(unsigned long long* dev_buf16);
-/* Process-wide kernel implementation switch for debugging: 0 = tensor-core kernels (wgmma / mma.sync; default),
- * 1 = plain SIMT reference kernels (same semantics, slow; also settable with DVT_GEMM_IMPL=simt), -1 = back to the default. */
+/* Process-wide kernel implementation switch for debugging, for every GEMM and the attention forward without lse:
+ * 0 = tensor-core kernels (wgmma / mma.sync; default), 1 = plain SIMT reference kernels (same semantics, slow; also
+ * settable with DVT_GEMM_IMPL=simt), -1 = back to the DVT_GEMM_IMPL default.  Read when a call enqueues its kernels
+ * (for dvt_fit_run with graphs: when the graph is captured). */
 int dvt_set_debug_impl(int impl);
 
 /* ---------------------------------------------------------------------------------------------------------
@@ -62,11 +61,14 @@ int dvt_set_debug_impl(int impl);
 int dvt_gemm_tn(const void* A, int lda, const void* B, int ldb, int dtype, int M, int N, int K, const float* bias,
                 int act, void* out, int ldo, int out_dtype, int splits, void* stream);
 
-/* out[m,n] += gamma[n] * (A.B^T + bias)[m,n] on an fp32 residual stream (LayerScale + residual add).
+/* out[m,n] += gamma[n] * (A.B^T + bias)[m,n] on an fp32 residual stream (LayerScale + residual add; gamma NULL: unit
+ * scale).  branch_out_bf16 (optional, [M, ld_branch], ld_branch >= N and a multiple of 4): also writes the pre-LayerScale
+ * branch value A.B^T + bias as bf16 (what dvt_layerscale_bwd needs); x_inout is updated identically with or without it.
  * Replaces: `x = x + ls(attn(...))` / `x = x + ls(mlp(...))` in timm Block.forward
  * (restated in the reference at evaluation/vitdet/vision_transformer.py:98-117). */
 int dvt_gemm_tn_residual(const void* A, int lda, const void* B, int ldb, int dtype, int M, int N, int K,
-                         const float* bias, const float* gamma, float* x_inout, int ldx, void* stream);
+                         const float* bias, const float* gamma, float* x_inout, int ldx, void* branch_out_bf16,
+                         int ld_branch, void* stream);
 
 /* y = LayerNorm(x) over rows of C fp32 (eps inside the sqrt, affine gamma/beta), output bf16 or fp32.
  * in_group/skip: rows are grouped in runs of `in_group`; the first `skip` rows of every group are dropped and the
@@ -75,13 +77,14 @@ int dvt_gemm_tn_residual(const void* A, int lda, const void* B, int ldb, int dty
 int dvt_layernorm(const float* x, int ldx, const float* gamma, const float* beta, void* y, int ldy, int y_dtype,
                   int rows, int C, float eps, int in_group, int skip, void* stream);
 
-/* Multi-head attention, head_dim 64, no mask, scale 1/8: qkv bf16 [B, N, 3*heads*64] -> out bf16 [B, N, heads*64].
+/* Multi-head attention, no mask, head_dim 64 or 80 (80: ViT-H/14), scale head_dim^-0.5: qkv bf16 [B, N, 3*heads*head_dim]
+ * -> out bf16 [B, N, heads*head_dim].  lse (optional, for the backward): f32 [B, heads, N], the log2-domain log-sum-exp of
+ * the scaled scores; a call with lse always runs the tensor-core kernel (the SIMT debug kernel has no lse output), one
+ * without follows dvt_set_debug_impl.  out is the same with or without lse.
  * Replaces: timm Attention.forward -> F.scaled_dot_product_attention
  * (reference restatement: evaluation/vitdet/vision_transformer.py:73-91). */
-int dvt_attention_fwd(const void* qkv_bf16, void* out_bf16, int B, int N, int heads, void* stream);
-/* dvt_attention_fwd for head_dim 64 or 80 (embed = heads * head_dim, scale head_dim^-0.5; 80: ViT-H/14).  head_dim 64
- * is exactly dvt_attention_fwd. */
-int dvt_attention_fwd_hd(const void* qkv_bf16, void* out_bf16, int B, int N, int heads, int head_dim, void* stream);
+int dvt_attention_fwd(const void* qkv_bf16, void* out_bf16, float* lse, int B, int N, int heads, int head_dim,
+                      void* stream);
 
 /* Patch extraction for Conv2d(3->C, kernel P, stride S): x [B,3,H,W] (f32 or bf16) -> bf16 [B*h*w, Kp],
  * Kp = round_up(3*P*P, 8), column = c*P*P + i*P + j.  h = (H-P)/S+1, w = (W-P)/S+1
@@ -94,15 +97,12 @@ int dvt_im2col(const void* x, int x_dtype, void* out_bf16, int B, int H, int W, 
  * ------------------------------------------------------------------------------------------------------- */
 typedef struct dvt_vit dvt_vit_t;
 
-/* prefix_tokens = 1 (cls) + number of register tokens.  Only head_dim 64 (embed == 64*heads). */
+/* prefix_tokens = 1 (cls) + number of register tokens.  head_dim = embed / heads is 64 or 80.  pre_norm != 0: a
+ * LayerNorm `norm_pre` (weights loaded as "norm_pre.weight" / "norm_pre.bias") over all token rows between the token
+ * assembly and the first block (timm pre_norm=True: the CLIP towers).  patch_bias == 0: the patch embedding has no bias
+ * ("patch_embed.proj.bias" is not a key).  ln_eps applies to every LayerNorm. */
 int dvt_vit_create(dvt_vit_t** out, int embed, int depth, int heads, int patch, int mlp_hidden, int swiglu,
-                   int layerscale, int prefix_tokens, float ln_eps);
-/* General form: head_dim = embed / heads is 64 or 80.  pre_norm != 0: a LayerNorm `norm_pre` (weights loaded as
- * "norm_pre.weight" / "norm_pre.bias") over all token rows between the token assembly and the first block (timm
- * pre_norm=True: the CLIP towers).  patch_bias == 0: the patch embedding has no bias ("patch_embed.proj.bias" is not a
- * key).  ln_eps applies to every LayerNorm.  dvt_vit_create(...) is dvt_vit_create_ex(..., 0, 1). */
-int dvt_vit_create_ex(dvt_vit_t** out, int embed, int depth, int heads, int patch, int mlp_hidden, int swiglu,
-                      int layerscale, int prefix_tokens, float ln_eps, int pre_norm, int patch_bias);
+                   int layerscale, int prefix_tokens, float ln_eps, int pre_norm, int patch_bias);
 void dvt_vit_destroy(dvt_vit_t* h);
 /* Loads one fp32 tensor by its timm state-dict key (without the wrapper's "model." prefix), e.g.
  * "blocks.3.attn.qkv.weight".  `src` may be host or device memory.  cls_token / reg_token / pos_embed are not
@@ -118,16 +118,23 @@ int dvt_vit_forward(dvt_vit_t* h, const void* x, int x_dtype, int B, int H, int 
                     const float* pos_patch, const float* prefix_rows, int layer_index, int norm, float* out,
                     int all_tokens, void* stream);
 
-/* General form of dvt_gemm_tn for bf16 operands: a_mn / b_mn = 1 reads the operand from its transposed storage
- * ([K, M] / [K, N] row-major, "MN-major") without a copy -- how the fit's weight-gradient GEMMs read activations.
- * Supported: (a_mn, b_mn) in {(0,0), (0,1), (1,1)}.  last_col_out (optional, splits >= 1, fp32 out): column N-1 of
- * the product is accumulated into last_col_out[M] instead of out (bias gradient via a ones column in B). */
-int dvt_gemm_bf16_ex(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, int M, int N, int K,
-                     void* out, int ldo, int out_dtype, int splits, float* last_col_out, void* stream);
+/* General form of dvt_gemm_tn for bf16 operands, no bias or activation: a_mn / b_mn = 1 reads the operand from its
+ * transposed storage ([K, M] / [K, N] row-major, "MN-major") without a copy.  Supported: (a_mn, b_mn) in {(0,0), (0,1),
+ * (1,1)}.  Used for the backward GEMMs: data gradients (b_mn = 1: the weight is read in its [out, in] storage) and weight
+ * gradients (a_mn = b_mn = 1: activations read in their [rows, features] storage, split-K over the rows).
+ *   splits > 1: partial sums added with f32 atomics into a zero-initialised `out`.
+ *   gelu_preact_bf16 (optional, [M, ld_preact]): the GELU derivative fused into the epilogue, out = (A.B^T) *
+ *     gelu'(gelu_preact[m, n]) (replaces autograd through nn.GELU).
+ *   last_col_out (optional): column N-1 of the product is accumulated into last_col_out[M] instead of out (bias gradient
+ *     via a ones column in B).
+ * splits > 1 and last_col_out accumulate, so they need out_dtype f32 and no gelu_preact. */
+int dvt_gemm_bf16(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, int M, int N, int K, void* out,
+                  int ldo, int out_dtype, int splits, const void* gelu_preact_bf16, int ld_preact, float* last_col_out,
+                  void* stream);
 
 /* fp32-accurate GEMM on the tensor cores ("3xTF32"): every fp32 operand is given as two planes, hi = the TF32-exact
  * part (low 13 mantissa bits zero) at the pointer and lo = x - hi at pointer + plane (elements); the kernel
- * accumulates A_hi.B_hi + A_hi.B_lo + A_lo.B_hi in fp32.  a_mn / b_mn as in dvt_gemm_bf16_ex.  This is what the
+ * accumulates A_hi.B_hi + A_hi.B_lo + A_lo.B_hi in fp32.  a_mn / b_mn as in dvt_gemm_bf16.  This is what the
  * stage-1 fit uses for nn.Linear forward/backward (the reference runs them in fp32 on cuBLAS:
  * dvt/models/neural_feature_field.py:40-44, dvt/models/offline_denoiser.py:40-46 with --dtype float32). */
 int dvt_gemm_f32x3(const float* A, int lda, size_t plane_a, int a_mn, const float* B, int ldb, size_t plane_b, int b_mn,
@@ -217,31 +224,17 @@ int dvt_fit_sweep_once(dvt_fit_t* h, int ctas, void* stream);
  * torch.optim.AdamW.step()).  Unit operators; dvt.models.Denoiser composes them into an autograd function, the forward
  * GEMMs are dvt_gemm_tn / dvt_gemm_tn_residual above.
  * ------------------------------------------------------------------------------------------------------- */
-/* dvt_attention_fwd that also writes lse f32 [B, heads, N]: log2-domain log-sum-exp of the scaled scores. */
-int dvt_attention_fwd_lse(const void* qkv_bf16, void* out_bf16, float* lse, int B, int N, int heads, void* stream);
-/* dvt_attention_fwd_lse for head_dim 64 or 80 (same lse convention). */
-int dvt_attention_fwd_lse_hd(const void* qkv_bf16, void* out_bf16, float* lse, int B, int N, int heads, int head_dim,
-                             void* stream);
-/* Flash-attention backward (replaces autograd through F.scaled_dot_product_attention in timm Attention): dqkv bf16
- * [B, N, 3*heads*64] from qkv, the forward output `out`, its gradient `dout` (bf16 [B, N, heads*64]) and lse.
- * Workspaces: dq_workspace f32 [B, N, heads*64], delta_workspace f32 [B, heads, N]. */
+/* Flash-attention backward (replaces autograd through F.scaled_dot_product_attention in timm Attention), head_dim 64 or
+ * 80 (D below): dqkv bf16 [B, N, 3*heads*D] from qkv, the forward output `out`, its gradient `dout` (bf16 [B, N,
+ * heads*D]) and the lse of dvt_attention_fwd.  Workspaces: dq_workspace f32 [B, N, heads*D], delta_workspace f32
+ * [B, heads, N]. */
 int dvt_attention_bwd(const void* qkv_bf16, const void* out_bf16, const void* dout_bf16, const float* lse, void* dqkv_bf16,
-                      float* dq_workspace, float* delta_workspace, int B, int N, int heads, void* stream);
-/* dvt_attention_bwd for head_dim 64 or 80: every heads*64 above becomes heads*head_dim. */
-int dvt_attention_bwd_hd(const void* qkv_bf16, const void* out_bf16, const void* dout_bf16, const float* lse,
-                         void* dqkv_bf16, float* dq_workspace, float* delta_workspace, int B, int N, int heads, int head_dim,
-                         void* stream);
+                      float* dq_workspace, float* delta_workspace, int B, int N, int heads, int head_dim, void* stream);
 /* LayerNorm backward: dx_accum [rows, C] += d/dx, dgamma / dbeta [C] += their gradients (all f32; x is the LN input). */
 int dvt_layernorm_bwd(const float* x, const float* gamma, const float* dy, float* dx_accum, float* dgamma, float* dbeta,
                       int rows, int C, float eps, void* stream);
 /* out_accum[n] += sum_m in[m, n]  (bias gradients); in: bf16 or f32 [rows, cols] with row pitch ld. */
 int dvt_colsum(const void* in, int dtype, int ld, int rows, int cols, float* out_accum, void* stream);
-/* dvt_gemm_bf16_ex for the backward GEMMs: data gradients (b_mn = 1: the weight is read in its [out, in] storage),
- * weight gradients (a_mn = b_mn = 1: activations read in their [rows, features] storage, split-K over the rows with
- * f32 atomics into a zeroed buffer), and optionally the GELU derivative fused into the epilogue: out = (A.B^T) *
- * gelu'(gelu_preact[m, n]) (replaces autograd through nn.GELU). */
-int dvt_gemm_bf16_bwd(const void* A, int lda, int a_mn, const void* B, int ldb, int b_mn, int M, int N, int K, void* out,
-                      int ldo, int out_dtype, int splits, const void* gelu_preact_bf16, int ld_preact, void* stream);
 /* out = gelu(in), erf form, bf16, n % 8 == 0  (forward of the MLP activation when the pre-activation must be kept). */
 int dvt_gelu(const void* in_bf16, void* out_bf16, size_t n, void* stream);
 /* Loss of main_denoiser.py:214-217 and its gradient: losses3 = (l2 + cos, l2 = mse, cos = 1 - mean cosine similarity);
@@ -260,14 +253,9 @@ int dvt_adamw(float* p, const float* g, float* m, float* v, size_t n, double lr,
  * calls are fixed-order two-level reductions through `workspace` (f32, at least 256 * C elements), so repeated calls are
  * bit-identical.
  * ------------------------------------------------------------------------------------------------------- */
-/* dvt_gemm_tn_residual that also writes the pre-LayerScale branch value A.B^T + bias as bf16 into branch_out
- * ([M, ld_branch], optional: NULL behaves exactly like dvt_gemm_tn_residual).  x_inout is updated identically. */
-int dvt_gemm_tn_residual_ex(const void* A, int lda, const void* B, int ldb, int dtype, int M, int N, int K,
-                            const float* bias, const float* gamma, float* x_inout, int ldx, void* branch_out_bf16,
-                            int ld_branch, void* stream);
 /* Backward of x += gamma * branch (branch = A.B^T + bias): one pass over dx (f32 [rows, C], row pitch ldx) that writes
  * dbranch = gamma * dx (bf16 [rows, C], optional), dbias[C] = sum_rows gamma * dx and, when dgamma is given, dgamma[C] =
- * sum_rows dx * branch (branch: the bf16 [rows, C] side output of dvt_gemm_tn_residual_ex).  gamma NULL: unit scale (no
+ * sum_rows dx * branch (branch: the bf16 [rows, C] side output of dvt_gemm_tn_residual).  gamma NULL: unit scale (no
  * LayerScale): the call casts dx to bf16 and sums its columns.  dbias / dgamma are overwritten. */
 int dvt_layerscale_bwd(const float* dx, int ldx, const void* branch_bf16, const float* gamma, void* dbranch_bf16, float* dbias,
                        float* dgamma, float* workspace, int rows, int C, void* stream);
@@ -302,8 +290,8 @@ int dvt_gemm_bf16_dgrad_swiglu(const void* dy_bf16, int ld_dy, const void* w_bf1
  * every float-atomic reduction of the backward.  Same inputs and outputs as the calls they replace; repeated calls on
  * the same GPU model give bit-identical results.  No kernel waits on another CTA.
  * ------------------------------------------------------------------------------------------------------- */
-/* dvt_attention_bwd_hd without float atomics: dK / dV come from the same key-major kernel (bit-identical to
- * dvt_attention_bwd_hd's), dQ from a query-major kernel that keeps it in registers over all key tiles and writes it once
+/* dvt_attention_bwd without float atomics: dK / dV come from the same key-major kernel (bit-identical to
+ * dvt_attention_bwd's), dQ from a query-major kernel that keeps it in registers over all key tiles and writes it once
  * (bf16).  No dQ workspace; delta_workspace f32 [B, heads, N]. */
 int dvt_attention_bwd_det(const void* qkv_bf16, const void* out_bf16, const void* dout_bf16, const float* lse,
                           void* dqkv_bf16, float* delta_workspace, int B, int N, int heads, int head_dim, void* stream);

@@ -41,7 +41,7 @@ def test_ctypes_binding_covers_header():
     from dvt import _lib
     assert sorted(_lib.SIGNATURES) == _declared()
     L = _lib.lib()
-    assert L.dvt_version() >= 100
+    assert L.dvt_version() == _lib.ABI_VERSION
     assert L.dvt_last_error() is not None
 
 

@@ -83,15 +83,17 @@ def test_attention_hd80_forward(impl, N, heads, B):
 
 
 def test_attention_hd64_forms_are_the_existing_kernels():
-    """head_dim 64 through the head_dim-taking entry points is bit-identical to the original symbols."""
-    from dvt import _lib, ops
-    from dvt._lib import cur_stream, lib, ptr
+    """head_dim 64: the lse form returns the output of the inference form bit for bit, and always runs the tensor-core
+    kernel (same bits under the SIMT debug implementation).  head_dim 72 is rejected."""
+    from dvt import _lib, ops, train_ops
     qkv = _qkv(2, 333, 6, 64, 5)
     a = ops.attention(qkv, 6)
-    b = torch.empty_like(a)
-    _lib.check(lib().dvt_attention_fwd_hd(ptr(qkv), ptr(b), 2, 333, 6, 64, cur_stream()))
+    b, lse = train_ops.attention_fwd_lse(qkv, 6)
+    with _impl(1):
+        c, lse_simt = train_ops.attention_fwd_lse(qkv, 6)
     _dev_ok()
     assert torch.equal(a, b)
+    assert torch.equal(b, c) and torch.equal(lse, lse_simt)
     with pytest.raises(_lib.DvtError):
         ops.attention(_qkv(1, 10, 2, 72, 1), 2, head_dim=72)
 

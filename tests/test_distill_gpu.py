@@ -100,7 +100,7 @@ def test_grouped_layernorm_backward(prefix, C):
 @pytest.mark.parametrize("impl", ["tc", "simt"])
 @pytest.mark.parametrize("with_gamma", [True, False], ids=["layerscale", "plain"])
 def test_residual_gemm_keeps_the_branch(impl, with_gamma):
-    from dvt import _lib, ops, train_ops
+    from dvt import _lib, ops
     g = torch.Generator(device="cuda").manual_seed(7)
     M, N, K = 333, 384, 256
     a = torch.randn(M, K, device="cuda", generator=g).bfloat16()
@@ -112,8 +112,8 @@ def test_residual_gemm_keeps_the_branch(impl, with_gamma):
     try:
         x1 = ops.gemm_tn_residual_(x0.clone(), a, w, bias, gamma)
         branch = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
-        x2 = train_ops.gemm_tn_residual_ex_(x0.clone(), a, w, bias, gamma, branch)
-        x3 = train_ops.gemm_tn_residual_ex_(x0.clone(), a, w, bias, gamma, None)
+        x2 = ops.gemm_tn_residual_(x0.clone(), a, w, bias, gamma, branch)
+        x3 = ops.gemm_tn_residual_(x0.clone(), a, w, bias, gamma, None)
         _dev_ok()
     finally:
         _lib.check(_lib.lib().dvt_set_debug_impl(-1))

@@ -94,12 +94,12 @@ def test_gemm_mn_major(impl):
     w = (torch.randn(C, H1, device="cuda", generator=g) / 20).bfloat16()
     with _impl(impl):
         # dgrad: dX[n, H1] = dY[n, C] . W[C, H1]  (B = W read as MN-major)
-        dx = ops.gemm_bf16_ex(dy, w, n, H1, C, a_mn=False, b_mn=True)
+        dx = ops.gemm_bf16(dy, w, n, H1, C, a_mn=False, b_mn=True)
         # wgrad + bias grad: dW[C, H1] | db[C] = dY^T . [X | 1]
-        dw, db = ops.gemm_bf16_ex(dy, x, C, H1 + 1, n, a_mn=True, b_mn=True, splits=8, last_col=True)
+        dw, db = ops.gemm_bf16(dy, x, C, H1 + 1, n, a_mn=True, b_mn=True, splits=8, last_col=True)
         # ragged: K = 200 rows, N = 129
         dy2, x2 = dy[:200, :256].contiguous(), x[:200, :136].contiguous()
-        dw2, db2 = ops.gemm_bf16_ex(dy2, x2, 256, 129, 200, a_mn=True, b_mn=True, splits=1, last_col=True)
+        dw2, db2 = ops.gemm_bf16(dy2, x2, 256, 129, 200, a_mn=True, b_mn=True, splits=1, last_col=True)
     torch.cuda.synchronize()
     assert (dx - dy.float() @ w.float()).abs().max().item() < 2e-2
     ref = dy.float().t() @ x[:, :H1 + 1].float()

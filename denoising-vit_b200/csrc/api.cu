@@ -118,7 +118,9 @@ int dvt_gemm_tn(const void* A, int lda, const void* B, int ldb, int dtype, int M
   e.out = out;
   e.ldo = ldo;
   if (splits > 1) {
-    DVT_REQUIRE(out_dtype == DVT_DTYPE_F32 && act == 0, "dvt_gemm_tn: split-K needs fp32 output and no activation");
+    // every split runs the epilogue on its partial sum, so a bias would be added once per split
+    DVT_REQUIRE(out_dtype == DVT_DTYPE_F32 && act == 0 && bias == nullptr,
+                "dvt_gemm_tn: split-K needs fp32 output, no activation and no bias");
     e.out_mode = OUT_F32_ATOMIC;
   } else {
     e.out_mode = out_dtype == DVT_DTYPE_BF16 ? OUT_BF16 : OUT_F32;

@@ -351,6 +351,15 @@ __device__ __forceinline__ float fast_erf(float x) {
 // GELU(x) = x Phi(x) = max(x, 0) - 0.5 |x| erfc(|x| / sqrt 2): with erfc = 2^q as in fast_erf (same polynomial, written in
 // a = |x| with the -1 of the factor 0.5 folded into the exponent) this is 11 instructions per element instead of 18 -- the
 // fc1 epilogue is issue bound (ncu: issue 50 %, tensor 51 %).  Max abs error vs the exact erf GELU 5.2e-7.
+// max(x, 0) is max.NaN (relu_nan below), not fmaxf: fmaxf drops a NaN operand, which would turn GELU(NaN) into -a e
+// ~ -3.7e-17 (a is clamped, so the polynomial stays finite) and hide a diverged pre-activation.  With max.NaN the NaN
+// reaches the final FMA: GELU(NaN) = NaN, at the same instruction count.  GELU(+inf) = +inf; GELU(-inf) = -8.49 * 2^q(8.49)
+// ~ -3.7e-17, i.e. 0 to bf16 (torch's x Phi(x) gives NaN there: -inf * 0).
+__device__ __forceinline__ float relu_nan(float x) {
+  float r;
+  asm("max.NaN.f32 %0, %1, 0f00000000;" : "=f"(r) : "f"(x));
+  return r;
+}
 __device__ __forceinline__ float gelu_erf(float x) {
   const float a = fminf(fabsf(x), 8.485281374f);
   float q = 1.9755745359180961e-05f;
@@ -362,7 +371,7 @@ __device__ __forceinline__ float gelu_erf(float x) {
   q = fmaf(q, a, -1.0f);
   float e;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(q));
-  return fmaf(-a, e, fmaxf(x, 0.0f));
+  return fmaf(-a, e, relu_nan(x));
 }
 
 // Two GELUs in packed fp32 pairs: the polynomial is evaluated in n = -min(|x|, 8.485) (one FMNMX with source modifiers; the
@@ -380,7 +389,7 @@ __device__ __forceinline__ float2 gelu_erf2(float2 x) {
   float2 e;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e.x) : "f"(q.x));
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e.y) : "f"(q.y));
-  return ffma2(n, e, make_float2(fmaxf(x.x, 0.0f), fmaxf(x.y, 0.0f)));
+  return ffma2(n, e, make_float2(relu_nan(x.x), relu_nan(x.y)));
 }
 
 // d/dx gelu_erf(x) = Phi(x) + x phi(x)

@@ -758,6 +758,34 @@ int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dty
                        ((reinterpret_cast<uintptr_t>(epi.mask) | reinterpret_cast<uintptr_t>(epi.out)) & 7) == 0),
               "gemm: the SwiGLU-backward epilogue needs bf16 A K-major / B MN-major, no split-K, bf16 output and 8-byte "
               "aligned [M, >= 2N] pre-activation / output with pitches that are multiples of 4");
+  // The epilogue reads and writes four consecutive columns at once (float4 / uint2), so every pointer it touches must be
+  // aligned for those accesses.  All checks run before any CUDA call: a bad argument is reported, never a fault.
+  auto misaligned = [](const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) != 0; };
+  DVT_REQUIRE(!misaligned(epi.out, epi.out_mode == OUT_BF16 ? 8 : 16),
+              "gemm: out must be %d-byte aligned", epi.out_mode == OUT_BF16 ? 8 : 16);
+  DVT_REQUIRE(!misaligned(epi.bias, 16) && !misaligned(epi.gamma, 16) && !misaligned(epi.addend, 16),
+              "gemm: bias, gamma and addend must be 16-byte aligned");
+  DVT_REQUIRE(epi.mask == nullptr || (!misaligned(epi.mask, 8) && epi.ldmask % 4 == 0),
+              "gemm: the bf16 mask / GELU pre-activation must be 8-byte aligned with a pitch that is a multiple of 4 (got %d)",
+              epi.ldmask);
+  DVT_REQUIRE(epi.mask_f32 == nullptr || (!misaligned(epi.mask_f32, 16) && epi.ldmask % 4 == 0),
+              "gemm: the fp32 mask must be 16-byte aligned with a pitch that is a multiple of 4 (got %d)", epi.ldmask);
+  DVT_REQUIRE(!misaligned(epi.branch, 8), "gemm: branch must be 8-byte aligned");
+  DVT_REQUIRE(!misaligned(epi.last_col_out, 4), "gemm: last_col_out must be 4-byte aligned");
+  DVT_REQUIRE(epi.out_mode != OUT_F32_SPLIT || epi.out_plane % 4 == 0, "gemm: the lo plane offset must be a multiple of 4");
+  const int elem = dtype == TMAP_BF16 ? 2 : 4;
+  DVT_REQUIRE(!misaligned(A, 16) && !misaligned(B, 16), "gemm: operands must be 16-byte aligned");
+  if (s.x3) {
+    DVT_REQUIRE(dtype == TMAP_F32, "gemm: x3 needs fp32 operands");
+    DVT_REQUIRE(!(s.a_mn && !s.b_mn), "gemm: A MN-major with B K-major is not instantiated");
+    DVT_REQUIRE((lda * 4) % 16 == 0 && (ldb * 4) % 16 == 0 && (s.plane_a * 4) % 16 == 0 && (s.plane_b * 4) % 16 == 0,
+                "gemm: x3 pitches must be multiples of 16 bytes");
+  } else {
+    DVT_REQUIRE(dtype == TMAP_BF16 || (!s.a_mn && !s.b_mn), "gemm: MN-major operands are implemented for bf16 only");
+    DVT_REQUIRE(!(s.a_mn && !s.b_mn), "gemm: A MN-major with B K-major is not instantiated");
+    DVT_REQUIRE((lda * elem) % 16 == 0 && (ldb * elem) % 16 == 0,
+                "gemm: row pitch must be a multiple of 16 bytes (lda=%d ldb=%d elem=%d)", lda, ldb, elem);
+  }
 
   if (impl == GEMM_SIMT_DEBUG) {
     dim3 grid((s.N + 15) / 16, (s.M + 15) / 16), block(16, 16);
@@ -776,13 +804,8 @@ int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dty
     int prc = gemm_prepare();
     if (prc) return prc;
   }
-  const int elem = dtype == TMAP_BF16 ? 2 : 4;
   const int bk = KB_BYTES / elem;
   if (s.x3) {
-    DVT_REQUIRE(dtype == TMAP_F32, "gemm: x3 needs fp32 operands");
-    DVT_REQUIRE(!(s.a_mn && !s.b_mn), "gemm: A MN-major with B K-major is not instantiated");
-    DVT_REQUIRE((lda * 4) % 16 == 0 && (ldb * 4) % 16 == 0 && (s.plane_a * 4) % 16 == 0 && (s.plane_b * 4) % 16 == 0,
-                "gemm: x3 pitches must be multiples of 16 bytes");
     CUtensorMap tA, tB;
     int rc3;
     const int bn3 = gemm_x3_tile_n(s.N, s.x3_wide_min_n);
@@ -801,12 +824,6 @@ int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dty
     if (s.b_mn) return launch_x3<64, false, true>(tA, tB, s, epi, stream);
     return launch_x3<64, false, false>(tA, tB, s, epi, stream);
   }
-  DVT_REQUIRE(dtype == TMAP_BF16 || (!s.a_mn && !s.b_mn), "gemm: MN-major operands are implemented for bf16 only");
-  DVT_REQUIRE(!(s.a_mn && !s.b_mn), "gemm: A MN-major with B K-major is not instantiated");
-  DVT_REQUIRE((lda * elem) % 16 == 0 && (ldb * elem) % 16 == 0,
-              "gemm: row pitch must be a multiple of 16 bytes (lda=%d ldb=%d elem=%d)", lda, ldb, elem);
-  DVT_REQUIRE((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(B) & 15) == 0,
-              "gemm: operands must be 16-byte aligned");
   CUtensorMap tmA, tmB;
   int rc;
   if (s.a_mn) rc = make_tmap_2d(&tmA, A, dtype, (uint64_t)s.K, (uint64_t)s.M, (uint64_t)lda * elem, bk, 64);

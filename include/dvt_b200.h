@@ -55,7 +55,9 @@ int dvt_set_debug_impl(int impl);
 /* C[M,N] = act(A[M,K] . B[N,K]^T + bias) with A, B row-major, K contiguous (torch nn.Linear convention:
  * B is the Linear weight).  dtype: DVT_DTYPE_BF16 (bf16 operands) or DVT_DTYPE_F32 (fp32 operands, TF32
  * tensor-core math).  act: 0 none, 1 GELU(erf), 2 ReLU.  out_dtype: bf16 or f32.  splits > 1 accumulates
- * split-K partial sums atomically into a zero-initialised fp32 `out`.
+ * split-K partial sums atomically into a zero-initialised fp32 `out` (no bias, no activation).  The epilogue accesses
+ * four columns at once: `out` must be 16-byte aligned (f32) or 8-byte aligned (bf16), `bias` 16-byte aligned, ldo a
+ * multiple of 4; A and B 16-byte aligned with row pitches that are multiples of 16 bytes.  GELU(NaN) = NaN.
  * Replaces: torch.nn.Linear / cuBLAS calls made by timm Block (qkv, proj, fc1, fc2) and by
  * dvt/models/neural_feature_field.py:40-44, dvt/models/offline_denoiser.py:40-46. */
 int dvt_gemm_tn(const void* A, int lda, const void* B, int ldb, int dtype, int M, int N, int K, const float* bias,
@@ -64,6 +66,7 @@ int dvt_gemm_tn(const void* A, int lda, const void* B, int ldb, int dtype, int M
 /* out[m,n] += gamma[n] * (A.B^T + bias)[m,n] on an fp32 residual stream (LayerScale + residual add; gamma NULL: unit
  * scale).  branch_out_bf16 (optional, [M, ld_branch], ld_branch >= N and a multiple of 4): also writes the pre-LayerScale
  * branch value A.B^T + bias as bf16 (what dvt_layerscale_bwd needs); x_inout is updated identically with or without it.
+ * Alignment: x_inout, bias and gamma 16 bytes, branch_out_bf16 8 bytes (as for dvt_gemm_tn).
  * Replaces: `x = x + ls(attn(...))` / `x = x + ls(mlp(...))` in timm Block.forward
  * (restated in the reference at evaluation/vitdet/vision_transformer.py:98-117). */
 int dvt_gemm_tn_residual(const void* A, int lda, const void* B, int ldb, int dtype, int M, int N, int K,
@@ -123,8 +126,8 @@ int dvt_vit_forward(dvt_vit_t* h, const void* x, int x_dtype, int B, int H, int 
  * (1,1)}.  Used for the backward GEMMs: data gradients (b_mn = 1: the weight is read in its [out, in] storage) and weight
  * gradients (a_mn = b_mn = 1: activations read in their [rows, features] storage, split-K over the rows).
  *   splits > 1: partial sums added with f32 atomics into a zero-initialised `out`.
- *   gelu_preact_bf16 (optional, [M, ld_preact]): the GELU derivative fused into the epilogue, out = (A.B^T) *
- *     gelu'(gelu_preact[m, n]) (replaces autograd through nn.GELU).
+ *   gelu_preact_bf16 (optional, [M, ld_preact], 8-byte aligned, ld_preact a multiple of 4): the GELU derivative fused
+ *     into the epilogue, out = (A.B^T) * gelu'(gelu_preact[m, n]) (replaces autograd through nn.GELU).
  *   last_col_out (optional): column N-1 of the product is accumulated into last_col_out[M] instead of out (bias gradient
  *     via a ones column in B).
  * splits > 1 and last_col_out accumulate, so they need out_dtype f32 and no gelu_preact. */

@@ -76,6 +76,10 @@ int launch_seg_slide_accumulate(const float* logits, int h, int w, int K, int y1
                                 float* count, int Hc, int Wc, cudaStream_t st);
 int launch_seg_predict_hist(float* acc, const float* count, int K, int Hc, int Wc, const uint8_t* labels, int Ho, int Wo,
                             unsigned long long* hist, cudaStream_t st);
+int launch_seg_aug_accumulate(const float* acc, const float* count, int K, int Hc, int Wc, int flip, float* prob, int Ho,
+                              int Wo, cudaStream_t st);
+int launch_seg_aug_argmax_hist(const float* prob, int n_aug, int K, const uint8_t* labels, int Ho, int Wo,
+                               unsigned long long* hist, cudaStream_t st);
 const char* last_error();
 }  // namespace dvt
 
@@ -454,6 +458,14 @@ int dvt_seg_slide_accumulate(const float* logits, int h, int w, int K, int y1, i
 int dvt_seg_predict_hist(float* acc, const float* count, int K, int Hc, int Wc, const uint8_t* labels, int Ho, int Wo,
                          unsigned long long* hist, void* stream) {
   return launch_seg_predict_hist(acc, count, K, Hc, Wc, labels, Ho, Wo, hist, reinterpret_cast<cudaStream_t>(stream));
+}
+int dvt_seg_aug_accumulate(const float* acc, const float* count, int K, int Hc, int Wc, int flip, float* prob, int Ho, int Wo,
+                           void* stream) {
+  return launch_seg_aug_accumulate(acc, count, K, Hc, Wc, flip, prob, Ho, Wo, reinterpret_cast<cudaStream_t>(stream));
+}
+int dvt_seg_aug_argmax_hist(const float* prob, int n_aug, int K, const uint8_t* labels, int Ho, int Wo,
+                            unsigned long long* hist, void* stream) {
+  return launch_seg_aug_argmax_hist(prob, n_aug, K, labels, Ho, Wo, hist, reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -343,4 +343,139 @@ int launch_seg_predict_hist(float* acc, const float* count, int K, int Hc, int W
   return DVT_OK;
 }
 
+// ----------------------------------------------------------------------------------------------------
+// Test-time augmentation (mmseg EncoderDecoder.aug_test), one augmentation: for every pixel of the original Ho x Wo image
+// the bilinear resize of acc / count from the augmentation's Hc x Wc (each tap divided by its count: the values of
+// mmseg's preds / count_mat), the softmax over the classes, the horizontal un-flip of a flipped augmentation, and
+// prob[k, y, x] += p_k.  A CTA takes kAugTile consecutive pixels at a time: one warp per pixel, lanes over the classes
+// (k = lane + 32 v), probabilities staged in shared memory as [class][pixel], then added to prob by rows of kAugTile
+// pixels per class (coalesced, where a warp's lanes over the classes would touch 32 planes).  A pixel is owned by one
+// CTA, so augmentations enqueued in order on one stream add in that order.
+// ----------------------------------------------------------------------------------------------------
+constexpr int kAugTile = 32;
+
+template <int KV>
+__global__ void __launch_bounds__(kSegWarps * 32) seg_aug_accumulate_kernel(
+    const float* __restrict__ acc, const float* __restrict__ count, int K, int Hc, int Wc, int flip,
+    float* __restrict__ prob, int Ho, int Wo) {
+  __shared__ float tile[KV * 32][kAugTile + 1];  // +1: a warp stores one pixel's classes down a column
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const float sy = (float)Hc / (float)Ho, sx = (float)Wc / (float)Wo;
+  const size_t plane = (size_t)Hc * Wc, oplane = (size_t)Ho * Wo;
+  const int n = Ho * Wo;
+  for (int t0 = blockIdx.x * kAugTile; t0 < n; t0 += gridDim.x * kAugTile) {
+    for (int j = warp; j < kAugTile && t0 + j < n; j += kSegWarps) {
+      const int e = t0 + j, y = e / Wo, x = e % Wo;
+      // output column x of a flipped augmentation is column Wo - 1 - x of its resized map
+      const SegTap ty = seg_tap(y, Hc, sy), tx = seg_tap(flip ? Wo - 1 - x : x, Wc, sx);
+      const size_t o00 = (size_t)ty.i0 * Wc + tx.i0, o01 = (size_t)ty.i0 * Wc + tx.i1;
+      const size_t o10 = (size_t)ty.i1 * Wc + tx.i0, o11 = (size_t)ty.i1 * Wc + tx.i1;
+      const float n00 = __ldg(count + o00), n01 = __ldg(count + o01), n10 = __ldg(count + o10), n11 = __ldg(count + o11);
+      float val[KV];
+      float m = -INFINITY;
+#pragma unroll
+      for (int v = 0; v < KV; ++v) {
+        const int k = lane + 32 * v;
+        if (k < K) {
+          const float* pk = acc + (size_t)k * plane;
+          val[v] = seg_lerp(ty, tx, __ldg(pk + o00) / n00, __ldg(pk + o01) / n01, __ldg(pk + o10) / n10,
+                            __ldg(pk + o11) / n11);
+        } else {
+          val[v] = -INFINITY;
+        }
+        m = fmaxf(m, val[v]);
+      }
+      m = warp_max_f(m);
+      float s = 0.f;
+#pragma unroll
+      for (int v = 0; v < KV; ++v) {
+        val[v] = expf(val[v] - m);  // exp(-inf) = 0 for the padding lanes
+        s += val[v];
+      }
+      s = warp_sum_f(s);
+#pragma unroll
+      for (int v = 0; v < KV; ++v) tile[lane + 32 * v][j] = val[v] / s;
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < K * kAugTile; i += blockDim.x) {
+      const int k = i / kAugTile, j = i % kAugTile;
+      if (t0 + j < n) prob[(size_t)k * oplane + t0 + j] += tile[k][j];
+    }
+    __syncthreads();
+  }
+}
+
+int launch_seg_aug_accumulate(const float* acc, const float* count, int K, int Hc, int Wc, int flip, float* prob, int Ho,
+                              int Wo, cudaStream_t st) {
+  DVT_REQUIRE(acc && count && prob, "seg_aug_accumulate: null argument");
+  DVT_REQUIRE(K > 0 && K <= 255 && Hc > 0 && Wc > 0 && Ho > 0 && Wo > 0,
+              "seg_aug_accumulate: bad shape K=%d accumulator %dx%d image %dx%d", K, Hc, Wc, Ho, Wo);
+  const int kv = (K + 31) / 32;
+  const int blocks = (int)std::min<long long>(((long long)Ho * Wo + kAugTile - 1) / kAugTile, (long long)num_sms() * 8);
+#define DVT_SEG_AUG(KV) \
+  seg_aug_accumulate_kernel<KV><<<blocks, kSegWarps * 32, 0, st>>>(acc, count, K, Hc, Wc, flip ? 1 : 0, prob, Ho, Wo)
+  if (kv <= 1) DVT_SEG_AUG(1);
+  else if (kv <= 2) DVT_SEG_AUG(2);
+  else if (kv <= 3) DVT_SEG_AUG(3);
+  else if (kv <= 5) DVT_SEG_AUG(5);
+  else DVT_SEG_AUG(8);
+#undef DVT_SEG_AUG
+  DVT_CUDA_OK(cudaGetLastError());
+  count_launch();
+  return DVT_OK;
+}
+
+// ----------------------------------------------------------------------------------------------------
+// Test-time augmentation, end of an image: prob / n_aug (the division of mmseg's aug_test, made before the argmax),
+// argmax over the classes (ties -> lowest index) and the histograms against the labels, in seg_predict_hist_kernel's
+// scheme: [3][K] unsigned counters in shared memory, added to hist [4, K] = (intersect, union, pred, label) with integer
+// atomics.
+// ----------------------------------------------------------------------------------------------------
+__global__ void seg_aug_argmax_hist_kernel(const float* __restrict__ prob, int n_aug, int K, const uint8_t* __restrict__ labels,
+                                           int Ho, int Wo, unsigned long long* __restrict__ hist) {
+  extern __shared__ unsigned int s_hist[];  // [3][K]: intersect, pred, label
+  for (int e = threadIdx.x; e < 3 * K; e += blockDim.x) s_hist[e] = 0u;
+  __syncthreads();
+  const float n = (float)n_aug;
+  const size_t plane = (size_t)Ho * Wo;
+  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < Ho * Wo; e += gridDim.x * blockDim.x) {
+    const int lab = labels[e];
+    if (lab == 255) continue;
+    float best = -INFINITY;
+    int arg = 0;
+    for (int k = 0; k < K; ++k) {
+      const float v = __ldg(prob + (size_t)k * plane + e) / n;
+      if (v > best) {
+        best = v;
+        arg = k;
+      }
+    }
+    atomicAdd(&s_hist[K + arg], 1u);
+    if (lab < K) {
+      atomicAdd(&s_hist[2 * K + lab], 1u);
+      if (arg == lab) atomicAdd(&s_hist[lab], 1u);
+    }
+  }
+  __syncthreads();
+  for (int k = threadIdx.x; k < K; k += blockDim.x) {
+    const unsigned int it = s_hist[k], pr = s_hist[K + k], lb = s_hist[2 * K + k];
+    if (it) atomicAdd(hist + k, (unsigned long long)it);
+    if (pr + lb - it) atomicAdd(hist + K + k, (unsigned long long)(pr + lb - it));
+    if (pr) atomicAdd(hist + 2 * K + k, (unsigned long long)pr);
+    if (lb) atomicAdd(hist + 3 * K + k, (unsigned long long)lb);
+  }
+}
+
+int launch_seg_aug_argmax_hist(const float* prob, int n_aug, int K, const uint8_t* labels, int Ho, int Wo,
+                               unsigned long long* hist, cudaStream_t st) {
+  DVT_REQUIRE(prob && labels && hist, "seg_aug_argmax_hist: null argument");
+  DVT_REQUIRE(n_aug > 0 && K > 0 && K <= 255 && Ho > 0 && Wo > 0,
+              "seg_aug_argmax_hist: bad shape n_aug=%d K=%d image %dx%d", n_aug, K, Ho, Wo);
+  const int blocks = (int)std::min<long long>(((long long)Ho * Wo + 255) / 256, (long long)num_sms() * 4);
+  seg_aug_argmax_hist_kernel<<<blocks, 256, 3 * K * sizeof(unsigned int), st>>>(prob, n_aug, K, labels, Ho, Wo, hist);
+  DVT_CUDA_OK(cudaGetLastError());
+  count_launch();
+  return DVT_OK;
+}
+
 }  // namespace dvt

@@ -94,6 +94,8 @@ SIGNATURES = {
     "dvt_seg_slide_accumulate": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
                                          c_int, c_void_p]),
     "dvt_seg_predict_hist": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "dvt_seg_aug_accumulate": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "dvt_seg_aug_argmax_hist": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "dvt_vit_create": (c_int, [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_int,
                                c_int]),
     "dvt_vit_destroy": (None, [c_void_p]),

@@ -122,8 +122,8 @@ class Resize:
         self.ratio_range = tuple(ratio_range) if ratio_range is not None else None
 
     def __call__(self, r, rng):
-        scale = r.get("scale", self.img_scale)
-        if self.ratio_range is not None:
+        scale = r.get("scale", self.img_scale)     # `scale`: preset by a test-time augmentation, which draws nothing
+        if "scale" not in r and self.ratio_range is not None:
             lo, hi = self.ratio_range
             ratio = rng.random_sample() * (hi - lo) + lo
             scale = int(self.img_scale[0] * ratio), int(self.img_scale[1] * ratio)
@@ -169,7 +169,7 @@ class RandomFlip:
         self.prob = prob
 
     def __call__(self, r, rng):
-        if self.prob is not None and rng.rand() < self.prob:
+        if r["flip"] if "flip" in r else (self.prob is not None and rng.rand() < self.prob):
             r["img"] = r["img"][:, ::-1]
             if "seg" in r:
                 r["seg"] = r["seg"][:, ::-1]
@@ -242,9 +242,38 @@ _STEPS = {"Resize": Resize, "RandomCrop": RandomCrop, "RandomFlip": RandomFlip,
 _NO_OP = ("LoadImageFromFile", "DefaultFormatBundle", "Collect", "ImageToTensor")
 
 
-def build_pipeline(steps: List[dict]) -> Tuple[list, bool]:
-    """(transforms, reduce_zero_label of LoadAnnotations).  MultiScaleFlipAug is flattened: single scale, no flip."""
-    out, rzl = [], False
+Aug = Tuple[Optional[Tuple[int, int]], bool]
+
+
+def multiscale_flip_augs(kw: dict) -> List[Aug]:
+    """mmseg MultiScaleFlipAug's augmentations, in its order (scale-major, then flip False, True): (scale (w, h), flip).
+    With `img_ratios` the scales are (int(w * r), int(h * r)) of `img_scale` (w, h) for each ratio; without, `img_scale`
+    itself.  One scale without flip (the linear configs) gives the single augmentation (img_scale, False)."""
+    ratios, flip, scale = kw.get("img_ratios"), bool(kw.get("flip", False)), kw.get("img_scale")
+    if not flip and (ratios is None or ratios in (1.0, [1.0], (1.0,))):
+        return [(tuple(scale) if scale is not None else None, False)]
+    if flip and kw.get("flip_direction", "horizontal") not in ("horizontal", ["horizontal"]):
+        raise ConfigError(f"MultiScaleFlipAug flip_direction {kw.get('flip_direction')!r}: only horizontal flips are "
+                          f"implemented")
+    if ratios is not None:
+        ratios = ratios if isinstance(ratios, list) else [ratios]
+        if not all(isinstance(r, float) for r in ratios):
+            raise ConfigError(f"MultiScaleFlipAug img_ratios {kw.get('img_ratios')!r}: a float or a list of floats")
+        if scale is None:
+            raise ConfigError("MultiScaleFlipAug img_ratios without img_scale (ratios of the image's own size) is not "
+                              "implemented: give img_scale=(w, h)")
+    if scale is None or len(scale) != 2 or not all(isinstance(v, (int, float)) for v in scale):
+        raise ConfigError(f"MultiScaleFlipAug img_scale {scale!r}: only one (w, h) scale is implemented")
+    scales = [(int(scale[0] * r), int(scale[1] * r)) for r in ratios] if ratios is not None else [tuple(scale)]
+    return [(s, f) for s in scales for f in ((False, True) if flip else (False,))]
+
+
+def build_pipeline(steps: List[dict]) -> Tuple[list, bool, List[Aug]]:
+    """(transforms, reduce_zero_label of LoadAnnotations, test-time augmentations).  MultiScaleFlipAug is flattened.
+    With one augmentation its scale becomes the img_scale of an inner Resize without one.  With several, each
+    augmentation runs the transforms with `scale` and `flip` preset; a pipeline without MultiScaleFlipAug has the single
+    augmentation (None, False)."""
+    out, rzl, augs, outside = [], False, [(None, False)], 0
     for step in steps:
         kw = dict(step)
         t = kw.pop("type")
@@ -253,19 +282,21 @@ def build_pipeline(steps: List[dict]) -> Tuple[list, bool]:
         if t == "LoadAnnotations":
             rzl = bool(kw.get("reduce_zero_label", False))
         elif t == "MultiScaleFlipAug":
-            ratios = kw.get("img_ratios")
-            if kw.get("flip", False) or (ratios is not None and ratios not in (1.0, [1.0], (1.0,))):
-                raise ConfigError("MultiScaleFlipAug: only one scale without flip is implemented")
-            inner, _ = build_pipeline(kw.get("transforms", []))
-            for tr in inner:
-                if isinstance(tr, Resize) and tr.img_scale is None:
-                    tr.img_scale = tuple(kw["img_scale"])
+            augs = multiscale_flip_augs(kw)
+            inner, _, _ = build_pipeline(kw.get("transforms", []))
+            if len(augs) == 1:
+                for tr in inner:
+                    if isinstance(tr, Resize) and tr.img_scale is None:
+                        tr.img_scale = augs[0][0]
             out.extend(inner)
         elif t in _STEPS:
             out.append(_STEPS[t](**kw))
+            outside += 1
         else:
             raise ConfigError(f"pipeline step {t!r} is not implemented")
-    return out, rzl
+    if len(augs) > 1 and outside:
+        raise ConfigError("MultiScaleFlipAug with several augmentations: pipeline steps outside it are not implemented")
+    return out, rzl, augs
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -297,7 +328,8 @@ class SegDataset(torch.utils.data.Dataset):
     Training (`train=True`): item t of the sample stream is image perm_e[t % n] of epoch e = t // n (a permutation drawn
     from `seed` + e), transformed with a RandomState seeded by (seed, t): returns (img f32 [3, H, W], seg u8 [H, W]).
     Evaluation: item i is image i after the test pipeline, with its ground truth at the original size (dataset-level
-    reduce_zero_label applied): returns (img f32 [3, H, W], gt u8 [Ho, Wo])."""
+    reduce_zero_label applied): returns (img f32 [3, H, W], gt u8 [Ho, Wo]).  With several test-time augmentations
+    (`augs`, mmseg's MultiScaleFlipAug order) it returns ([(img f32 [3, H_a, W_a], flip_a) per augmentation], gt)."""
 
     def __init__(self, ds_cfg: dict, num_classes: int, train: bool, seed: int = 0):
         d = dict(DATASET_DEFAULTS[ds_cfg["type"]])
@@ -316,7 +348,7 @@ class SegDataset(torch.utils.data.Dataset):
             raise FileNotFoundError(f"no images found under {img_dir}")
         self.images = [os.path.join(img_dir, r) for r in rel]
         self.labels = [os.path.join(ann_dir, r[:-len(d["img_suffix"])] + d["seg_map_suffix"]) for r in rel]
-        self.transforms, self.pipeline_rzl = build_pipeline(ds_cfg["pipeline"])
+        self.transforms, self.pipeline_rzl, self.augs = build_pipeline(ds_cfg["pipeline"])
         self.reduce_zero_label = d["reduce_zero_label"]
         self.num_classes, self.train, self.seed = num_classes, train, seed
         self._perm = (None, None)
@@ -352,11 +384,17 @@ class SegDataset(torch.utils.data.Dataset):
             return img_t, torch.from_numpy(np.ascontiguousarray(r["seg"]))
         gt = reduce_zero_label(seg) if self.reduce_zero_label else seg
         self._check(gt, self.labels[i])
-        r = {"img": img}
+        gt = torch.from_numpy(np.ascontiguousarray(gt))
+        if len(self.augs) > 1:
+            return [(self._test_image(img, {"scale": scale, "flip": flip}), flip) for scale, flip in self.augs], gt
+        return self._test_image(img, {}), gt
+
+    def _test_image(self, img, preset):
+        r = dict(preset, img=img)
         rng = np.random.RandomState(0)
         for tr in self.transforms:
             r = tr(r, rng)
-        return torch.from_numpy(np.ascontiguousarray(r["img"].transpose(2, 0, 1))), torch.from_numpy(np.ascontiguousarray(gt))
+        return torch.from_numpy(np.ascontiguousarray(r["img"].transpose(2, 0, 1)))
 
 
 class StreamSampler(torch.utils.data.Sampler):

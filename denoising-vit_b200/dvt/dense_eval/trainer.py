@@ -51,7 +51,7 @@ def evaluate(backbone: ProbeBackbone, head: LinearSegHead, dataset: SegDataset, 
              device, workers: int = 0) -> dict:
     """Slide inference over this rank's share of the validation set (images rank, rank + world, ...), decoded and resized
     by `workers` DataLoader workers (results in index order), histograms summed over ranks (exact int64 all-reduce),
-    metrics from the totals."""
+    metrics from the totals.  A test pipeline with several augmentations (multi-scale / flip) runs mmseg's aug_test."""
     rank, world = _rank_world()
     was_training = head.training
     head.eval()
@@ -62,8 +62,13 @@ def evaluate(backbone: ProbeBackbone, head: LinearSegHead, dataset: SegDataset, 
         share, batch_size=None, num_workers=workers, pin_memory=True,
         worker_init_fn=partial(worker_init_fn, num_workers=workers, rank=rank, seed=0) if workers > 0 else None)
     for img, gt in loader:
-        seg_ops.slide_inference_hist(fn, img.to(device, non_blocking=True), gt.to(device, non_blocking=True), num_classes,
-                                     test_cfg["crop_size"], test_cfg["stride"], hist)
+        gt = gt.to(device, non_blocking=True)
+        if len(dataset.augs) > 1:       # mmseg aug_test: img is [(image, flip)] per augmentation
+            augs = [(a.to(device, non_blocking=True), bool(flip)) for a, flip in img]
+            seg_ops.aug_slide_inference_hist(fn, augs, gt, num_classes, test_cfg["crop_size"], test_cfg["stride"], hist)
+        else:
+            seg_ops.slide_inference_hist(fn, img.to(device, non_blocking=True), gt, num_classes, test_cfg["crop_size"],
+                                         test_cfg["stride"], hist)
     if world > 1:
         dist.all_reduce(hist)
     head.train(was_training)

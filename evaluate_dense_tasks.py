@@ -5,7 +5,9 @@ vitb_ade20k_linear_config.py, read as plain Python: no mmcv), same backbones (:1
 optionally with `--load-distilled-model-from`, optionally under the `--load-denoiser-from` Denoiser), same probe (frozen
 backbone behind CenterPadding, BNHead on the `in_index` features, cross-entropy of the bilinearly upsampled logits,
 AdamW + poly schedule with linear warmup, slide inference, mIoU / mAcc / aAcc).  Only the layers `in_index` selects are
-computed.  The full-resolution loss and slide inference run on sm_90a kernels (dvt/dense_eval).
+computed.  The full-resolution loss and slide inference run on sm_90a kernels (dvt/dense_eval), and so does mmseg's
+multi-scale + flip test (e.g. `--cfg-options data.val.pipeline.1.img_ratios=[0.5,0.75,1.0,1.25,1.5,1.75]
+data.val.pipeline.1.flip=True`).
 
 Outputs in the work dir: `iter_<n>.pth` every checkpoint_config.interval iterations and at the end ({"state_dict":
 decode_head.* weights, "optimizer", "iter"}), `latest.pth` pointing at the newest, and `<timestamp>.log.json` (one JSON

@@ -350,6 +350,18 @@ int dvt_seg_slide_accumulate(const float* logits, int h, int w, int K, int y1, i
  * The resized logits are never written. */
 int dvt_seg_predict_hist(float* acc, const float* count, int K, int Hc, int Wc, const uint8_t* labels, int Ho, int Wo,
                          unsigned long long* hist, void* stream);
+/* Test-time augmentation (mmseg EncoderDecoder.aug_test), one augmentation: acc f32 [K, Hc, Wc] and count f32 [Hc, Wc]
+ * are the augmentation's slide-inference sums (dvt_seg_slide_accumulate; neither is written).  For every pixel of the
+ * original Ho x Wo image: the bilinear resize of acc / count from Hc x Wc, softmax over K, un-flipped horizontally when
+ * flip != 0, added into prob f32 [K, Ho, Wo].  Each pixel is owned by one CTA: augmentations enqueued in order on one
+ * stream add in that order.  K <= 255. */
+int dvt_seg_aug_accumulate(const float* acc, const float* count, int K, int Hc, int Wc, int flip, float* prob, int Ho, int Wo,
+                           void* stream);
+/* Test-time augmentation, end of an image: prob f32 [K, Ho, Wo] (the sum over n_aug augmentations) / n_aug, argmax over
+ * K (ties: lowest class) and mmseg's intersect_and_union against labels u8 [Ho, Wo], as dvt_seg_predict_hist:
+ * hist u64 [4, K] += (intersect, union, pred, label).  prob is not written. */
+int dvt_seg_aug_argmax_hist(const float* prob, int n_aug, int K, const uint8_t* labels, int Ho, int Wo,
+                            unsigned long long* hist, void* stream);
 
 #ifdef __cplusplus
 }

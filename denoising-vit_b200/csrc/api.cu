@@ -157,7 +157,7 @@ int dvt_gemm_tn_residual(const void* A, int lda, const void* B, int ldb, int dty
 int dvt_layernorm(const float* x, int ldx, const float* gamma, const float* beta, void* y, int ldy, int y_dtype,
                   int rows, int C, float eps, int in_group, int skip, void* stream) {
   DVT_REQUIRE(x && gamma && beta && y, "dvt_layernorm: null pointer");
-  DVT_REQUIRE(in_group >= 1 && skip >= 0 && skip < in_group + (in_group == 1), "dvt_layernorm: bad in_group/skip");
+  DVT_REQUIRE(y_dtype == DVT_DTYPE_BF16 || y_dtype == DVT_DTYPE_F32, "dvt_layernorm: bad y_dtype %d", y_dtype);
   return launch_layernorm(x, ldx, gamma, beta, y, ldy, y_dtype == DVT_DTYPE_BF16, rows, C, eps, in_group, skip,
                           reinterpret_cast<cudaStream_t>(stream));
 }

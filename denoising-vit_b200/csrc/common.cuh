@@ -39,6 +39,10 @@ int cuda_fail(cudaError_t e, const char* what, const char* file, int line);
 
 enum { DVT_OK = 0, DVT_ERR_INVALID = 1, DVT_ERR_CUDA = 2, DVT_ERR_DEVICE = 3 };
 
+// Launchers check every pointer a kernel reads or writes with vector accesses (float4 / uint2 / bf16x2) against this before
+// any CUDA call: a misaligned vector access faults and leaves the CUDA context unusable.  A null pointer is aligned.
+inline bool misaligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) != 0; }
+
 // device-side error word: 0 = fine; otherwise (code << 16 | detail)
 // (defined here: the library is built as ONE translation unit, see dvt_b200_all.cu)
 __device__ unsigned int g_dvt_dev_error = 0;

@@ -103,6 +103,11 @@ int launch_layerscale_bwd(const float* dx, int ldx, const __nv_bfloat16* branch,
                           float* dbias, float* dgamma, float* workspace, int rows, int C, cudaStream_t st) {
   DVT_REQUIRE(dx && dbias && workspace && rows > 0 && C > 0, "layerscale_bwd: bad arguments");
   DVT_REQUIRE(C % 4 == 0 && ldx % 4 == 0, "layerscale_bwd: C=%d and ldx=%d must be multiples of 4", C, ldx);
+  DVT_REQUIRE(ldx >= C, "layerscale_bwd: row pitch ldx=%d must be >= C=%d", ldx, C);
+  DVT_REQUIRE(!misaligned(dx, 16) && !misaligned(gamma, 16) && !misaligned(workspace, 16),
+              "layerscale_bwd: dx, gamma and workspace must be 16-byte aligned (float4 accesses)");
+  DVT_REQUIRE(!misaligned(branch, 8) && !misaligned(dbranch, 8),
+              "layerscale_bwd: branch and dbranch must be 8-byte aligned (4 x bf16 accesses)");
   DVT_REQUIRE(!dgamma || (branch && gamma), "layerscale_bwd: dgamma needs the saved branch and gamma");
   const int chunks = det_chunks(rows);
   branch_bwd_partial_kernel<float><<<dim3((C + 127) / 128, chunks), 256, 0, st>>>(dx, ldx, dgamma ? branch : nullptr, gamma, dbranch,
@@ -117,6 +122,9 @@ int launch_layerscale_bwd(const float* dx, int ldx, const __nv_bfloat16* branch,
 int launch_colsum_ordered(const void* in, bool bf16, int ld, int rows, int cols, float* out, float* workspace, cudaStream_t st) {
   DVT_REQUIRE(in && out && workspace && rows > 0 && cols > 0, "colsum_ordered: bad arguments");
   DVT_REQUIRE(cols % 4 == 0 && ld % 4 == 0, "colsum_ordered: cols=%d and ld=%d must be multiples of 4", cols, ld);
+  DVT_REQUIRE(ld >= cols, "colsum_ordered: row pitch ld=%d must be >= cols=%d", ld, cols);
+  DVT_REQUIRE(!misaligned(in, bf16 ? 8 : 16), "colsum_ordered: in must be %d-byte aligned", bf16 ? 8 : 16);
+  DVT_REQUIRE(!misaligned(workspace, 16), "colsum_ordered: workspace must be 16-byte aligned");
   const int chunks = det_chunks(rows);
   const dim3 grid((cols + 127) / 128, chunks);
   if (bf16)
@@ -164,6 +172,9 @@ int launch_vit_embed_bwd(const float* dx0, int B, int ntok, int prefix, int C, _
   DVT_REQUIRE(dx0 && dpatch && dpos && dprefix && dbias && workspace, "vit_embed_bwd: null argument");
   DVT_REQUIRE(B > 0 && prefix >= 1 && ntok > prefix && C > 0 && C % 4 == 0, "vit_embed_bwd: bad shape B=%d ntok=%d prefix=%d C=%d",
               B, ntok, prefix, C);
+  DVT_REQUIRE(!misaligned(dx0, 16) && !misaligned(dpos, 16) && !misaligned(dprefix, 16) && !misaligned(workspace, 16),
+              "vit_embed_bwd: dx0, dpos, dprefix and workspace must be 16-byte aligned (float4 accesses)");
+  DVT_REQUIRE(!misaligned(dpatch, 8), "vit_embed_bwd: dpatch must be 8-byte aligned (4 x bf16 stores)");
   const size_t total = (size_t)ntok * (C / 4);
   const int blocks = (int)std::min<size_t>((total + 255) / 256, (size_t)num_sms() * 16);
   embed_bwd_kernel<<<blocks, 256, 0, st>>>(dx0, B, ntok, prefix, C, dpatch, dpos, dprefix);
@@ -276,8 +287,10 @@ layernorm_bwd_grouped_kernel(const float* __restrict__ x, const float* __restric
 int launch_layernorm_bwd_grouped(const float* x, const float* gamma, const float* dy, float* dx_accum, float* dgamma,
                                  float* dbeta, float* workspace, int rows, int C, float eps, int in_group, int skip,
                                  cudaStream_t st) {
-  DVT_REQUIRE(C % 4 == 0 && C <= 2048, "layernorm_bwd_grouped: C=%d unsupported", C);
+  DVT_REQUIRE(C > 0 && C % 4 == 0 && C <= 2048, "layernorm_bwd_grouped: C=%d unsupported", C);
   DVT_REQUIRE(x && gamma && dy && dx_accum && dgamma && dbeta && workspace, "layernorm_bwd_grouped: null argument");
+  DVT_REQUIRE(!misaligned(x, 16) && !misaligned(gamma, 16) && !misaligned(dy, 16) && !misaligned(dx_accum, 16),
+              "layernorm_bwd_grouped: x, gamma, dy and dx_accum must be 16-byte aligned (float4 accesses)");
   DVT_REQUIRE(in_group >= 1 && skip >= 0 && skip < in_group && rows % in_group == 0,
               "layernorm_bwd_grouped: bad rows=%d in_group=%d skip=%d", rows, in_group, skip);
   const int out_rows = rows / in_group * (in_group - skip);
@@ -306,6 +319,9 @@ int launch_vit_embed_fwd(const __nv_bfloat16* patches, int Kp, const __nv_bfloat
                          const float* prefix_rows, int B, int np, int prefix, int C, float* out, cudaStream_t st) {
   DVT_REQUIRE(patches && w && pos_patch && prefix_rows && out, "vit_embed_fwd: null argument");  // bias may be null
   DVT_REQUIRE(B > 0 && np > 0 && prefix >= 1 && C % 4 == 0 && Kp % 8 == 0, "vit_embed_fwd: bad shape");
+  // the GEMM epilogue adds bias and pos_patch and stores out four columns at a time (the GEMM checks them too, by role)
+  DVT_REQUIRE(!misaligned(out, 16) && !misaligned(bias, 16) && !misaligned(pos_patch, 16),
+              "vit_embed_fwd: out, bias and pos_patch must be 16-byte aligned (float4 accesses)");
   const int ntok = np + prefix;
   GemmEpi e;
   e.bias = bias; e.out_mode = OUT_F32_REMAP; e.out = out; e.ldo = C; e.addend = pos_patch;

@@ -760,7 +760,6 @@ int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dty
               "aligned [M, >= 2N] pre-activation / output with pitches that are multiples of 4");
   // The epilogue reads and writes four consecutive columns at once (float4 / uint2), so every pointer it touches must be
   // aligned for those accesses.  All checks run before any CUDA call: a bad argument is reported, never a fault.
-  auto misaligned = [](const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) != 0; };
   DVT_REQUIRE(!misaligned(epi.out, epi.out_mode == OUT_BF16 ? 8 : 16),
               "gemm: out must be %d-byte aligned", epi.out_mode == OUT_BF16 ? 8 : 16);
   DVT_REQUIRE(!misaligned(epi.bias, 16) && !misaligned(epi.gamma, 16) && !misaligned(epi.addend, 16),

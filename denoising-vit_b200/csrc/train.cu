@@ -105,8 +105,10 @@ layernorm_bwd_kernel(const float* __restrict__ x, const float* __restrict__ gamm
 
 int launch_layernorm_bwd(const float* x, const float* gamma, const float* dy, float* dx_accum, float* dgamma, float* dbeta,
                          int rows, int C, float eps, cudaStream_t st) {
-  DVT_REQUIRE(C % 4 == 0 && C <= 2048, "layernorm_bwd: C=%d unsupported", C);
+  DVT_REQUIRE(C > 0 && C % 4 == 0 && C <= 2048, "layernorm_bwd: C=%d unsupported", C);
   DVT_REQUIRE(x && gamma && dy && dx_accum && dgamma && dbeta, "layernorm_bwd: null argument");
+  DVT_REQUIRE(!misaligned(x, 16) && !misaligned(gamma, 16) && !misaligned(dy, 16) && !misaligned(dx_accum, 16),
+              "layernorm_bwd: x, gamma, dy and dx_accum must be 16-byte aligned (float4 accesses)");
   if (rows <= 0) return DVT_OK;
   const int nv = (C / 4 + 31) / 32;
   const int blocks = std::min(num_sms(), (rows + 7) / 8);
@@ -164,6 +166,8 @@ __global__ void __launch_bounds__(256) colsum_kernel(const T* __restrict__ in, i
 int launch_colsum(const void* in, bool bf16, int ld, int rows, int cols, float* out, cudaStream_t st) {
   DVT_REQUIRE(in && out && rows > 0 && cols > 0, "colsum: bad arguments");
   DVT_REQUIRE(!bf16 || (cols % 2 == 0 && ld % 2 == 0), "colsum: bf16 input needs even cols / pitch");
+  DVT_REQUIRE(ld >= cols, "colsum: row pitch ld=%d must be >= cols=%d", ld, cols);
+  DVT_REQUIRE(!misaligned(in, 4), "colsum: in must be 4-byte aligned (bf16x2 / f32 loads)");
   const int strip = bf16 ? 64 : 32;
   const int gx = (cols + strip - 1) / strip;
   const int gy = std::max(1, std::min((rows + 63) / 64, (num_sms() * 4 + gx - 1) / gx));
@@ -307,7 +311,9 @@ __global__ void loss_final_kernel(const float* __restrict__ part, int n, float* 
 int launch_denoise_loss(const float* pred, const float* tgt, float* dpred, float* losses, int rows, int C, float grad_scale,
                         cudaStream_t st) {
   DVT_REQUIRE(pred && tgt && losses && rows > 0, "denoise_loss: bad arguments");
-  DVT_REQUIRE(C % 4 == 0 && C <= 2048, "denoise_loss: C=%d unsupported", C);
+  DVT_REQUIRE(C > 0 && C % 4 == 0 && C <= 2048, "denoise_loss: C=%d unsupported", C);
+  DVT_REQUIRE(!misaligned(pred, 16) && !misaligned(tgt, 16) && !misaligned(dpred, 16),
+              "denoise_loss: pred, target and dpred must be 16-byte aligned (float4 accesses)");
   const int nv = (C / 4 + 31) / 32;
   const int blocks = std::min(num_sms() * 4, (rows + 7) / 8);
   DVT_CUDA_OK(cudaMemsetAsync(losses, 0, 3 * sizeof(float), st));
@@ -327,7 +333,9 @@ int launch_denoise_loss(const float* pred, const float* tgt, float* dpred, float
 int launch_denoise_loss_ordered(const float* pred, const float* tgt, float* dpred, float* losses, float* workspace, int rows,
                                 int C, float grad_scale, cudaStream_t st) {
   DVT_REQUIRE(pred && tgt && losses && workspace && rows > 0, "denoise_loss_ordered: bad arguments");
-  DVT_REQUIRE(C % 4 == 0 && C <= 2048, "denoise_loss_ordered: C=%d unsupported", C);
+  DVT_REQUIRE(C > 0 && C % 4 == 0 && C <= 2048, "denoise_loss_ordered: C=%d unsupported", C);
+  DVT_REQUIRE(!misaligned(pred, 16) && !misaligned(tgt, 16) && !misaligned(dpred, 16),
+              "denoise_loss_ordered: pred, target and dpred must be 16-byte aligned (float4 accesses)");
   const int nv = (C / 4 + 31) / 32;
   const int blocks = std::min(num_sms() * 4, (rows + 7) / 8);
 #define DVT_DL(NV) denoise_loss_kernel<NV, true><<<blocks, 256, 0, st>>>(pred, tgt, dpred, workspace, rows, C, grad_scale)
@@ -414,6 +422,8 @@ int launch_adamw(float* p, const float* g, float* m, float* v, size_t n, double 
   DVT_REQUIRE(p && g && m && v, "adamw: null argument");
   DVT_REQUIRE(n % 4 == 0, "adamw: the flat buffer must hold a multiple of 4 elements (got %zu)", n);
   DVT_REQUIRE(step >= 1, "adamw: step counts from 1");
+  DVT_REQUIRE(!misaligned(p, 16) && !misaligned(g, 16) && !misaligned(m, 16) && !misaligned(v, 16),
+              "adamw: p, g, m and v must be 16-byte aligned (float4 accesses)");
   if (n == 0) return DVT_OK;
   const double bc1 = 1.0 - pow(beta1, (double)step), bc2 = 1.0 - pow(beta2, (double)step);
   const size_t n4 = n / 4;

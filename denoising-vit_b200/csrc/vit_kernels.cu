@@ -106,17 +106,26 @@ static void launch_ln_nv(int nv, int blocks, int threads, cudaStream_t stream, c
 
 int launch_layernorm(const float* x, int ldx, const float* gamma, const float* beta, void* y, int ldy, bool out_bf16,
                      int rows, int C, float eps, int in_group, int skip, cudaStream_t stream) {
-  DVT_REQUIRE(C % 4 == 0 && C <= 2048 && ldx % 4 == 0 && ldy % 4 == 0, "layernorm: C=%d ldx=%d ldy=%d unsupported", C,
-              ldx, ldy);
+  DVT_REQUIRE(C > 0 && C % 4 == 0 && C <= 2048 && ldx % 4 == 0 && ldy % 4 == 0, "layernorm: C=%d ldx=%d ldy=%d unsupported",
+              C, ldx, ldy);
+  DVT_REQUIRE(ldx >= C && ldy >= C, "layernorm: row pitches ldx=%d and ldy=%d must be >= C=%d", ldx, ldy, C);
+  // skip > 0 compacts whole groups: a partial last group would map its rows past rows / in_group * (in_group - skip)
+  DVT_REQUIRE(in_group >= 1 && skip >= 0 && skip < in_group && (skip == 0 || rows % in_group == 0),
+              "layernorm: bad in_group=%d / skip=%d for rows=%d (0 <= skip < in_group; rows %% in_group == 0 when skip > 0)",
+              in_group, skip, rows);
+  // float4 loads of x, gamma and beta; float4 (f32) or uint2 (bf16) stores of y
+  DVT_REQUIRE(!misaligned(x, 16), "layernorm: x must be 16-byte aligned");
+  DVT_REQUIRE(!misaligned(gamma, 16) && !misaligned(beta, 16), "layernorm: gamma and beta must be 16-byte aligned");
+  DVT_REQUIRE(!misaligned(y, out_bf16 ? 8 : 16), "layernorm: y must be %d-byte aligned", out_bf16 ? 8 : 16);
   if (rows <= 0) return DVT_OK;
   const int threads = 256;
   const int blocks = (rows * 32 + threads - 1) / threads;  // upper bound; launch_ln_one caps it at one full wave
   const int nv = (C / 4 + 31) / 32;
-  const int grp = in_group > 0 ? in_group : 1;
   if (out_bf16)
-    launch_ln_nv<__nv_bfloat16>(nv, blocks, threads, stream, x, ldx, gamma, beta, (__nv_bfloat16*)y, ldy, rows, C, eps, grp, skip);
+    launch_ln_nv<__nv_bfloat16>(nv, blocks, threads, stream, x, ldx, gamma, beta, (__nv_bfloat16*)y, ldy, rows, C, eps, in_group,
+                                skip);
   else
-    launch_ln_nv<float>(nv, blocks, threads, stream, x, ldx, gamma, beta, (float*)y, ldy, rows, C, eps, grp, skip);
+    launch_ln_nv<float>(nv, blocks, threads, stream, x, ldx, gamma, beta, (float*)y, ldy, rows, C, eps, in_group, skip);
   DVT_CUDA_OK(cudaGetLastError());
   count_launch();
   return DVT_OK;

@@ -75,7 +75,9 @@ int dvt_gemm_tn_residual(const void* A, int lda, const void* B, int ldb, int dty
 
 /* y = LayerNorm(x) over rows of C fp32 (eps inside the sqrt, affine gamma/beta), output bf16 or fp32.
  * in_group/skip: rows are grouped in runs of `in_group`; the first `skip` rows of every group are dropped and the
- * output is compacted (used to strip prefix tokens); pass in_group=1, skip=0 for a plain LayerNorm.
+ * output is compacted (used to strip prefix tokens); pass in_group=1, skip=0 for a plain LayerNorm.  0 <= skip < in_group,
+ * and rows % in_group == 0 when skip > 0.  C % 4 == 0, 4 <= C <= 2048; ldx, ldy >= C and multiples of 4.  Alignment:
+ * x, gamma and beta 16 bytes; y 16 bytes (f32) or 8 bytes (bf16).
  * Replaces: nn.LayerNorm(eps=1e-6) in timm Block / VisionTransformer.norm. */
 int dvt_layernorm(const float* x, int ldx, const float* gamma, const float* beta, void* y, int ldy, int y_dtype,
                   int rows, int C, float eps, int in_group, int skip, void* stream);
@@ -233,19 +235,22 @@ int dvt_fit_sweep_once(dvt_fit_t* h, int ctas, void* stream);
  * [B, heads, N]. */
 int dvt_attention_bwd(const void* qkv_bf16, const void* out_bf16, const void* dout_bf16, const float* lse, void* dqkv_bf16,
                       float* dq_workspace, float* delta_workspace, int B, int N, int heads, int head_dim, void* stream);
-/* LayerNorm backward: dx_accum [rows, C] += d/dx, dgamma / dbeta [C] += their gradients (all f32; x is the LN input). */
+/* LayerNorm backward: dx_accum [rows, C] += d/dx, dgamma / dbeta [C] += their gradients (all f32; x is the LN input).
+ * C % 4 == 0, C <= 2048; x, gamma, dy and dx_accum 16-byte aligned. */
 int dvt_layernorm_bwd(const float* x, const float* gamma, const float* dy, float* dx_accum, float* dgamma, float* dbeta,
                       int rows, int C, float eps, void* stream);
-/* out_accum[n] += sum_m in[m, n]  (bias gradients); in: bf16 or f32 [rows, cols] with row pitch ld. */
+/* out_accum[n] += sum_m in[m, n]  (bias gradients); in: bf16 or f32 [rows, cols] with row pitch ld >= cols, 4-byte
+ * aligned (bf16: cols and ld even). */
 int dvt_colsum(const void* in, int dtype, int ld, int rows, int cols, float* out_accum, void* stream);
 /* out = gelu(in), erf form, bf16, n % 8 == 0  (forward of the MLP activation when the pre-activation must be kept). */
 int dvt_gelu(const void* in_bf16, void* out_bf16, size_t n, void* stream);
 /* Loss of main_denoiser.py:214-217 and its gradient: losses3 = (l2 + cos, l2 = mse, cos = 1 - mean cosine similarity);
- * dpred (optional) = grad_scale * d(l2 + cos)/dpred.  pred, target, dpred f32 [rows, C]. */
+ * dpred (optional) = grad_scale * d(l2 + cos)/dpred.  pred, target, dpred f32 [rows, C], 16-byte aligned; C % 4 == 0,
+ * C <= 2048. */
 int dvt_denoise_loss(const float* pred, const float* target, float* dpred, float* losses3, int rows, int C, float grad_scale,
                      void* stream);
 /* torch.optim.AdamW step (main_denoiser.py:176-180,220) over one flat f32 buffer of n (multiple of 4) parameters;
- * step counts from 1. */
+ * step counts from 1.  p, g, m and v 16-byte aligned. */
 int dvt_adamw(float* p, const float* g, float* m, float* v, size_t n, double lr, double beta1, double beta2, double eps,
               double weight_decay, long long step, void* stream);
 
@@ -259,23 +264,26 @@ int dvt_adamw(float* p, const float* g, float* m, float* v, size_t n, double lr,
 /* Backward of x += gamma * branch (branch = A.B^T + bias): one pass over dx (f32 [rows, C], row pitch ldx) that writes
  * dbranch = gamma * dx (bf16 [rows, C], optional), dbias[C] = sum_rows gamma * dx and, when dgamma is given, dgamma[C] =
  * sum_rows dx * branch (branch: the bf16 [rows, C] side output of dvt_gemm_tn_residual).  gamma NULL: unit scale (no
- * LayerScale): the call casts dx to bf16 and sums its columns.  dbias / dgamma are overwritten. */
+ * LayerScale): the call casts dx to bf16 and sums its columns.  dbias / dgamma are overwritten.  C and ldx >= C multiples
+ * of 4; dx, gamma and workspace 16-byte aligned, branch and dbranch 8-byte aligned. */
 int dvt_layerscale_bwd(const float* dx, int ldx, const void* branch_bf16, const float* gamma, void* dbranch_bf16, float* dbias,
                        float* dgamma, float* workspace, int rows, int C, void* stream);
 /* Token assembly of the ViT forward on caller-owned tensors: out [B, prefix + np, C] f32 = patch rows
  * patches (bf16 [B*np, Kp], dvt_im2col) . w^T (bf16 [C, Kp], zero-padded conv weight) + bias + pos_patch[p] after
  * `prefix` rows copied from prefix_rows [prefix, C] (what dvt_vit_forward does before the first block).  bias may be
- * NULL: a patch embedding without bias (the CLIP towers). */
+ * NULL: a patch embedding without bias (the CLIP towers).  out, bias and pos_patch 16-byte aligned. */
 int dvt_vit_embed_fwd(const void* patches_bf16, int Kp, const void* w_bf16, const float* bias, const float* pos_patch,
                       const float* prefix_rows, int B, int np, int prefix, int C, float* out, void* stream);
 /* Backward of dvt_vit_embed_fwd w.r.t. everything but the image: from dx0 (f32 [B, ntok, C], ntok = prefix + np) writes
  * dpatch (bf16 [B*np, C], the patch rows compacted: the dY of the patch-embed weight gradient), dpos (f32 [np, C], summed
- * over the batch), dprefix (f32 [prefix, C], summed over the batch) and dbias (f32 [C]).  All overwritten. */
+ * over the batch), dprefix (f32 [prefix, C], summed over the batch) and dbias (f32 [C]).  All overwritten.  dx0, dpos,
+ * dprefix and workspace 16-byte aligned, dpatch 8-byte aligned. */
 int dvt_vit_embed_bwd(const float* dx0, int B, int ntok, int prefix, int C, void* dpatch_bf16, float* dpos, float* dprefix,
                       float* dbias, float* workspace, void* stream);
 /* Backward of dvt_layernorm in its in_group / skip form (final norm + prefix strip): dy f32 [rows / in_group * (in_group -
  * skip), C] holds the compacted rows, x and dx_accum f32 [rows, C] the full ones; dx_accum += d/dx on the kept rows only
- * (the skipped rows are not touched); dgamma / dbeta [C] are overwritten. */
+ * (the skipped rows are not touched); dgamma / dbeta [C] are overwritten.  0 <= skip < in_group, rows % in_group == 0;
+ * x, gamma, dy and dx_accum 16-byte aligned. */
 int dvt_layernorm_bwd_grouped(const float* x, const float* gamma, const float* dy, float* dx_accum, float* dgamma, float* dbeta,
                               float* workspace, int rows, int C, float eps, int in_group, int skip, void* stream);
 /* SwiGLU MLP (timm SwiGLUPacked, ViT-g/14): out [M, Hh] = silu(g) * u with [g | u] = hpre [M, 2 Hh] (bf16, contiguous), the
@@ -303,10 +311,11 @@ int dvt_attention_bwd_det(const void* qkv_bf16, const void* out_bf16, const void
  * with plain stores into plane s of workspace (f32 [splits, M, ldo]), then the planes are added in split order. */
 int dvt_gemm_bf16_wgrad_ordered(const void* dy_bf16, int ld_dy, const void* x_bf16, int ldx, int M, int N, int K, float* out,
                                 int ldo, int splits, float* workspace, void* stream);
-/* out[c] = sum_r in[r, c] (overwritten) in a fixed order; in bf16 or f32 [rows, cols], cols and ld multiples of 4;
- * workspace f32 [256 * cols]. */
+/* out[c] = sum_r in[r, c] (overwritten) in a fixed order; in bf16 or f32 [rows, cols], cols and ld >= cols multiples of 4,
+ * in 16-byte (f32) or 8-byte (bf16) aligned; workspace f32 [256 * cols], 16-byte aligned. */
 int dvt_colsum_ordered(const void* in, int dtype, int ld, int rows, int cols, float* out, float* workspace, void* stream);
-/* dvt_denoise_loss with per-CTA partials added in a fixed order (losses3 overwritten); workspace f32 [2 * ceil(rows / 8)]. */
+/* dvt_denoise_loss with per-CTA partials added in a fixed order (losses3 overwritten); workspace f32 [2 * ceil(rows / 8)].
+ * Same shape and alignment rules as dvt_denoise_loss. */
 int dvt_denoise_loss_ordered(const float* pred, const float* target, float* dpred, float* losses3, float* workspace, int rows,
                              int C, float grad_scale, void* stream);
 /* Backward of a separable resampling of a [gh, gw, C] grid to [h, w, C] (the bicubic antialiased position-embedding

@@ -80,6 +80,15 @@ int launch_seg_aug_accumulate(const float* acc, const float* count, int K, int H
                               int Wo, cudaStream_t st);
 int launch_seg_aug_argmax_hist(const float* prob, int n_aug, int K, const uint8_t* labels, int Ho, int Wo,
                                unsigned long long* hist, cudaStream_t st);
+int launch_depth_head_fwd(const float* logits, int B, int h, int w, int K, int up, const float* bins, float* depth,
+                          cudaStream_t st);
+int launch_depth_head_bwd(const float* logits, int B, int h, int w, int K, int up, const float* bins, const float* ddepth,
+                          float* dlogits, cudaStream_t st);
+int launch_depth_resize_fwd(const float* in, int B, int Hi, int Wi, float* out, int Ho, int Wo, cudaStream_t st);
+int launch_depth_resize_bwd(const float* dout, int B, int Hi, int Wi, int Ho, int Wo, float* din, cudaStream_t st);
+int launch_depth_eval_sums(const float* maps, int n_aug, unsigned int flip_mask, int Hu, int Wu, const float* gt, int Ho,
+                           int Wo, float min_depth, float max_depth, int cy0, int cy1, int cx0, int cx1, double* workspace,
+                           double* sums, cudaStream_t st);
 const char* last_error();
 }  // namespace dvt
 
@@ -87,7 +96,7 @@ using namespace dvt;
 
 extern "C" {
 
-int dvt_version(void) { return 101; }
+int dvt_version(void) { return 102; }
 
 const char* dvt_last_error(void) { return dvt::last_error(); }
 
@@ -466,6 +475,26 @@ int dvt_seg_aug_accumulate(const float* acc, const float* count, int K, int Hc, 
 int dvt_seg_aug_argmax_hist(const float* prob, int n_aug, int K, const uint8_t* labels, int Ho, int Wo,
                             unsigned long long* hist, void* stream) {
   return launch_seg_aug_argmax_hist(prob, n_aug, K, labels, Ho, Wo, hist, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int dvt_depth_head_fwd(const float* logits, int B, int h, int w, int K, int up, const float* bins, float* depth, void* stream) {
+  return launch_depth_head_fwd(logits, B, h, w, K, up, bins, depth, reinterpret_cast<cudaStream_t>(stream));
+}
+int dvt_depth_head_bwd(const float* logits, int B, int h, int w, int K, int up, const float* bins, const float* ddepth,
+                       float* dlogits, void* stream) {
+  return launch_depth_head_bwd(logits, B, h, w, K, up, bins, ddepth, dlogits, reinterpret_cast<cudaStream_t>(stream));
+}
+int dvt_depth_resize_fwd(const float* in, int B, int Hi, int Wi, float* out, int Ho, int Wo, void* stream) {
+  return launch_depth_resize_fwd(in, B, Hi, Wi, out, Ho, Wo, reinterpret_cast<cudaStream_t>(stream));
+}
+int dvt_depth_resize_bwd(const float* dout, int B, int Hi, int Wi, int Ho, int Wo, float* din, void* stream) {
+  return launch_depth_resize_bwd(dout, B, Hi, Wi, Ho, Wo, din, reinterpret_cast<cudaStream_t>(stream));
+}
+int dvt_depth_eval_sums(const float* maps, int n_aug, unsigned int flip_mask, int Hu, int Wu, const float* gt, int Ho, int Wo,
+                        float min_depth, float max_depth, int cy0, int cy1, int cx0, int cx1, double* workspace,
+                        double* sums, void* stream) {
+  return launch_depth_eval_sums(maps, n_aug, flip_mask, Hu, Wu, gt, Ho, Wo, min_depth, max_depth, cy0, cy1, cx0, cx1,
+                                workspace, sums, reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("DVT_LIB_PATH") or os.path.join(os.path.dirname(_HERE), "libdvt_b200.so")
 # dvt_version() of the library SIGNATURES describes.  A library with another version is refused: an entry point may keep
 # its name across versions but take other arguments, and calling it through these argtypes would pass garbage pointers.
-ABI_VERSION = 101
+ABI_VERSION = 102
 
 
 class DvtError(RuntimeError):
@@ -96,6 +96,12 @@ SIGNATURES = {
     "dvt_seg_predict_hist": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "dvt_seg_aug_accumulate": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
     "dvt_seg_aug_argmax_hist": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "dvt_depth_head_fwd": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "dvt_depth_head_bwd": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "dvt_depth_resize_fwd": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "dvt_depth_resize_bwd": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "dvt_depth_eval_sums": (c_int, [c_void_p, c_int, c_uint, c_int, c_int, c_void_p, c_int, c_int, c_float, c_float, c_int,
+                                    c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "dvt_vit_create": (c_int, [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_int,
                                c_int]),
     "dvt_vit_destroy": (None, [c_void_p]),

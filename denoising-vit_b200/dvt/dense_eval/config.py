@@ -150,3 +150,72 @@ def check_supported(cfg: Dict[str, Any]) -> None:
             steps.extend(step.get("transforms", []))
         for step in steps:
             _require(step.get("type") in allowed, f"data.{split} pipeline step {step.get('type')!r} is not implemented")
+
+
+DEPTH_TRAIN_PIPELINE = ("LoadImageFromFile", "DepthLoadAnnotations", "NYUCrop", "RandomRotate", "RandomFlip", "RandomCrop",
+                        "ColorAug", "Normalize", "DefaultFormatBundle", "Collect")
+DEPTH_TEST_PIPELINE = ("LoadImageFromFile", "MultiScaleFlipAug", "RandomFlip", "Normalize", "ImageToTensor", "Collect")
+MAX_DEPTH_BINS = 256
+
+
+def check_supported_depth(cfg: Dict[str, Any]) -> None:
+    """The NYU depth probe (vitb_nyu_linear_config.py): refuses, naming it, what `dvt.dense_eval.depth` does not
+    implement."""
+    model = cfg.get("model", {})
+    _require(model.get("type") == "DepthEncoderDecoder",
+             f"model type {model.get('type')!r}: the depth probe implements DepthEncoderDecoder")
+    bb = model.get("backbone", {})
+    _require(bb.get("output_cls_token", True),
+             "backbone output_cls_token=False is not implemented (the reference's format_output would then index the batch)")
+    head = model.get("decode_head", {})
+    _require(head.get("type") == "BNHead", f"decode_head type {head.get('type')!r}: only the linear BNHead is implemented")
+    _require(head.get("classify", False), "BNHead classify=False (direct regression) is not implemented")
+    _require(head.get("bins_strategy", "UD") == "UD", f"BNHead bins_strategy {head.get('bins_strategy')!r}: only UD is "
+             f"implemented (SID is not)")
+    _require(head.get("norm_strategy", "linear") == "linear",
+             f"BNHead norm_strategy {head.get('norm_strategy')!r}: only linear is implemented")
+    _require(int(head.get("n_bins", 256)) <= MAX_DEPTH_BINS,
+             f"BNHead n_bins {head.get('n_bins')}: at most {MAX_DEPTH_BINS} bins are implemented")
+    _require(head.get("input_transform") == "resize_concat",
+             f"BNHead input_transform {head.get('input_transform')!r}: only resize_concat is implemented")
+    _require(not head.get("align_corners", False), "BNHead align_corners=True is not implemented")
+    _require(not head.get("scale_up", False), "BNHead scale_up is not implemented")
+    losses = head.get("loss_decode", [])
+    losses = [losses] if isinstance(losses, dict) else list(losses)
+    kinds = [(l.get("type"), l.get("valid_mask", True), l.get("max_depth")) for l in losses]
+    _require(sorted(k[0] for k in kinds) == ["GradientLoss", "SigLoss"] and all(k[1] and k[2] is None for k in kinds),
+             f"loss_decode {losses}: only SigLoss + GradientLoss with valid_mask and no max_depth are implemented")
+    test_cfg = model.get("test_cfg", cfg.get("test_cfg", {})) or {}
+    _require(test_cfg.get("mode") == "whole", f"test_cfg mode {test_cfg.get('mode')!r}: only whole inference is implemented")
+    opt = cfg.get("optimizer", {})
+    _require(opt.get("type") == "AdamW", f"optimizer {opt.get('type')!r}: only AdamW is implemented")
+    pw = opt.get("paramwise_cfg") or {}
+    _require(set(pw) <= {"custom_keys"}, f"optimizer paramwise_cfg {sorted(pw)}: only custom_keys is implemented")
+    lr = cfg.get("lr_config", {})
+    _require(lr.get("policy") == "CosineAnnealing" and not lr.get("by_epoch", False) and "min_lr" not in lr,
+             f"lr_config policy {lr.get('policy')!r}: only the iteration-based CosineAnnealing schedule with min_lr_ratio "
+             f"is implemented")
+    _require(lr.get("warmup") in (None, "linear"), f"lr_config warmup {lr.get('warmup')!r}: only linear warmup is implemented")
+    mom = cfg.get("momentum_config")
+    _require(mom is None or mom.get("policy") == "OneCycle",
+             f"momentum_config policy {(mom or {}).get('policy')!r}: only OneCycle is implemented")
+    _require(cfg.get("runner", {}).get("type") == "IterBasedRunner", "runner: only IterBasedRunner is implemented")
+    _require(len(cfg.get("workflow", [("train", 1)])) == 1, "workflow: only [('train', 1)] is implemented")
+    oc = cfg.get("optimizer_config", {}) or {}
+    clip = oc.get("grad_clip")
+    _require((clip is None or clip.get("norm_type", 2) == 2) and not oc.get("use_fp16", False)
+             and oc.get("update_interval", 1) == 1,
+             "optimizer_config: only L2 gradient clipping, without fp16 or accumulation, is implemented")
+    ev = cfg.get("evaluation", {})
+    _require(ev.get("rule", "less") in ("less", "greater"), f"evaluation rule {ev.get('rule')!r} is not implemented")
+    data = cfg.get("data", {})
+    for split in ("train", "val"):
+        ds = data.get(split, {})
+        _require(ds.get("type") == "NYUDataset", f"data.{split} type {ds.get('type')!r}: only NYUDataset is implemented")
+        _require(ds.get("split") is not None, f"data.{split}: a split file is required (as in the reference)")
+        allowed = DEPTH_TRAIN_PIPELINE if split == "train" else DEPTH_TEST_PIPELINE
+        steps = list(ds.get("pipeline", []))
+        for step in list(steps):
+            steps.extend(step.get("transforms", []))
+        for step in steps:
+            _require(step.get("type") in allowed, f"data.{split} pipeline step {step.get('type')!r} is not implemented")

@@ -158,7 +158,9 @@ class RandomCrop:
                     break
                 box = self.bbox(r["img"], rng)
         r["img"] = r["img"][box[0]:box[1], box[2]:box[3]]
-        r["seg"] = r["seg"][box[0]:box[1], box[2]:box[3]]
+        for k in ("seg", "depth"):
+            if k in r:
+                r[k] = r[k][box[0]:box[1], box[2]:box[3]]
         return r
 
 
@@ -171,8 +173,9 @@ class RandomFlip:
     def __call__(self, r, rng):
         if r["flip"] if "flip" in r else (self.prob is not None and rng.rand() < self.prob):
             r["img"] = r["img"][:, ::-1]
-            if "seg" in r:
-                r["seg"] = r["seg"][:, ::-1]
+            for k in ("seg", "depth"):
+                if k in r:
+                    r[k] = r[k][:, ::-1]
         return r
 
 
@@ -268,11 +271,12 @@ def multiscale_flip_augs(kw: dict) -> List[Aug]:
     return [(s, f) for s in scales for f in ((False, True) if flip else (False,))]
 
 
-def build_pipeline(steps: List[dict]) -> Tuple[list, bool, List[Aug]]:
+def build_pipeline(steps: List[dict], table: Optional[Dict[str, type]] = None) -> Tuple[list, bool, List[Aug]]:
     """(transforms, reduce_zero_label of LoadAnnotations, test-time augmentations).  MultiScaleFlipAug is flattened.
     With one augmentation its scale becomes the img_scale of an inner Resize without one.  With several, each
     augmentation runs the transforms with `scale` and `flip` preset; a pipeline without MultiScaleFlipAug has the single
-    augmentation (None, False)."""
+    augmentation (None, False).  `table` maps step names to classes (default: the segmentation steps)."""
+    table = _STEPS if table is None else table
     out, rzl, augs, outside = [], False, [(None, False)], 0
     for step in steps:
         kw = dict(step)
@@ -283,14 +287,14 @@ def build_pipeline(steps: List[dict]) -> Tuple[list, bool, List[Aug]]:
             rzl = bool(kw.get("reduce_zero_label", False))
         elif t == "MultiScaleFlipAug":
             augs = multiscale_flip_augs(kw)
-            inner, _, _ = build_pipeline(kw.get("transforms", []))
+            inner, _, _ = build_pipeline(kw.get("transforms", []), table)
             if len(augs) == 1:
                 for tr in inner:
                     if isinstance(tr, Resize) and tr.img_scale is None:
                         tr.img_scale = augs[0][0]
             out.extend(inner)
-        elif t in _STEPS:
-            out.append(_STEPS[t](**kw))
+        elif t in table:
+            out.append(table[t](**kw))
             outside += 1
         else:
             raise ConfigError(f"pipeline step {t!r} is not implemented")

@@ -57,11 +57,17 @@ def build_backbone(backbone_type: str, load_distilled_model_from: Optional[str] 
 
 class ProbeBackbone(nn.Module):
     """Frozen feature extractor of the probe: x [B, 3, H, W] -> NHWC [B, h, w, C * len(in_index)] (the `resize_concat`
-    input of the BNHead; the selected maps all share one grid, so the resize is the identity)."""
+    input of the BNHead; the selected maps all share one grid, so the resize is the identity).
 
-    def __init__(self, model: nn.Module, out_indices: Sequence[int], in_index: Sequence[int]):
+    The depth probe (`return_cls=True`, `norm=final_norm`) reads the ViT with `get_intermediate_layers(...,
+    return_prefix_tokens=True, norm=norm)` and the Denoiser with `denoiser(x, return_class_token=True, norm=norm)`, and
+    returns (features, cls [B, C * len(in_index)]) with prefix token 0 (the cls token, registers or not) per map."""
+
+    def __init__(self, model: nn.Module, out_indices: Sequence[int], in_index: Sequence[int], return_cls: bool = False,
+                 norm: bool = False):
         super().__init__()
         self.model = model
+        self.return_cls, self.norm = return_cls, norm
         self.is_denoiser = isinstance(model, Denoiser)
         vit = model.vit if self.is_denoiser else model
         self.pad = CenterPadding(vit.model.patch_embed.patch_size[0])
@@ -70,8 +76,19 @@ class ProbeBackbone(nn.Module):
         self.channels = vit.n_output_dims * len(self.in_index)
 
     @torch.no_grad()
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
+    def forward(self, x: torch.Tensor):
         x = self.pad(x)
+        if self.return_cls:
+            if self.is_denoiser:
+                f, c = self.model(x, return_class_token=True, norm=self.norm)
+                feats, cls = [f] * len(self.in_index), [c] * len(self.in_index)
+            else:
+                outs = self.model.get_intermediate_layers(x, n=self.layers, reshape=True, return_prefix_tokens=True,
+                                                          norm=self.norm)
+                feats, cls = [o[0].permute(0, 2, 3, 1) for o in outs], [o[1][:, 0] for o in outs]
+            if len(feats) == 1:
+                return feats[0], cls[0]
+            return torch.cat(feats, dim=-1), torch.cat(cls, dim=-1)
         if self.is_denoiser:
             f = self.model(x)                                  # [B, h, w, C]
             feats = [f] * len(self.in_index)

@@ -12,25 +12,20 @@ data.val.pipeline.1.flip=True`).
 Outputs in the work dir: `iter_<n>.pth` every checkpoint_config.interval iterations and at the end ({"state_dict":
 decode_head.* weights, "optimizer", "iter"}), `latest.pth` pointing at the newest, and `<timestamp>.log.json` (one JSON
 object per line: training losses every log_config.interval iterations, and mIoU, mAcc, aAcc, per-class IoU / Acc of
-every evaluation, as fractions).  `--task depth` (the NYU depth probe) is not implemented.
+every evaluation, as fractions).  `--task depth` is refused: the NYU depth probe is evaluate_depth.py.
 
 Launch: `--launcher none` runs one process; `--launcher pytorch` (the default, as in the reference) runs under torchrun,
 one process per GPU, with SyncBatchNorm in the head and DDP over NCCL."""
 import argparse
 import os
 import os.path as osp
-import random
 import sys
-import time
-import warnings
-
-import numpy as np
-import torch
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(ROOT, "denoising-vit_b200"))
 
-from dvt.dense_eval import DictAction, check_supported, load_config, merge_options  # noqa: E402
+from dvt.dense_eval import DictAction, check_supported  # noqa: E402
+from dvt.dense_eval.launch import finish_run, init_run, load_run_config  # noqa: E402
 
 
 def parse_args(argv=None):
@@ -65,72 +60,17 @@ def parse_args(argv=None):
 
 def main(args):
     if args.task == "depth":
-        raise NotImplementedError("--task depth: the NYU depth probe (reference build_depther, evaluation/depth: the "
-                                  "depther, its decode head and datasets) is not implemented; only segmentation is")
-    cfg = load_config(args.config)
-    if args.cfg_options is not None:
-        merge_options(cfg, args.cfg_options)
-    if args.options is not None:
-        warnings.warn("--options is deprecated in favor of --cfg-options")
-        merge_options(cfg, args.options)
-    check_supported(cfg)
-    if args.work_dir is not None:
-        cfg["work_dir"] = args.work_dir
-    elif cfg.get("work_dir") is None:
-        cfg["work_dir"] = osp.join("./work_dirs", osp.splitext(osp.basename(args.config))[0])
-    resume_from = args.resume_from if args.resume_from is not None else cfg.get("resume_from")
-    if resume_from is None and args.auto_resume and osp.exists(osp.join(cfg["work_dir"], "latest.pth")):
-        resume_from = osp.join(cfg["work_dir"], "latest.pth")
-
-    assert torch.cuda.is_available(), "the H100 segmentation probe needs a CUDA device (no CPU fallback)"
-    import torch.distributed as dist
-    if args.launcher == "none":
-        rank, world, local = 0, 1, 0
-    elif args.launcher == "pytorch":
-        if "RANK" not in os.environ or "WORLD_SIZE" not in os.environ:
-            raise RuntimeError("--launcher pytorch runs under torchrun (RANK / WORLD_SIZE are not set); use --launcher none "
-                               "for one process")
-        rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-    else:
-        raise NotImplementedError(f"--launcher {args.launcher}: only none and pytorch (torchrun) are implemented")
-    torch.cuda.set_device(local)
-    device = torch.device("cuda", local)
-    if args.launcher == "pytorch":
-        dist.init_process_group(cfg.get("dist_params", {}).get("backend", "nccl"), device_id=device)
-    os.makedirs(osp.abspath(cfg["work_dir"]), exist_ok=True)
-    timestamp = time.strftime("%Y%m%d_%H%M%S", time.localtime())
-
-    # init_random_seed: a random seed is drawn on rank 0 and shared; --diff_seed adds the rank
-    seed = args.seed
-    if seed is None:
-        t = torch.tensor([np.random.randint(2 ** 31)], dtype=torch.int64, device=device)
-        if world > 1:
-            dist.broadcast(t, 0)
-        seed = int(t.item())
-    if args.diff_seed:
-        seed += rank
-    random.seed(seed)
-    np.random.seed(seed)
-    torch.manual_seed(seed)
-    torch.cuda.manual_seed_all(seed)
-    if args.deterministic:
-        os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")
-        torch.use_deterministic_algorithms(True)
-        torch.backends.cudnn.benchmark = False
-    elif cfg.get("cudnn_benchmark", False):
-        torch.backends.cudnn.benchmark = True
-    if rank == 0:
-        print(f"Set random seed to {seed}, deterministic: {args.deterministic}; work dir {cfg['work_dir']}", flush=True)
-
+        raise NotImplementedError("--task depth: evaluate_dense_tasks.py runs the segmentation probe only; the NYU depth "
+                                  "probe is evaluate_depth.py (same flags and config files)")
+    cfg, resume_from = load_run_config(args, check_supported)
+    rank, world, device, seed, timestamp = init_run(args, cfg, "segmentation probe")
     from dvt.dense_eval.model import build_backbone
     from dvt.dense_eval.trainer import train
     backbone = build_backbone(args.backbone_type, args.load_distilled_model_from, args.load_denoiser_from, args.num_blocks,
                               device)
     out = train(cfg, backbone, cfg["work_dir"], seed, device, validate=not args.no_validate, resume_from=resume_from,
                 timestamp=timestamp, exp_name=osp.basename(args.config))
-    if world > 1:
-        dist.barrier()
-        dist.destroy_process_group()
+    finish_run(world)
     return out
 
 

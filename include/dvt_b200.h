@@ -372,6 +372,35 @@ int dvt_seg_aug_accumulate(const float* acc, const float* count, int K, int Hc, 
 int dvt_seg_aug_argmax_hist(const float* prob, int n_aug, int K, const uint8_t* labels, int Ho, int Wo,
                             unsigned long long* hist, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------
+ * Dense-task linear probe, NYU depth (reference evaluation/configs/vitb_nyu_linear_config.py: DepthEncoderDecoder with
+ * the BNHead, classify=True, UD bins, linear norm).  Resizes are ATen's bilinear upsample with align_corners=False in fp32.
+ * No float atomics: repeated calls are bit-identical.
+ * ------------------------------------------------------------------------------------------------------- */
+/* Bin-expectation head, forward.  logits f32 [B, h, w, K] (NHWC) are the head's 1x1-conv logits at the feature grid
+ * (conv and bilinear upsample commute); bins f32 [K] (device; torch.linspace(min_depth, max_depth, K)).  For every pixel
+ * of the (h * up) x (w * up) grid: r = bilinear(logits), a = relu(r) + 0.1, depth = sum_k a_k / sum_j a_j * bins_k.
+ * depth f32 [B, h * up, w * up] (overwritten).  1 <= K <= 256. */
+int dvt_depth_head_fwd(const float* logits, int B, int h, int w, int K, int up, const float* bins, float* depth, void* stream);
+/* Bin-expectation head, backward: ddepth f32 [B, h * up, w * up] -> dlogits f32 [B, h, w, K] (overwritten), gathered
+ * per low-resolution cell in a fixed order; d r_k = ddepth (bins_k - depth) / sum_j a_j where r_k > 0, else 0. */
+int dvt_depth_head_bwd(const float* logits, int B, int h, int w, int K, int up, const float* bins, const float* ddepth,
+                       float* dlogits, void* stream);
+/* One-channel bilinear resize in f32 [B, Hi, Wi] -> out [B, Ho, Wo] (overwritten). */
+int dvt_depth_resize_fwd(const float* in, int B, int Hi, int Wi, float* out, int Ho, int Wo, void* stream);
+/* Its backward in gather form: dout f32 [B, Ho, Wo] -> din f32 [B, Hi, Wi] (overwritten), each input cell summing the
+ * output pixels whose taps reach it in row-major order (deterministic, unlike the scatter of F.interpolate). */
+int dvt_depth_resize_bwd(const float* dout, int B, int Hi, int Wi, int Ho, int Wo, float* din, void* stream);
+/* Whole-image evaluation of one image: maps f32 [n_aug, Hu, Wu] are the head's depth per augmentation (bit a of
+ * flip_mask set: augmentation a was flipped horizontally); each is clamped to [min_depth, max_depth], resized to the
+ * original Ho x Wo, un-flipped, and the augmentations are averaged in fp32.  Pixels with min_depth < gt < max_depth
+ * (gt f32 [Ho, Wo]) inside rows [cy0, cy1) and columns [cx0, cx1) give sums f64 [10] (overwritten) = (count,
+ * #ratio < 1.25, < 1.25^2, < 1.25^3, sum |d|/gt, sum d^2/gt, sum d^2, sum err, sum err^2, sum |log10 gt - log10 pred|)
+ * with d = gt - pred, err = log pred - log gt.  workspace f64 [1280].  1 <= n_aug <= 32. */
+int dvt_depth_eval_sums(const float* maps, int n_aug, unsigned int flip_mask, int Hu, int Wu, const float* gt, int Ho, int Wo,
+                        float min_depth, float max_depth, int cy0, int cy1, int cx0, int cx1, double* workspace,
+                        double* sums, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -738,9 +738,31 @@ fit_adam_table_kernel(TableBufs tb, size_t nvec, const AdamScalars* __restrict__
   }
 }
 
+// The weights the data-gradient GEMMs read transposed (W1, W2, R2, R3): segment q is [rows[q], cols[q]] at off[q] of the
+// flat small-parameter buffer; its transpose [cols, rows] is kept at the same offset of Fit::wtsplit.
+struct TransSegs {
+  int off[4], rows[4], cols[4];
+};
+
+// TF32 hi / lo planes of element e of the small parameters into wt, transposed, if e lies in one of the segments
+__device__ __forceinline__ void split_store_t(const TransSegs& ts, float* __restrict__ wt, size_t plane, int e, float v) {
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const int l = e - ts.off[q];
+    if (l >= 0 && l < ts.rows[q] * ts.cols[q]) {
+      const int r = l / ts.cols[q], c = l - r * ts.cols[q];
+      const size_t o = (size_t)ts.off[q] + (size_t)c * ts.rows[q] + r;
+      const float hi = tf32_hi(v);
+      wt[o] = hi;
+      wt[plane + o] = v - hi;
+    }
+  }
+}
+
 // small params: one flat buffer; [g_lo, g_hi) is G, [r_lo, r_hi) the residual MLP, the rest the field MLP.
 __global__ void fit_adam_small_kernel(float4* __restrict__ p, float4* __restrict__ m, float4* __restrict__ v,
-                                      float4* __restrict__ g, float* __restrict__ wsplit, int nvec, int g_lo,
+                                      float4* __restrict__ g, float* __restrict__ wsplit, float* __restrict__ wtsplit,
+                                      TransSegs ts, int nvec, int g_lo,
                                       int g_hi, int r_lo, int r_hi, const AdamScalars* __restrict__ sc_main,
                                       const AdamScalars* __restrict__ sc_res, const int* __restrict__ step_base,
                                       int step_off, int freeze_step, float wd) {
@@ -765,6 +787,11 @@ __global__ void fit_adam_small_kernel(float4* __restrict__ p, float4* __restrict
       *reinterpret_cast<float4*>(wsplit + (size_t)i * 4) = hi;
       *reinterpret_cast<float4*>(wsplit + (size_t)(nvec + i) * 4) =
           make_float4(pp.x - hi.x, pp.y - hi.y, pp.z - hi.z, pp.w - hi.w);
+      const size_t plane = (size_t)nvec * 4;
+      split_store_t(ts, wtsplit, plane, 4 * i, pp.x);
+      split_store_t(ts, wtsplit, plane, 4 * i + 1, pp.y);
+      split_store_t(ts, wtsplit, plane, 4 * i + 2, pp.z);
+      split_store_t(ts, wtsplit, plane, 4 * i + 3, pp.w);
     }
   }
 }
@@ -789,12 +816,15 @@ __global__ void fit_transpose_kernel(const float* __restrict__ in, float* __rest
   }
 }
 
-// TF32 hi / lo operand planes of n parameters: wsplit[e] = hi, wsplit[plane + e] = lo
-__global__ void fit_split_kernel(const float* __restrict__ p, float* __restrict__ wsplit, size_t n, size_t plane) {
-  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (size_t)gridDim.x * blockDim.x) {
-    const float v = p[e], hi = tf32_hi(v);
+// TF32 hi / lo operand planes of the n parameters from element e0 of the small parameters: wsplit[e] = hi,
+// wsplit[plane + e] = lo, and the transposed planes in wtsplit for the elements in a segment of ts
+__global__ void fit_split_kernel(const float* __restrict__ sp, float* __restrict__ wsplit, float* __restrict__ wtsplit,
+                                 TransSegs ts, int e0, int n, size_t plane) {
+  for (int e = e0 + blockIdx.x * blockDim.x + threadIdx.x; e < e0 + n; e += gridDim.x * blockDim.x) {
+    const float v = sp[e], hi = tf32_hi(v);
     wsplit[e] = hi;
     wsplit[plane + e] = v - hi;
+    split_store_t(ts, wtsplit, plane, e, v);
   }
 }
 
@@ -835,13 +865,14 @@ struct Fit {
   bool epoch_forked = false;                   // this epoch forked sweeps onto sD (pipelined schedule)
   int sweep_steps[2] = {4, 4};                 // DVT_FIT_SWEEP_STEPS "k1,k2": window of the pipelined sweep per phase
   bool enc_ready = false;                      // f->enc already holds the encoding of the next step
-  int x3_wide_min_n[2] = {0, 256};             // DVT_FIT_X3_WIDE_MIN_N "p1,p2": 128 x 128 GEMM tiles when N >= this (0: never)
+  int x3_wide_min_n[2] = {0, 256};             // DVT_FIT_X3_WIDE_MIN_N "p1,p2": 128 x 128 weight-gradient tiles when N >= this (0: never)
   int wgrad_sms = 96;                          // DVT_FIT_WGRAD_SMS: weight-gradient GEMMs split K to fill at most this many SMs
   bool pdl = true;                             // DVT_FIT_PDL: programmatic dependent launch along the kernel chains of a step
   bool pipe[2] = {true, true};                 // software-pipelined table sweep in phase 1 / 2 (see fit_enqueue_step)
   int sweep_ctas[2] = {0, 0};                  // persistent sweep CTAs in phase 1 / 2 (0 = many small CTAs)
   float *sp = nullptr, *sm = nullptr, *sv = nullptr, *sg = nullptr;
   float* wsplit = nullptr;  // [2][n_small] TF32 hi / lo planes of the small params (x3 GEMM operands)
+  float* wtsplit = nullptr; // [2][n_small] the same planes of W1, W2, R2, R3 transposed (K-major B of the data gradients)
   // activations: GEMM operands are stored as two fp32 planes (hi, lo), plane stride = bsz * ld
   float *enc = nullptr, *h1 = nullptr, *dpred = nullptr, *dh1 = nullptr;
   float *Fout = nullptr, *denc = nullptr;
@@ -894,6 +925,13 @@ struct Fit {
   std::vector<void*> owned;
 };
 
+static TransSegs fit_trans_segs(const Fit* f) {
+  TransSegs t;
+  const Seg* s[4] = {&f->W1, &f->W2, &f->R2, &f->R3};
+  for (int q = 0; q < 4; ++q) { t.off[q] = s[q]->off; t.rows[q] = s[q]->rows; t.cols[q] = s[q]->cols; }
+  return t;
+}
+
 static int fit_prepare_kernels() {
   static bool done = false;
   if (done) return DVT_OK;
@@ -921,7 +959,7 @@ static int r8(int x) { return (x + 7) / 8 * 8; }
 //   DVT_FIT_PDL=0                 plain stream-ordered launches (no programmatic dependent launch)
 //   DVT_FIT_WGRAD_SMS=n           split-K of the weight-gradient GEMMs fills at most n SMs (they share the GPU with the
 //                                 data-gradient GEMMs of the critical path)
-//   DVT_FIT_X3_WIDE_MIN_N="a[,b]" per phase: 3xTF32 GEMMs with N >= this use 128 x 128 tiles (0: always 128 x 64)
+//   DVT_FIT_X3_WIDE_MIN_N="a[,b]" per phase: weight-gradient GEMMs with N >= this use 128 x 128 tiles (0: always 128 x 64)
 // (DVT_FIT_DEBUG_GRAPH=1 is read by fit_capture: it prints what each capture recorded.)
 static int fit_read_schedule_env(Fit* f) {
   int win[2] = {f->sweep_steps[0], f->sweep_steps[1]};
@@ -1017,6 +1055,7 @@ int fit_create(Fit** out, int C, int gh, int gw, int bsz, int n_levels, const fl
   A((void**)&f->tb.stamp, f->tb.ring * f->tb.n_entries * 4);
   A((void**)&f->sp, (size_t)off * 4); A((void**)&f->sm, (size_t)off * 4); A((void**)&f->sv, (size_t)off * 4);
   A((void**)&f->sg, (size_t)off * 4); A((void**)&f->wsplit, (size_t)off * 8);
+  A((void**)&f->wtsplit, (size_t)off * 8);
   const size_t n = bsz;
   A((void**)&f->enc, n * f->ld_enc * 8); A((void**)&f->h1, n * f->ld_h1 * 8); A((void**)&f->dpred, n * C * 8);
   A((void**)&f->dh1, n * H1 * 8); A((void**)&f->Fout, n * C * 4); A((void**)&f->denc, n * f->Lf * 4);
@@ -1134,7 +1173,8 @@ int fit_set_param(Fit* f, const char* name_c, const float* src, size_t numel, cu
   } else {
     DVT_CUDA_OK(cudaMemcpyAsync(f->sp + s->off, src, numel * 4, cudaMemcpyDefault, st));
     // the GEMMs read the weights as TF32 hi / lo planes: keep them current (fit_query / fit_residual may follow directly)
-    fit_split_kernel<<<64, 256, 0, st>>>(f->sp + s->off, f->wsplit + s->off, numel, (size_t)f->n_small);
+    fit_split_kernel<<<64, 256, 0, st>>>(f->sp, f->wsplit, f->wtsplit, fit_trans_segs(f), s->off, (int)numel,
+                                         (size_t)f->n_small);
     DVT_CUDA_OK(cudaGetLastError());
   }
   return fit_before_caller(f, caller);
@@ -1244,7 +1284,7 @@ int fit_init_params(Fit* f, uint64_t seed, cudaStream_t caller) {
     FIT_RC0(launch(f->sp + l.b->off, (size_t)l.b->rows, l.tid + 1, 0, bound));
   }
   FIT_RC0(launch(f->sp + f->G.off, (size_t)f->hw * f->C, 11, 1, 0.02f, f->C, f->hw));
-  fit_split_kernel<<<256, 256, 0, st>>>(f->sp, f->wsplit, (size_t)f->n_small, (size_t)f->n_small);
+  fit_split_kernel<<<256, 256, 0, st>>>(f->sp, f->wsplit, f->wtsplit, fit_trans_segs(f), 0, f->n_small, (size_t)f->n_small);
   DVT_CUDA_OK(cudaGetLastError());
   return fit_before_caller(f, caller);
 }
@@ -1390,7 +1430,7 @@ int fit_begin(Fit* f, const float* bank, const float* coords, size_t bank_rows, 
   DVT_CUDA_OK(cudaMemsetAsync(f->sm, 0, (size_t)f->n_small * 4, st));
   DVT_CUDA_OK(cudaMemsetAsync(f->sv, 0, (size_t)f->n_small * 4, st));
   DVT_CUDA_OK(cudaMemsetAsync(f->sg, 0, (size_t)f->n_small * 4, st));
-  fit_split_kernel<<<256, 256, 0, st>>>(f->sp, f->wsplit, (size_t)f->n_small, (size_t)f->n_small);
+  fit_split_kernel<<<256, 256, 0, st>>>(f->sp, f->wsplit, f->wtsplit, fit_trans_segs(f), 0, f->n_small, (size_t)f->n_small);
   DVT_CUDA_OK(cudaGetLastError());
   count_launch();
   if (validate) return fit_check(f);
@@ -1428,15 +1468,14 @@ static int fit_linear(Op X, int M, int K, Op W, int N, const float* bias, int ac
   return launch_gemm_tn(X.p, X.ld, W.p, W.ld, TMAP_F32, s, e, st);
 }
 
-// dX = (dY . W) * (H > 0):  dY [M, Nout] K-major A; W stored [Nout, Kin] = MN-major B with N = Kin
-static int fit_dgrad(Op dY, int M, int Nout, Op W, int Kin, const float* Hmask, int ldmask, float* out, int ldo,
+// dX = (dY . W) * (H > 0):  dY [M, Nout] K-major A; Wt = W^T stored [Kin, Nout] (Fit::wtsplit) = K-major B with N = Kin
+static int fit_dgrad(Op dY, int M, int Nout, Op Wt, int Kin, const float* Hmask, int ldmask, float* out, int ldo,
                      size_t out_plane, bool split_out, cudaStream_t st, const GemmOpt& o) {
   GemmEpi e;
   e.mask_f32 = Hmask; e.ldmask = ldmask; e.out = out; e.ldo = ldo; e.out_plane = out_plane;
   e.out_mode = split_out ? OUT_F32_SPLIT : OUT_F32;
-  GemmShape s = fit_gemm_shape(M, Kin, Nout, 1, dY, W, o);
-  s.b_mn = 1;
-  return launch_gemm_tn(dY.p, dY.ld, W.p, W.ld, TMAP_F32, s, e, st);
+  const GemmShape s = fit_gemm_shape(M, Kin, Nout, 1, dY, Wt, o);
+  return launch_gemm_tn(dY.p, dY.ld, Wt.p, Wt.ld, TMAP_F32, s, e, st);
 }
 
 // dW[Nout, Kin] (+ db[Nout]) += dY^T . [X | 1]:  dY stored [n, Nout] (MN-major A), X stored [n, Kin + ones] (MN-major B)
@@ -1537,6 +1576,7 @@ static int fit_enqueue_step(Fit* f, int step_off, bool phase2, bool epoch_end, c
   float* sp = f->sp; float* sg = f->sg;
   const size_t wp = (size_t)f->n_small;  // weight plane stride
   auto W = [&](const Seg& sgm) { return Op{f->wsplit + sgm.off, sgm.cols, wp}; };
+  auto Wt = [&](const Seg& sgm) { return Op{f->wtsplit + sgm.off, sgm.rows, wp}; };
   const size_t p_enc = (size_t)n * f->ld_enc, p_h1 = (size_t)n * f->ld_h1, p_nc = (size_t)n * C, p_nh = (size_t)n * H1;
   const size_t p_raw = (size_t)n * f->ld_raw, p_r = (size_t)n * f->ld_r, p_nr = (size_t)n * Hr;
   const Op enc{f->enc, f->ld_enc, p_enc}, h1{f->h1, f->ld_h1, p_h1}, dpred{f->dpred, C, p_nc}, dh1{f->dh1, H1, p_nh};
@@ -1590,10 +1630,10 @@ static int fit_enqueue_step(Fit* f, int step_off, bool phase2, bool epoch_end, c
     FIT_RC(fork(sE, f->ev[11]));
   }
   FIT_RC(fit_wgrad(dpred, n, C, h1, H1, sg + f->W2.off, sg + f->b2.off, f->wg_sem + 0 * FIT_SEM_TILES, wcap, sB, gopt));   // side B
-  FIT_RC(fit_dgrad(dpred, n, C, W(f->W2), H1, f->h1, f->ld_h1, f->dh1, H1, p_nh, true, st, gopt));  // main
+  FIT_RC(fit_dgrad(dpred, n, C, Wt(f->W2), H1, f->h1, f->ld_h1, f->dh1, H1, p_nh, true, st, gopt));  // main
   FIT_RC(fork(sB, f->ev[4]));  // dh1 ready
   FIT_RC(fit_wgrad(dh1, n, H1, enc, Lf, sg + f->W1.off, sg + f->b1.off, f->wg_sem + 1 * FIT_SEM_TILES, wcap, sB, gopt));  // side B (reads enc)
-  FIT_RC(fit_dgrad(dh1, n, H1, W(f->W1), Lf, nullptr, 0, f->denc, Lf, 0, false, st, gopt));
+  FIT_RC(fit_dgrad(dh1, n, H1, Wt(f->W1), Lf, nullptr, 0, f->denc, Lf, 0, false, st, gopt));
   if (!phase2) {
     // dG (+ grid_sample's neighbour shares) on side C, enqueued BEHIND the two data-gradient GEMMs: launched beside them, its
     // 256 small CTAs take the registers the GEMM CTAs need and delay the critical path.
@@ -1616,9 +1656,9 @@ static int fit_enqueue_step(Fit* f, int step_off, bool phase2, bool epoch_end, c
   if (phase2) {
     // residual MLP backward: the data-gradient chain on side C, the weight-gradient GEMMs that do not feed it on side E
     //   side C: dr2 = dR.R3 -> dr1 = dr2.R2 -> dR1      side E: dR3 (needs dR, r2 only) -> [dr2 ready] dR2
-    FIT_RC(fit_dgrad(dR, n, C, W(f->R3), Hr, f->r2, f->ld_r, f->dr2, Hr, p_nr, true, sC, gopt));
+    FIT_RC(fit_dgrad(dR, n, C, Wt(f->R3), Hr, f->r2, f->ld_r, f->dr2, Hr, p_nr, true, sC, gopt));
     DVT_CUDA_OK(cudaEventRecord(f->ev[12], sC));                                              // dr2 ready
-    FIT_RC(fit_dgrad(dr2, n, Hr, W(f->R2), Hr, f->r1, f->ld_r, f->dr1, Hr, p_nr, true, sC, gopt));
+    FIT_RC(fit_dgrad(dr2, n, Hr, Wt(f->R2), Hr, f->r1, f->ld_r, f->dr1, Hr, p_nr, true, sC, gopt));
     FIT_RC(fit_wgrad(dr1, n, Hr, rawb, C, sg + f->R1.off, sg + f->rb1.off, f->wg_sem + 2 * FIT_SEM_TILES, wcap, sC, gopt));
     FIT_RC(fit_wgrad(dR, n, C, r2, Hr, sg + f->R3.off, sg + f->rb3.off, f->wg_sem + 3 * FIT_SEM_TILES, wcap, sE, gopt));
     DVT_CUDA_OK(cudaStreamWaitEvent(sE, f->ev[12], 0));
@@ -1631,7 +1671,7 @@ static int fit_enqueue_step(Fit* f, int step_off, bool phase2, bool epoch_end, c
   FIT_RC(fork(sB, f->ev[7]));
   const int nv = f->n_small / 4;
   DVT_CUDA_OK(launch_k(pdl, fit_adam_small_kernel, dim3((nv + 255) / 256), dim3(256), 0, sB, (float4*)f->sp, (float4*)f->sm,
-                       (float4*)f->sv, (float4*)f->sg, f->wsplit, nv, f->G.off / 4,
+                       (float4*)f->sv, (float4*)f->sg, f->wsplit, f->wtsplit, fit_trans_segs(f), nv, f->G.off / 4,
                        (f->G.off + r8(f->G.rows * f->G.cols)) / 4, f->R1.off / 4, f->n_small / 4, f->sc_main, f->sc_res,
                        f->step_base, step_off, f->freeze_step, f->wd));
   DVT_CUDA_OK(cudaGetLastError());

@@ -7,9 +7,12 @@
 //   The accumulators are then staged through shared memory (the drained operand ring) and the eight consumer warps run
 //   the fused epilogue on 32 x 32 chunks in a coalesced layout.  Three stages (96 KB) keep two CTAs resident per SM, so
 //   one CTA's epilogue overlaps the other's main loop.
-// 3xTF32 products of the stage-1 fit (gemm_x3_kernel, fp32 hi/lo operand planes): 128 x 64 or 128 x 128 tiles, 8 warps
-//   of mma.sync m16n8k8 TF32 with fragments read from the swizzled TMA tiles -- the fit's backward products read
-//   MN-major fp32 operands, which wgmma's TF32 form does not accept (K-major only).
+// 3xTF32 products of the stage-1 fit (fp32 hi/lo operand planes):
+//   both operands K-major (forward linears, data gradients against the transposed weights): gemm_wgmma_x3_kernel,
+//   128 x 64 tiles of wgmma m64n64k8 TF32, two CTAs per SM
+//   an MN-major operand (weight gradients dY^T [X | 1], which read the activations in place): gemm_x3_kernel, 128 x 64 or
+//   128 x 128 tiles, 8 warps of mma.sync m16n8k8 TF32 with fragments read from the swizzled TMA tiles -- wgmma's TF32
+//   form takes K-major operands only.
 // K tails, M tails and N tails are handled by TMA zero-fill plus masking in the epilogue.
 //
 // Used for: patch-embed, QKV, attention out-proj, MLP fc1/fc2 (reference: timm VisionTransformer reached from
@@ -601,6 +604,131 @@ gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 }
 
 // ----------------------------------------------------------------------------------------------------
+// 3xTF32 on wgmma (gemm_wgmma_x3_kernel): both operands K-major hi / lo planes, 128 x 64 output tiles, 9 warps as in
+// gemm_wgmma_kernel.  Per stage one 3-D TMA box per operand ([plane][rows][32 fp32], 128-byte swizzle: two ordinary
+// K-major wgmma tiles, hi then lo).  Each k8 step issues A_lo.B_hi, A_hi.B_lo, A_hi.B_hi (the order of gemm_x3_kernel)
+// into one fp32 accumulator.  Two stages (96 KB) keep two CTAs on an SM: the fit's GEMMs are 2048 rows by 128-768
+// columns, 48-192 tiles, so one CTA's epilogue and ramp-up overlap the other's main loop.
+// ----------------------------------------------------------------------------------------------------
+constexpr int X3W_BN = 64;
+constexpr int X3W_STAGES = 2;
+constexpr int X3W_A_BYTES = 2 * BM * KB_BYTES;
+constexpr int X3W_STAGE = X3W_A_BYTES + 2 * X3W_BN * KB_BYTES;
+constexpr int X3W_OFF_BAR = X3W_STAGES * X3W_STAGE;
+constexpr int X3W_PITCH = X3W_BN + 8;
+constexpr int X3W_SMEM = X3W_OFF_BAR + 2 * X3W_STAGES * 8 + 1024;
+static_assert(BM * X3W_PITCH * 4 <= X3W_OFF_BAR, "staged accumulators must fit in the operand ring");
+static_assert(2 * (X3W_SMEM + 1024) <= 228 * 1024, "two CTAs per SM");
+
+__global__ void __launch_bounds__(WG_THREADS, 2)
+gemm_wgmma_x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmShape s,
+                     GemmEpi e) {
+  constexpr int BK = KB_BYTES / 4;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + X3W_OFF_BAR);
+  uint64_t* empty = full + X3W_STAGES;
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  gemm_entry_guard(e);
+  const TileIdx ti = tile_of(s, X3W_BN, BK);
+
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    for (int i = 0; i < X3W_STAGES; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], 8);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_wait();
+  pdl_trigger();
+
+  if (warp == 8) {
+    // ===================== TMA producer =====================
+    if (lane == 0) {
+      for (int kb = ti.kb0, it = 0; kb < ti.kb1; ++kb, ++it) {
+        const int st = it % X3W_STAGES;
+        mbar_wait_relaxed(&empty[st], ((it / X3W_STAGES) & 1) ^ 1, 1);
+        uint8_t* sA = smem + st * X3W_STAGE;
+        mbar_expect_tx(&full[st], X3W_STAGE);
+        tma_load_3d(sA, &tmA, &full[st], kb * BK, ti.tm * BM, 0);
+        tma_load_3d(sA + X3W_A_BYTES, &tmB, &full[st], kb * BK, ti.tn * X3W_BN, 0);
+      }
+    }
+    return;
+  }
+
+  // ===================== consumer warpgroups =====================
+  const int wg = warp >> 2;  // rows [64 wg, 64 wg + 64) of the tile
+  float acc[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+  reg_fence(acc);
+  for (int kb = ti.kb0, it = 0; kb < ti.kb1; ++kb, ++it) {
+    const int st = it % X3W_STAGES;
+    mbar_wait(&full[st], (it / X3W_STAGES) & 1, 3);
+    const uint32_t a_hi = smem_u32(smem + st * X3W_STAGE) + wg * 64 * KB_BYTES;
+    const uint32_t a_lo = a_hi + BM * KB_BYTES;
+    const uint32_t b_hi = smem_u32(smem + st * X3W_STAGE) + X3W_A_BYTES;
+    const uint32_t b_lo = b_hi + X3W_BN * KB_BYTES;
+    const uint64_t dah = make_wgmma_desc(a_hi, 0, 1024), dal = make_wgmma_desc(a_lo, 0, 1024);
+    const uint64_t dbh = make_wgmma_desc(b_hi, 0, 1024), dbl = make_wgmma_desc(b_lo, 0, 1024);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const uint64_t adv = (uint64_t)((k * 32) >> 4);  // K advances 32 B (8 fp32) per MMA within the swizzled rows
+      wgmma_64_tf32(acc, dal + adv, dbh + adv);        // small terms first
+      wgmma_64_tf32(acc, dah + adv, dbl + adv);
+      wgmma_64_tf32(acc, dah + adv, dbh + adv);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();  // the MMAs of the previous stage have completed: release its slot
+    reg_fence(acc);
+    if (it > 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[(it - 1) % X3W_STAGES]);
+    }
+  }
+  wgmma_wait<0>();
+  reg_fence(acc);
+
+  // ---- stage the accumulators in the drained operand ring, then the fused epilogue ----
+  named_bar(1, 256);
+  float* tile = reinterpret_cast<float*>(smem);
+  {
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int c0 = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      *reinterpret_cast<float2*>(tile + r0 * X3W_PITCH + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(tile + (r0 + 8) * X3W_PITCH + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    }
+  }
+  named_bar(1, 256);
+  // split-K with counters, as in gemm_x3_kernel: the splits of a tile add in split order
+  const bool serial = e.splitk_sem != nullptr && s.splits > 1;
+  unsigned* sem = e.splitk_sem + blockIdx.x / s.splits;
+  const unsigned split = blockIdx.x % s.splits;
+  if (serial) {
+    if (threadIdx.x == 0) {
+      const long long t0 = clock64();
+      while (ld_acquire_u32(sem) != split)
+        if (clock64() - t0 > DVT_WATCHDOG_CYCLES) dev_fail(0x5E3u, split);
+    }
+    named_bar(1, 256);
+  }
+  epi_tile<true, X3W_BN>(e, s, tile, X3W_PITCH, warp, 8, lane, ti.tm, ti.tn, ti.kb0 < ti.kb_total);
+  if (serial) {
+    __threadfence();
+    named_bar(1, 256);
+    if (threadIdx.x == 0) st_release_u32(sem, split + 1 == (unsigned)s.splits ? 0u : split + 1);
+  }
+}
+
+// ----------------------------------------------------------------------------------------------------
 // SIMT debug GEMM (fp32 FMA, 16x16 tiles).  Same epilogue semantics; selected with DVT_GEMM_IMPL=simt or
 // dvt_set_debug_impl(1).  It exists so that a broken tensor-core path can be told apart from a broken caller in
 // one GPU session; it is never the default.
@@ -718,17 +846,16 @@ int gemm_prepare() {
   if ((rc = set_smem(gemm_wgmma_kernel<false, true, true>, WG_SMEM))) return rc;
   if ((rc = set_smem(gemm_wgmma_swiglu_bwd_kernel, WG_SMEM))) return rc;
   if ((rc = set_smem(gemm_wgmma_planes_kernel, WG_SMEM))) return rc;
-  if ((rc = set_smem(gemm_x3_kernel<64, false, false>, X3Smem<64>::TOTAL))) return rc;
+  if ((rc = set_smem(gemm_wgmma_x3_kernel, X3W_SMEM))) return rc;
   if ((rc = set_smem(gemm_x3_kernel<64, false, true>, X3Smem<64>::TOTAL))) return rc;
   if ((rc = set_smem(gemm_x3_kernel<64, true, true>, X3Smem<64>::TOTAL))) return rc;
-  if ((rc = set_smem(gemm_x3_kernel<128, false, false>, X3Smem<128>::TOTAL))) return rc;
   if ((rc = set_smem(gemm_x3_kernel<128, false, true>, X3Smem<128>::TOTAL))) return rc;
   if ((rc = set_smem(gemm_x3_kernel<128, true, true>, X3Smem<128>::TOTAL))) return rc;
   done = true;
   return DVT_OK;
 }
 
-// Tile width of the 3xTF32 kernels: 128 x 128 halves the operand traffic per flop, 128 x 64 gives twice the CTAs and the
+// Tile width of the mma.sync 3xTF32 kernels (an MN-major operand): 128 x 128 halves the operand traffic per flop, 128 x 64 gives twice the CTAs and the
 // shorter epilogue.  The caller chooses per call (GemmShape::x3_wide_min_n; 0 = always 128 x 64).
 int gemm_x3_tile_n(int N, int wide_min_n) { return (wide_min_n > 0 && N >= wide_min_n) ? 128 : 64; }
 
@@ -807,21 +934,29 @@ int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dty
   if (s.x3) {
     CUtensorMap tA, tB;
     int rc3;
-    const int bn3 = gemm_x3_tile_n(s.N, s.x3_wide_min_n);
+    // both operands K-major: wgmma (gemm_wgmma_x3_kernel); an MN-major operand: mma.sync (gemm_x3_kernel)
+    const bool kk = !s.a_mn && !s.b_mn;
+    const int bn3 = kk ? X3W_BN : gemm_x3_tile_n(s.N, s.x3_wide_min_n);
     if (s.a_mn) rc3 = make_tmap_3d(&tA, A, TMAP_F32, (uint64_t)s.M, (uint64_t)s.K, 2, (uint64_t)lda * 4, s.plane_a * 4, 32, 32, 2);
     else rc3 = make_tmap_3d(&tA, A, TMAP_F32, (uint64_t)s.K, (uint64_t)s.M, 2, (uint64_t)lda * 4, s.plane_a * 4, 32, BM, 2);
     if (rc3) return rc3;
     if (s.b_mn) rc3 = make_tmap_3d(&tB, B, TMAP_F32, (uint64_t)s.N, (uint64_t)s.K, 2, (uint64_t)ldb * 4, s.plane_b * 4, 32, 32, 2);
     else rc3 = make_tmap_3d(&tB, B, TMAP_F32, (uint64_t)s.K, (uint64_t)s.N, 2, (uint64_t)ldb * 4, s.plane_b * 4, 32, bn3, 2);
     if (rc3) return rc3;
+    if (kk) {
+      const int tiles = ((s.M + BM - 1) / BM) * ((s.N + X3W_BN - 1) / X3W_BN) * s.splits;
+      DVT_CUDA_OK(launch_k(s.pdl != 0, gemm_wgmma_x3_kernel, dim3(tiles), dim3(WG_THREADS), (size_t)X3W_SMEM, stream, tA, tB,
+                           s, epi));
+      count_launch();
+      DVT_CUDA_OK(cudaGetLastError());
+      return DVT_OK;
+    }
     if (bn3 == 128) {
       if (s.a_mn) return launch_x3<128, true, true>(tA, tB, s, epi, stream);
-      if (s.b_mn) return launch_x3<128, false, true>(tA, tB, s, epi, stream);
-      return launch_x3<128, false, false>(tA, tB, s, epi, stream);
+      return launch_x3<128, false, true>(tA, tB, s, epi, stream);
     }
     if (s.a_mn) return launch_x3<64, true, true>(tA, tB, s, epi, stream);
-    if (s.b_mn) return launch_x3<64, false, true>(tA, tB, s, epi, stream);
-    return launch_x3<64, false, false>(tA, tB, s, epi, stream);
+    return launch_x3<64, false, true>(tA, tB, s, epi, stream);
   }
   CUtensorMap tmA, tmB;
   int rc;

@@ -62,7 +62,7 @@ struct GemmShape {
   int x3 = 0;    // 1: 3xTF32 as described
   size_t plane_a = 0, plane_b = 0;
   int pdl = 0;   // launch with programmatic stream serialisation (the kernel calls pdl_wait() after its set-up)
-  int x3_wide_min_n = 0;  // x3: 128 x 128 tiles when N >= this (0: always 128 x 64)
+  int x3_wide_min_n = 0;  // x3 with an MN-major operand (mma.sync kernel): 128 x 128 tiles when N >= this (0: always 128 x 64)
 };
 
 // FIT = true (the 3xTF32 kernels of the stage-1 fit): epilogue features only other callers use -- GELU, the bf16 mask with

@@ -14,8 +14,9 @@
 //           (3 GEMM) / backward (5 GEMM), weight-gradient GEMMs, Adam(small params), and the dense Adam sweep of the
 //           hash table (one pass per window of k steps, software-pipelined one to two windows deep)
 // All GEMMs run on the tensor cores (gemm.cu) as 3xTF32 products of fp32 hi/lo planes (fp32-accurate: bf16 operands cannot
-// hold the cosine >= 0.999 parity bar, see DESIGN.md); weight-gradient GEMMs read the activations as MN-major
-// operands, so no transposed copies exist; bias gradients come from a ones column appended to the activation buffers.
+// hold the cosine >= 0.999 parity bar, see DESIGN.md), all with both operands K-major (wgmma's TF32 form takes no other):
+// the weight-gradient GEMMs dY^T [X | 1] read transposed copies of dY and X that their producers write beside the
+// row-major planes (Fit::enc_t ...), and the bias gradients come from a ones row at the end of each transposed activation.
 //
 // HBM layout: table p/m/v as two ping-pong copies of three fp32 arrays of n_entries*8, gradients as a ring of 2k
 // such arrays with per-entry step stamps; "small" params (field MLP, G as [h*w, C],
@@ -158,12 +159,13 @@ __device__ __forceinline__ void adam8(float4& pa, float4& pb, float4& ma, float4
 // shuffles.  npeek = number of Adam steps (0 .. MAXPEEK) that are still pending in the sweeps and are applied on the fly:
 // the encoded step is s, the state that is read is S_{s - npeek}, in state buffer (step_base[1] + buf_off) & 1.  All
 // stamp and gradient loads are issued before the first adam8 (the encode is on the critical path).
-// table_fixed != nullptr: read that table (query mode).
+// table_fixed != nullptr: read that table (query mode).  enc_t != nullptr: also the transposed planes [Lf + 1][n] (pitch n,
+// lo plane at plane_t), the K-major operand of the W1 weight gradient; the 8 samples of a warp store a 32-byte sector.
 template <int MAXPEEK>
 __global__ void __launch_bounds__(256)
 fit_encode_kernel(GridLevels g, TableBufs tb, const float* __restrict__ table_fixed, const float* __restrict__ coords,
-                  StepRows sr, int n, float* __restrict__ enc, int ld_enc, size_t plane,
-                  const AdamScalars* __restrict__ sc, float wd, int npeek, int buf_off) {
+                  StepRows sr, int n, float* __restrict__ enc, int ld_enc, size_t plane, float* __restrict__ enc_t,
+                  size_t plane_t, const AdamScalars* __restrict__ sc, float wd, int npeek, int buf_off) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   const int k = t & 3;
   // Threads past the end stay in the kernel (clamped to the last element, store predicated off): the shuffles below name
@@ -230,6 +232,11 @@ fit_encode_kernel(GridLevels g, TableBufs tb, const float* __restrict__ table_fi
   }
   float* dst = enc + (size_t)i * ld_enc + l * FIT_F + (k & 1) * 4 + ((k & 2) ? plane : 0);
   if (live) *reinterpret_cast<float4*>(dst) = make_float4(o[0], o[1], o[2], o[3]);
+  if (live && enc_t) {
+    float* dt = enc_t + (size_t)(l * FIT_F + (k & 1) * 4) * n + i + ((k & 2) ? plane_t : 0);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) dt[(size_t)j * n] = o[j];
+  }
 }
 
 // fp32 encode (unit-test entry point: bit-level check of indices / weights against the oracle)
@@ -359,20 +366,49 @@ fit_grid_bwd_kernel(GridLevels g, const float* __restrict__ coords, StepRows sr,
   }
 }
 
-// gather bank rows (fp32) -> hi/lo planes [n, ld] (input of the residual MLP)
-__global__ void fit_gather_rows_kernel(const float* __restrict__ bank, int C, StepRows sr, int n,
-                                       float* __restrict__ out, int ld, size_t plane) {
+// Rows per CTA of the kernels that also store their [n, C] output transposed ([C][n]): the 8 values of a column are one
+// 32-byte sector.  The rows are staged in shared memory, [FIT_T_ROWS][C + 4] (the padding spreads a column over 32 banks).
+constexpr int FIT_T_ROWS = 8;
+__host__ __device__ constexpr int fit_t_stage_bytes(int C) { return FIT_T_ROWS * (C + 4) * 4; }
+
+// The staged rows i0 .. i0 + rows - 1 stored transposed as TF32 hi / lo planes: out_t[c * n + i] (lo plane at plane_t).
+__device__ __forceinline__ void fit_store_rows_t(const float* stage, int C, int i0, int rows, int n, float* __restrict__ out_t,
+                                                 size_t plane_t) {
+  for (int e = threadIdx.x; e < C * FIT_T_ROWS; e += blockDim.x) {
+    const int c = e / FIT_T_ROWS, r = e % FIT_T_ROWS;
+    if (r >= rows) continue;
+    const float v = stage[r * (C + 4) + c], hi = tf32_hi(v);
+    float* o = out_t + (size_t)c * n + i0 + r;
+    o[0] = hi;
+    o[plane_t] = v - hi;
+  }
+}
+
+// gather bank rows (fp32) -> hi/lo planes [n, ld] (input of the residual MLP), FIT_T_ROWS rows per CTA; out_t != nullptr:
+// also the transposed planes (operand of the R1 weight gradient), staged in fit_t_stage_bytes(C) of dynamic shared memory.
+__global__ void __launch_bounds__(256)
+fit_gather_rows_kernel(const float* __restrict__ bank, int C, StepRows sr, int n, float* __restrict__ out, int ld,
+                       size_t plane, float* __restrict__ out_t, size_t plane_t) {
+  extern __shared__ float stage[];
   pdl_wait();     // (no-ops unless launched with programmatic stream serialisation)
   pdl_trigger();
-  const int i = blockIdx.x;
+  const int i0 = blockIdx.x * FIT_T_ROWS, rows_here = min(FIT_T_ROWS, n - i0);
   const int* rows = sr.rows(n);
-  const float4* src = reinterpret_cast<const float4*>(sr.bank(bank) + (size_t)(rows ? rows[i] : i) * C);
-  for (int c4 = threadIdx.x; c4 < C / 4; c4 += blockDim.x) {
-    const float4 v = __ldg(src + c4);
+  const float* b = sr.bank(bank);
+  const int c4n = C / 4;
+#pragma unroll 2
+  for (int e = threadIdx.x; e < rows_here * c4n; e += blockDim.x) {
+    const int r = e / c4n, c4 = e - r * c4n, i = i0 + r;
+    const float4 v = __ldg(reinterpret_cast<const float4*>(b + (size_t)(rows ? rows[i] : i) * C) + c4);
     const float4 hi = make_float4(tf32_hi(v.x), tf32_hi(v.y), tf32_hi(v.z), tf32_hi(v.w));
     float* dst = out + (size_t)i * ld + c4 * 4;
     *reinterpret_cast<float4*>(dst) = hi;
     *reinterpret_cast<float4*>(dst + plane) = make_float4(v.x - hi.x, v.y - hi.y, v.z - hi.z, v.w - hi.w);
+    if (out_t) *reinterpret_cast<float4*>(stage + r * (C + 4) + c4 * 4) = v;
+  }
+  if (out_t) {
+    __syncthreads();
+    fit_store_rows_t(stage, C, i0, rows_here, n, out_t, plane_t);
   }
 }
 
@@ -392,6 +428,9 @@ struct LossArgs {
   float* dpred;             // [2 planes][n, C] (hi / lo)
   float* dR;                // [2 planes][n, C] or nullptr
   size_t plane;             // n * C
+  float* dpred_t;           // [2 planes][C, n]: the same values transposed (K-major operand of the weight gradients)
+  float* dR_t;              // [2 planes][C, n] or nullptr
+  size_t plane_t;           // C * n
   float* gG;                // [hw, C] gradient accumulator or nullptr (G frozen)
   float* losses;            // [num_iters, 5]; this step's slots are used
   int n, C, hw;
@@ -407,9 +446,11 @@ struct LossArgs {
   int gw, gh;
 };
 
-// NV = float4 per lane (ceil(C / 128)); all global loads of a row are issued before the first use.
+// NV = float4 per lane (ceil(C / 128)); all global loads of a row are issued before the first use.  d pred (and d R) of
+// the CTA's 8 rows are staged in dynamic shared memory (fit_t_stage_bytes(C) each) for the transposed stores.
 template <int NV, bool HAS_R>
 __global__ void __launch_bounds__(256, 2) fit_loss_kernel(LossArgs a) {
+  extern __shared__ float stage[];  // [FIT_T_ROWS][C + 4] d pred, then (HAS_R) the same for d R
   pdl_wait();     // (no-ops unless launched with programmatic stream serialisation)
   pdl_trigger();
   const int row_raw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -486,6 +527,7 @@ __global__ void __launch_bounds__(256, 2) fit_loss_kernel(LossArgs a) {
   const float k_cr = -inv_n * a.loss_scale / (np_ * nr_);        // coefficient of raw
   const float k_cp = inv_n * a.loss_scale * cosv / (np_ * np_);  // coefficient of pred
   float res_sq = 0.f, res_abs = 0.f;
+  float* st_row = stage + (threadIdx.x >> 5) * (C + 4);  // this warp's row of the staging
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const int v = lane + 32 * i;
@@ -501,6 +543,7 @@ __global__ void __launch_bounds__(256, 2) fit_loss_kernel(LossArgs a) {
       float* dp = a.dpred + (size_t)row * C + v * 4;
       *reinterpret_cast<float4*>(dp) = hi;
       *reinterpret_cast<float4*>(dp + a.plane) = make_float4(d.x - hi.x, d.y - hi.y, d.z - hi.z, d.w - hi.w);
+      *reinterpret_cast<float4*>(st_row + v * 4) = d;
     }
     if (HAS_R) {
       // gt_residual = raw - denoised - shared = raw - (pred - R); e = R - gt = pred - raw
@@ -516,6 +559,7 @@ __global__ void __launch_bounds__(256, 2) fit_loss_kernel(LossArgs a) {
       float* dp = a.dR + (size_t)row * C + v * 4;
       *reinterpret_cast<float4*>(dp) = hi;
       *reinterpret_cast<float4*>(dp + a.plane) = make_float4(dr.x - hi.x, dr.y - hi.y, dr.z - hi.z, dr.w - hi.w);
+      *reinterpret_cast<float4*>(st_row + FIT_T_ROWS * (C + 4) + v * 4) = dr;
     }
   }
   if (HAS_R) {
@@ -536,14 +580,17 @@ __global__ void __launch_bounds__(256, 2) fit_loss_kernel(LossArgs a) {
     s_part[wib][4] = ls;
   }
   __syncthreads();
+  const int nw = min(8, a.n - (int)(blockIdx.x * (blockDim.x >> 5)));  // warps of this CTA that own a row
   if (threadIdx.x < 5 && (HAS_R || threadIdx.x < 3)) {
     float t = 0.f;
-    const int nw = min(8, a.n - (int)(blockIdx.x * (blockDim.x >> 5)));  // warps of this CTA that own a row
 #pragma unroll
     for (int k = 0; k < 8; ++k)
       if (k < nw) t += s_part[k][threadIdx.x];
     atomicAdd(losses + threadIdx.x, t);
   }
+  const int i0 = blockIdx.x * (blockDim.x >> 5);
+  fit_store_rows_t(stage, C, i0, nw, a.n, a.dpred_t, a.plane_t);
+  if (HAS_R) fit_store_rows_t(stage + FIT_T_ROWS * (C + 4), C, i0, nw, a.n, a.dR_t, a.plane_t);
 }
 
 // dG of phase 1, off the critical path: the loss kernel stores d pred (hi / lo planes); this kernel, on a side stream,
@@ -624,19 +671,20 @@ template <bool HAS_R>
 static int launch_loss_nv(const LossArgs& la, int blocks, int tb, cudaStream_t st, bool pdl) {
   const int nv = (la.C / 4 + 31) / 32;
   const dim3 g(blocks), b(tb);
-  if (nv <= 1) DVT_CUDA_OK(launch_k(pdl, fit_loss_kernel<1, HAS_R>, g, b, 0, st, la));
-  else if (nv <= 2) DVT_CUDA_OK(launch_k(pdl, fit_loss_kernel<2, HAS_R>, g, b, 0, st, la));
-  else if (nv <= 3) DVT_CUDA_OK(launch_k(pdl, fit_loss_kernel<3, HAS_R>, g, b, 0, st, la));
-  else if (nv <= 6) DVT_CUDA_OK(launch_k(pdl, fit_loss_kernel<6, HAS_R>, g, b, 0, st, la));
-  else if (nv <= 8) DVT_CUDA_OK(launch_k(pdl, fit_loss_kernel<8, HAS_R>, g, b, 0, st, la));
-  else DVT_CUDA_OK(launch_k(pdl, fit_loss_kernel<12, HAS_R>, g, b, 0, st, la));
+  const size_t sm = (HAS_R ? 2 : 1) * (size_t)fit_t_stage_bytes(la.C);
+  if (nv <= 1) DVT_CUDA_OK(launch_k(pdl, fit_loss_kernel<1, HAS_R>, g, b, sm, st, la));
+  else if (nv <= 2) DVT_CUDA_OK(launch_k(pdl, fit_loss_kernel<2, HAS_R>, g, b, sm, st, la));
+  else if (nv <= 3) DVT_CUDA_OK(launch_k(pdl, fit_loss_kernel<3, HAS_R>, g, b, sm, st, la));
+  else if (nv <= 6) DVT_CUDA_OK(launch_k(pdl, fit_loss_kernel<6, HAS_R>, g, b, sm, st, la));
+  else if (nv <= 8) DVT_CUDA_OK(launch_k(pdl, fit_loss_kernel<8, HAS_R>, g, b, sm, st, la));
+  else DVT_CUDA_OK(launch_k(pdl, fit_loss_kernel<12, HAS_R>, g, b, sm, st, la));
   DVT_CUDA_OK(cudaGetLastError());
   count_launch();
   return DVT_OK;
 }
 
 static int launch_loss(const LossArgs& la, cudaStream_t st, bool pdl) {
-  const int tb = 256, blocks = (la.n * 32 + tb - 1) / tb;
+  const int tb = 256, blocks = (la.n * 32 + tb - 1) / tb;  // (8 warps = FIT_T_ROWS rows per CTA)
   return la.R ? launch_loss_nv<true>(la, blocks, tb, st, pdl) : launch_loss_nv<false>(la, blocks, tb, st, pdl);
 }
 
@@ -802,9 +850,9 @@ __global__ void fit_advance_kernel(int* step_base, int steps, int sweeps) {
   step_base[1] += sweeps;
 }
 
-__global__ void fit_fill_col_kernel(float* buf, int ld, int col, int rows, float val) {
+__global__ void fit_fill_kernel(float* buf, int n, float val) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < rows) buf[(size_t)i * ld + col] = val;
+  if (i < n) buf[i] = val;
 }
 
 __global__ void fit_transpose_kernel(const float* __restrict__ in, float* __restrict__ out, int rows, int cols) {
@@ -865,7 +913,6 @@ struct Fit {
   bool epoch_forked = false;                   // this epoch forked sweeps onto sD (pipelined schedule)
   int sweep_steps[2] = {4, 4};                 // DVT_FIT_SWEEP_STEPS "k1,k2": window of the pipelined sweep per phase
   bool enc_ready = false;                      // f->enc already holds the encoding of the next step
-  int x3_wide_min_n[2] = {0, 256};             // DVT_FIT_X3_WIDE_MIN_N "p1,p2": 128 x 128 weight-gradient tiles when N >= this (0: never)
   int wgrad_sms = 96;                          // DVT_FIT_WGRAD_SMS: weight-gradient GEMMs split K to fill at most this many SMs
   bool pdl = true;                             // DVT_FIT_PDL: programmatic dependent launch along the kernel chains of a step
   bool pipe[2] = {true, true};                 // software-pipelined table sweep in phase 1 / 2 (see fit_enqueue_step)
@@ -879,6 +926,11 @@ struct Fit {
   float *rawb = nullptr, *r1 = nullptr, *r2 = nullptr, *dR = nullptr, *dr2 = nullptr, *dr1 = nullptr;
   float* Rout = nullptr;
   int ld_enc, ld_h1, ld_raw, ld_r;
+  // The same hi / lo values transposed, [rows][bsz] per plane: the K-major operands of the weight gradients dY^T [X | 1]
+  // (wgmma's TF32 form reads K-major operands only), written by the producers of the row-major planes.  The last row of an
+  // activation is the ones row (hi 1, lo 0; written by fit_create) that yields the bias gradient.
+  float *enc_t = nullptr, *h1_t = nullptr, *rawb_t = nullptr, *r1_t = nullptr, *r2_t = nullptr;  // [Kin + 1] rows
+  float *dpred_t = nullptr, *dR_t = nullptr, *dh1_t = nullptr, *dr2_t = nullptr, *dr1_t = nullptr;  // [Nout] rows
   // schedule
   int num_iters = 0, freeze_step = 0;
   int cur_step = 0;                            // steps of the current schedule already enqueued (host mirror of step_base[0])
@@ -932,11 +984,25 @@ static TransSegs fit_trans_segs(const Fit* f) {
   return t;
 }
 
+template <bool HAS_R>
+static int fit_loss_smem(int bytes) {
+  for (const void* k : {(const void*)fit_loss_kernel<1, HAS_R>, (const void*)fit_loss_kernel<2, HAS_R>,
+                        (const void*)fit_loss_kernel<3, HAS_R>, (const void*)fit_loss_kernel<6, HAS_R>,
+                        (const void*)fit_loss_kernel<8, HAS_R>, (const void*)fit_loss_kernel<12, HAS_R>})
+    DVT_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+  return DVT_OK;
+}
+
 static int fit_prepare_kernels() {
   static bool done = false;
   if (done) return DVT_OK;
   done = true;
   DVT_CUDA_OK(cudaFuncSetAttribute(fit_grid_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GB_SMEM));
+  // staging of the transposed stores, sized for the largest C (fit_create)
+  const int st = fit_t_stage_bytes(1536);
+  DVT_CUDA_OK(cudaFuncSetAttribute(fit_gather_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, st));
+  FIT_RC0(fit_loss_smem<false>(st));
+  FIT_RC0(fit_loss_smem<true>(2 * st));
   return DVT_OK;
 }
 
@@ -959,7 +1025,6 @@ static int r8(int x) { return (x + 7) / 8 * 8; }
 //   DVT_FIT_PDL=0                 plain stream-ordered launches (no programmatic dependent launch)
 //   DVT_FIT_WGRAD_SMS=n           split-K of the weight-gradient GEMMs fills at most n SMs (they share the GPU with the
 //                                 data-gradient GEMMs of the critical path)
-//   DVT_FIT_X3_WIDE_MIN_N="a[,b]" per phase: weight-gradient GEMMs with N >= this use 128 x 128 tiles (0: always 128 x 64)
 // (DVT_FIT_DEBUG_GRAPH=1 is read by fit_capture: it prints what each capture recorded.)
 static int fit_read_schedule_env(Fit* f) {
   int win[2] = {f->sweep_steps[0], f->sweep_steps[1]};
@@ -987,12 +1052,6 @@ static int fit_read_schedule_env(Fit* f) {
   const char* pd = getenv("DVT_FIT_PDL");
   f->pdl = !(pd && pd[0] == '0');
   if (const char* ws = getenv("DVT_FIT_WGRAD_SMS")) f->wgrad_sms = std::max(1, atoi(ws));
-  if (const char* wm = getenv("DVT_FIT_X3_WIDE_MIN_N")) {
-    int a = 0, b = 0;
-    const int got = sscanf(wm, "%d,%d", &a, &b);
-    if (got >= 1) f->x3_wide_min_n[0] = f->x3_wide_min_n[1] = std::max(0, a);
-    if (got == 2) f->x3_wide_min_n[1] = std::max(0, b);
-  }
   return DVT_OK;
 }
 
@@ -1039,7 +1098,7 @@ int fit_create(Fit** out, int C, int gh, int gw, int bsz, int n_levels, const fl
   seg(f->G, f->hw, C);
   seg(f->R1, Hr, C); seg(f->rb1, Hr, 1); seg(f->R2, Hr, Hr); seg(f->rb2, Hr, 1); seg(f->R3, C, Hr); seg(f->rb3, C, 1);
   f->n_small = off;
-  f->ld_enc = f->Lf + 8; f->ld_h1 = H1 + 8; f->ld_raw = C + 8; f->ld_r = Hr + 8;
+  f->ld_enc = f->Lf; f->ld_h1 = H1; f->ld_raw = C; f->ld_r = Hr;
   int rc = 0;
   auto A = [&](void** p, size_t bytes) { if (!rc) rc = fit_alloc(f, p, bytes); };
   for (int q = 0; q < 2; ++q) {
@@ -1062,18 +1121,23 @@ int fit_create(Fit** out, int C, int gh, int gw, int bsz, int n_levels, const fl
   A((void**)&f->rawb, n * f->ld_raw * 8); A((void**)&f->r1, n * f->ld_r * 8); A((void**)&f->r2, n * f->ld_r * 8);
   A((void**)&f->dR, n * C * 8); A((void**)&f->dr2, n * Hr * 8); A((void**)&f->dr1, n * Hr * 8);
   A((void**)&f->Rout, n * C * 4); A((void**)&f->step_base, 2 * sizeof(int));
+  A((void**)&f->enc_t, (f->Lf + 1) * n * 8); A((void**)&f->h1_t, (H1 + 1) * n * 8); A((void**)&f->rawb_t, (C + 1) * n * 8);
+  A((void**)&f->r1_t, (Hr + 1) * n * 8); A((void**)&f->r2_t, (Hr + 1) * n * 8);
+  A((void**)&f->dpred_t, C * n * 8); A((void**)&f->dR_t, C * n * 8); A((void**)&f->dh1_t, H1 * n * 8);
+  A((void**)&f->dr2_t, Hr * n * 8); A((void**)&f->dr1_t, Hr * n * 8);
   A((void**)&f->inputs_dev, sizeof(FitInputs));
   A((void**)&f->flags_dev, sizeof(int));
   A((void**)&f->wg_sem, 5 * FIT_SEM_TILES * sizeof(unsigned));
   if (!rc && cudaHostAlloc((void**)&f->flags_pinned, sizeof(int), cudaHostAllocDefault) != cudaSuccess) rc = DVT_ERR_CUDA;
   if (rc) { for (void* p : f->owned) cudaFree(p); delete f; return rc; }
-  // ones columns (bias gradients through the weight-gradient GEMMs)
+  // ones rows of the transposed activations (bias gradients through the weight-gradient GEMMs; the lo planes stay 0)
   const int tb = 256, nb = (bsz + tb - 1) / tb;
-  fit_fill_col_kernel<<<nb, tb>>>(f->enc, f->ld_enc, f->Lf, bsz, 1.f);
-  fit_fill_col_kernel<<<nb, tb>>>(f->h1, f->ld_h1, H1, bsz, 1.f);
-  fit_fill_col_kernel<<<nb, tb>>>(f->rawb, f->ld_raw, C, bsz, 1.f);
-  fit_fill_col_kernel<<<nb, tb>>>(f->r1, f->ld_r, Hr, bsz, 1.f);
-  fit_fill_col_kernel<<<nb, tb>>>(f->r2, f->ld_r, Hr, bsz, 1.f);
+  fit_fill_kernel<<<nb, tb>>>(f->enc_t + n * f->Lf, bsz, 1.f);
+  fit_fill_kernel<<<nb, tb>>>(f->h1_t + n * H1, bsz, 1.f);
+  fit_fill_kernel<<<nb, tb>>>(f->rawb_t + n * C, bsz, 1.f);
+  fit_fill_kernel<<<nb, tb>>>(f->r1_t + n * Hr, bsz, 1.f);
+  fit_fill_kernel<<<nb, tb>>>(f->r2_t + n * Hr, bsz, 1.f);
+  DVT_CUDA_OK(cudaGetLastError());
   DVT_CUDA_OK(cudaDeviceSynchronize());
   *out = f;
   return DVT_OK;
@@ -1449,51 +1513,57 @@ struct Op {
 // What all GEMMs of one step (or one query) share.
 struct GemmOpt {
   bool pdl;  // programmatic dependent launch
-  int wide;  // 128 x 128 tiles when N >= this (GemmShape::x3_wide_min_n)
 };
 
 static GemmShape fit_gemm_shape(int M, int N, int K, int splits, Op A, Op B, const GemmOpt& o) {
   GemmShape s{M, N, K, splits};
-  s.x3 = 1; s.plane_a = A.plane; s.plane_b = B.plane; s.pdl = o.pdl; s.x3_wide_min_n = o.wide;
+  s.x3 = 1; s.plane_a = A.plane; s.plane_b = B.plane; s.pdl = o.pdl;
   return s;
 }
 
-// Y = act(X W^T + b):  X [M, K] planes, W [N, K] planes.  split_out: Y is written as hi/lo planes (feeds a GEMM).
+// Y = act(X W^T + b):  X [M, K] planes, W [N, K] planes.  split_out: Y is written as hi/lo planes (feeds a GEMM), and
+// transposed into out_t ([N][M] planes, lo plane at plane_t) unless it is null.
 static int fit_linear(Op X, int M, int K, Op W, int N, const float* bias, int act, float* out, int ldo, size_t out_plane,
-                      bool split_out, cudaStream_t st, const GemmOpt& o) {
+                      bool split_out, float* out_t, size_t plane_t, cudaStream_t st, const GemmOpt& o) {
   GemmEpi e;
   e.bias = bias; e.act = act; e.out = out; e.ldo = ldo; e.out_plane = out_plane;
   e.out_mode = split_out ? OUT_F32_SPLIT : OUT_F32;
+  e.out_t = out_t; e.ldt = M; e.plane_t = plane_t;
   const GemmShape s = fit_gemm_shape(M, N, K, 1, X, W, o);
   return launch_gemm_tn(X.p, X.ld, W.p, W.ld, TMAP_F32, s, e, st);
 }
 
-// dX = (dY . W) * (H > 0):  dY [M, Nout] K-major A; Wt = W^T stored [Kin, Nout] (Fit::wtsplit) = K-major B with N = Kin
+// dX = (dY . W) * (H > 0):  dY [M, Nout] K-major A; Wt = W^T stored [Kin, Nout] (Fit::wtsplit) = K-major B with N = Kin.
+// out_t as in fit_linear.
 static int fit_dgrad(Op dY, int M, int Nout, Op Wt, int Kin, const float* Hmask, int ldmask, float* out, int ldo,
-                     size_t out_plane, bool split_out, cudaStream_t st, const GemmOpt& o) {
+                     size_t out_plane, bool split_out, float* out_t, size_t plane_t, cudaStream_t st, const GemmOpt& o) {
   GemmEpi e;
   e.mask_f32 = Hmask; e.ldmask = ldmask; e.out = out; e.ldo = ldo; e.out_plane = out_plane;
   e.out_mode = split_out ? OUT_F32_SPLIT : OUT_F32;
+  e.out_t = out_t; e.ldt = M; e.plane_t = plane_t;
   const GemmShape s = fit_gemm_shape(M, Kin, Nout, 1, dY, Wt, o);
   return launch_gemm_tn(dY.p, dY.ld, Wt.p, Wt.ld, TMAP_F32, s, e, st);
 }
 
-// dW[Nout, Kin] (+ db[Nout]) += dY^T . [X | 1]:  dY stored [n, Nout] (MN-major A), X stored [n, Kin + ones] (MN-major B)
+// dW[Nout, Kin] (+ db[Nout]) += dY^T . [X | 1]:  dYt = dY^T stored [Nout, n] (K-major A), Xt = [X | 1]^T stored
+// [Kin + 1, n] with the ones row last (K-major B): the transposed planes of Fit.
 // sem: FIT_SEM_TILES zeroed per-tile counters of this call site: the splits of a tile add their partial sums in split
 // order, so the gradient does not depend on which split finishes first.  sm_cap: see Fit::wgrad_sms.
-static int fit_wgrad(Op dY, int n, int Nout, Op X, int Kin, float* gW, float* gb, unsigned* sem, int sm_cap, cudaStream_t st,
-                     const GemmOpt& o) {
+static int fit_wgrad(Op dYt, int n, int Nout, Op Xt, int Kin, float* gW, float* gb, unsigned* sem, int sm_cap, bool phase2,
+                     cudaStream_t st, const GemmOpt& o) {
   GemmEpi e;
   e.out = gW; e.ldo = Kin; e.out_mode = OUT_F32_ATOMIC; e.last_col_out = gb; e.splitk_sem = sem;
-  // split-K so that (output tiles x splits) fills the SMs once: tiles are 128 x 64 or 128 x 128, k-blocks 32 samples
-  const int kb = (n + 31) / 32;
-  const int bn = gemm_x3_tile_n(Kin + 1, o.wide);
-  const int tiles = ((Nout + 127) / 128) * ((Kin + bn) / bn);
+  const int kb = (n + 31) / 32;  // k-blocks of 32 samples
+  const int tiles = ((Nout + 127) / 128) * ((Kin + 64) / 64);  // 128 x 64 output tiles
   DVT_REQUIRE(tiles <= FIT_SEM_TILES, "fit: %d weight-gradient tiles exceed the split-K counters", tiles);
-  const int splits = std::max(1, std::min(std::min(num_sms(), sm_cap) / std::max(tiles, 1), kb / 4));
-  GemmShape s = fit_gemm_shape(Nout, Kin + 1, n, splits, dY, X, o);
-  s.a_mn = 1; s.b_mn = 1;
-  return launch_gemm_tn(dY.p, dY.ld, X.p, X.ld, TMAP_F32, s, e, st);
+  // Split-K so that (output tiles x splits) fills at most sm_cap SMs.  In phase 2 the products with N >= 256 (W2, R1)
+  // count their tiles 128 columns wide: that is the partition of the fit's reference trajectory.  The split partition
+  // fixes the order of every sum, and any other one changes the gradients at rounding level, which 1000 Adam steps
+  // amplify into a visibly different fit.
+  const int split_tiles = (phase2 && Kin + 1 >= 256) ? ((Nout + 127) / 128) * ((Kin + 128) / 128) : tiles;
+  const int splits = std::max(1, std::min(std::min(num_sms(), sm_cap) / split_tiles, kb / 4));
+  const GemmShape s = fit_gemm_shape(Nout, Kin + 1, n, splits, dYt, Xt, o);
+  return launch_gemm_tn(dYt.p, dYt.ld, Xt.p, Xt.ld, TMAP_F32, s, e, st);
 }
 
 // Sweep launch geometry: n > 0 persistent CTAs of FIT_SWEEP_CTA_THREADS threads (one per SM), else 8 x #SM CTAs of 256
@@ -1537,7 +1607,7 @@ static int fit_enqueue_encode(Fit* f, int step_off, int npeek, int buf_off, cuda
   const int tb = 256, blocks = (n * f->grid.n_levels * 4 + tb - 1) / tb;
   auto go = [&](auto kern) {
     return launch_k(f->pdl, kern, dim3(blocks), dim3(tb), 0, st, f->grid, f->tb, nullptr, f->coords, sr, n, f->enc, f->ld_enc,
-                    (size_t)n * f->ld_enc, f->sc_main, f->wd, npeek, buf_off);
+                    (size_t)n * f->ld_enc, f->enc_t, (size_t)n * (f->Lf + 1), f->sc_main, f->wd, npeek, buf_off);
   };
   static_assert(2 * FIT_MAX_WINDOW <= 16, "add an encode kernel instance");
   DVT_REQUIRE(npeek >= 0 && npeek <= 2 * FIT_MAX_WINDOW, "fit: encode with %d pending steps", npeek);
@@ -1582,14 +1652,21 @@ static int fit_enqueue_step(Fit* f, int step_off, bool phase2, bool epoch_end, c
   const Op enc{f->enc, f->ld_enc, p_enc}, h1{f->h1, f->ld_h1, p_h1}, dpred{f->dpred, C, p_nc}, dh1{f->dh1, H1, p_nh};
   const Op rawb{f->rawb, f->ld_raw, p_raw}, r1{f->r1, f->ld_r, p_r}, r2{f->r2, f->ld_r, p_r};
   const Op dR{f->dR, C, p_nc}, dr2{f->dr2, Hr, p_nr}, dr1{f->dr1, Hr, p_nr};
+  // transposed planes: [rows][n], plane stride rows * n (activations: rows = width + 1, the ones row)
+  const size_t t_enc = (size_t)(Lf + 1) * n, t_h1 = (size_t)(H1 + 1) * n, t_raw = (size_t)(C + 1) * n,
+               t_r = (size_t)(Hr + 1) * n;
+  const Op enc_t{f->enc_t, n, t_enc}, h1_t{f->h1_t, n, t_h1}, rawb_t{f->rawb_t, n, t_raw}, r1_t{f->r1_t, n, t_r},
+      r2_t{f->r2_t, n, t_r};
+  const Op dpred_t{f->dpred_t, n, p_nc}, dR_t{f->dR_t, n, p_nc}, dh1_t{f->dh1_t, n, p_nh}, dr2_t{f->dr2_t, n, p_nr},
+      dr1_t{f->dr1_t, n, p_nr};
   cudaStream_t sB = f->sB, sC = f->sC, sD = f->sD, sE = f->sE;
   const bool pdl = f->pdl;
   // The weight-gradient GEMMs only feed Adam(small), and are kept small (wcap): the CUPTI timeline (tools/fit_timeline.py)
   // shows the next kernel of the critical path waiting one CTA lifetime (~12 us, twice per step) whenever a finishing
-  // data-gradient GEMM hands its SMs to the queued CTAs of a weight-gradient GEMM -- every 3xTF32 CTA fills the shared
-  // memory of its SM.
+  // data-gradient GEMM hands its SMs to the queued CTAs of a weight-gradient GEMM (measured with mma.sync CTAs that filled
+  // the shared memory of their SM; the wgmma CTAs take half of it.  DESIGN.md section 4 has the caps measured since).
   const int wcap = f->wgrad_sms;
-  const GemmOpt gopt{pdl, f->x3_wide_min_n[phase2 ? 1 : 0]};
+  const GemmOpt gopt{pdl};
   auto fork = [&](cudaStream_t to, cudaEvent_t e) -> int {
     DVT_CUDA_OK(cudaEventRecord(e, st));
     DVT_CUDA_OK(cudaStreamWaitEvent(to, e, 0));
@@ -1602,23 +1679,28 @@ static int fit_enqueue_step(Fit* f, int step_off, bool phase2, bool epoch_end, c
   };
   // ---- forward ----
   FIT_RC(fork(sB, f->ev[0]));  // side B: gather the sampled bank rows (+ residual MLP forward in phase 2)
-  DVT_CUDA_OK(launch_k(pdl, fit_gather_rows_kernel, dim3(n), dim3(192), 0, sB, f->bank, C, sr, n, f->rawb, f->ld_raw, p_raw));
+  DVT_CUDA_OK(launch_k(pdl, fit_gather_rows_kernel, dim3((n + FIT_T_ROWS - 1) / FIT_T_ROWS), dim3(256),
+                       (size_t)fit_t_stage_bytes(C), sB, f->bank, C, sr, n, f->rawb, f->ld_raw, p_raw, f->rawb_t, t_raw));
   DVT_CUDA_OK(cudaGetLastError());
   count_launch();
   const bool pipe = f->pipe[phase2 ? 1 : 0];
   if (!pipe) FIT_RC(fit_enqueue_encode(f, step_off, 0, f->epoch_windows, st));  // else f->enc is already this step's (fit_run)
   if (phase2) {
-    FIT_RC(fit_linear(rawb, n, C, W(f->R1), Hr, sp + f->rb1.off, ACT_RELU, f->r1, f->ld_r, p_r, true, sB, gopt));
-    FIT_RC(fit_linear(r1, n, Hr, W(f->R2), Hr, sp + f->rb2.off, ACT_RELU, f->r2, f->ld_r, p_r, true, sB, gopt));
-    FIT_RC(fit_linear(r2, n, Hr, W(f->R3), C, sp + f->rb3.off, ACT_NONE, f->Rout, C, 0, false, sB, gopt));
+    FIT_RC(fit_linear(rawb, n, C, W(f->R1), Hr, sp + f->rb1.off, ACT_RELU, f->r1, f->ld_r, p_r, true, f->r1_t, t_r, sB,
+                      gopt));
+    FIT_RC(fit_linear(r1, n, Hr, W(f->R2), Hr, sp + f->rb2.off, ACT_RELU, f->r2, f->ld_r, p_r, true, f->r2_t, t_r, sB,
+                      gopt));
+    FIT_RC(fit_linear(r2, n, Hr, W(f->R3), C, sp + f->rb3.off, ACT_NONE, f->Rout, C, 0, false, nullptr, 0, sB, gopt));
   }
-  FIT_RC(fit_linear(enc, n, Lf, W(f->W1), H1, sp + f->b1.off, ACT_RELU, f->h1, f->ld_h1, p_h1, true, st, gopt));
-  FIT_RC(fit_linear(h1, n, H1, W(f->W2), C, sp + f->b2.off, ACT_NONE, f->Fout, C, 0, false, st, gopt));
+  FIT_RC(fit_linear(enc, n, Lf, W(f->W1), H1, sp + f->b1.off, ACT_RELU, f->h1, f->ld_h1, p_h1, true, f->h1_t, t_h1, st,
+                    gopt));
+  FIT_RC(fit_linear(h1, n, H1, W(f->W2), C, sp + f->b2.off, ACT_NONE, f->Fout, C, 0, false, nullptr, 0, st, gopt));
   FIT_RC(join(sB, f->ev[1]));
   // ---- loss + d pred ----
   LossArgs la;
   la.raw = f->rawb; la.ld_raw = f->ld_raw; la.raw_plane = p_raw; la.sr = sr; la.F = f->Fout; la.G = sp + f->G.off; la.R = phase2 ? f->Rout : nullptr;
   la.dpred = f->dpred; la.dR = phase2 ? f->dR : nullptr; la.plane = p_nc;
+  la.dpred_t = f->dpred_t; la.dR_t = phase2 ? f->dR_t : nullptr; la.plane_t = p_nc;
   la.gG = nullptr;  // dG is scattered by fit_g_scatter_kernel on side C (phase 1), off the critical path
   la.losses = f->losses; la.n = n; la.C = C; la.hw = f->hw; la.loss_scale = f->loss_scale;
   la.ax_i0 = f->ax_i0; la.ax_w0 = f->ax_w0; la.ax_w1 = f->ax_w1; la.gw = f->gw; la.gh = f->gh;
@@ -1629,11 +1711,11 @@ static int fit_enqueue_step(Fit* f, int step_off, bool phase2, bool epoch_end, c
     FIT_RC(fork(sC, f->ev[3]));
     FIT_RC(fork(sE, f->ev[11]));
   }
-  FIT_RC(fit_wgrad(dpred, n, C, h1, H1, sg + f->W2.off, sg + f->b2.off, f->wg_sem + 0 * FIT_SEM_TILES, wcap, sB, gopt));   // side B
-  FIT_RC(fit_dgrad(dpred, n, C, Wt(f->W2), H1, f->h1, f->ld_h1, f->dh1, H1, p_nh, true, st, gopt));  // main
+  FIT_RC(fit_wgrad(dpred_t, n, C, h1_t, H1, sg + f->W2.off, sg + f->b2.off, f->wg_sem + 0 * FIT_SEM_TILES, wcap, phase2, sB, gopt));   // side B
+  FIT_RC(fit_dgrad(dpred, n, C, Wt(f->W2), H1, f->h1, f->ld_h1, f->dh1, H1, p_nh, true, f->dh1_t, p_nh, st, gopt));  // main
   FIT_RC(fork(sB, f->ev[4]));  // dh1 ready
-  FIT_RC(fit_wgrad(dh1, n, H1, enc, Lf, sg + f->W1.off, sg + f->b1.off, f->wg_sem + 1 * FIT_SEM_TILES, wcap, sB, gopt));  // side B (reads enc)
-  FIT_RC(fit_dgrad(dh1, n, H1, Wt(f->W1), Lf, nullptr, 0, f->denc, Lf, 0, false, st, gopt));
+  FIT_RC(fit_wgrad(dh1_t, n, H1, enc_t, Lf, sg + f->W1.off, sg + f->b1.off, f->wg_sem + 1 * FIT_SEM_TILES, wcap, phase2, sB, gopt));  // side B (reads enc_t)
+  FIT_RC(fit_dgrad(dh1, n, H1, Wt(f->W1), Lf, nullptr, 0, f->denc, Lf, 0, false, nullptr, 0, st, gopt));
   if (!phase2) {
     // dG (+ grid_sample's neighbour shares) on side C, enqueued BEHIND the two data-gradient GEMMs: launched beside them, its
     // 256 small CTAs take the registers the GEMM CTAs need and delay the critical path.
@@ -1656,17 +1738,17 @@ static int fit_enqueue_step(Fit* f, int step_off, bool phase2, bool epoch_end, c
   if (phase2) {
     // residual MLP backward: the data-gradient chain on side C, the weight-gradient GEMMs that do not feed it on side E
     //   side C: dr2 = dR.R3 -> dr1 = dr2.R2 -> dR1      side E: dR3 (needs dR, r2 only) -> [dr2 ready] dR2
-    FIT_RC(fit_dgrad(dR, n, C, Wt(f->R3), Hr, f->r2, f->ld_r, f->dr2, Hr, p_nr, true, sC, gopt));
+    FIT_RC(fit_dgrad(dR, n, C, Wt(f->R3), Hr, f->r2, f->ld_r, f->dr2, Hr, p_nr, true, f->dr2_t, p_nr, sC, gopt));
     DVT_CUDA_OK(cudaEventRecord(f->ev[12], sC));                                              // dr2 ready
-    FIT_RC(fit_dgrad(dr2, n, Hr, Wt(f->R2), Hr, f->r1, f->ld_r, f->dr1, Hr, p_nr, true, sC, gopt));
-    FIT_RC(fit_wgrad(dr1, n, Hr, rawb, C, sg + f->R1.off, sg + f->rb1.off, f->wg_sem + 2 * FIT_SEM_TILES, wcap, sC, gopt));
-    FIT_RC(fit_wgrad(dR, n, C, r2, Hr, sg + f->R3.off, sg + f->rb3.off, f->wg_sem + 3 * FIT_SEM_TILES, wcap, sE, gopt));
+    FIT_RC(fit_dgrad(dr2, n, Hr, Wt(f->R2), Hr, f->r1, f->ld_r, f->dr1, Hr, p_nr, true, f->dr1_t, p_nr, sC, gopt));
+    FIT_RC(fit_wgrad(dr1_t, n, Hr, rawb_t, C, sg + f->R1.off, sg + f->rb1.off, f->wg_sem + 2 * FIT_SEM_TILES, wcap, phase2, sC, gopt));
+    FIT_RC(fit_wgrad(dR_t, n, C, r2_t, Hr, sg + f->R3.off, sg + f->rb3.off, f->wg_sem + 3 * FIT_SEM_TILES, wcap, phase2, sE, gopt));
     DVT_CUDA_OK(cudaStreamWaitEvent(sE, f->ev[12], 0));
-    FIT_RC(fit_wgrad(dr2, n, Hr, r1, Hr, sg + f->R2.off, sg + f->rb2.off, f->wg_sem + 4 * FIT_SEM_TILES, wcap, sE, gopt));
+    FIT_RC(fit_wgrad(dr2_t, n, Hr, r1_t, Hr, sg + f->R2.off, sg + f->rb2.off, f->wg_sem + 4 * FIT_SEM_TILES, wcap, phase2, sE, gopt));
     FIT_RC(join(sE, f->ev[13]));
   }
   FIT_RC(join(sC, f->ev[5]));
-  FIT_RC(join(sB, f->ev[6]));  // all small-parameter gradients complete; enc no longer read by a wgrad
+  FIT_RC(join(sB, f->ev[6]));  // all small-parameter gradients complete; enc_t no longer read by a wgrad
   // ---- Adam(small) on side B, beside the table work ----
   FIT_RC(fork(sB, f->ev[7]));
   const int nv = f->n_small / 4;
@@ -1873,16 +1955,17 @@ int fit_query(Fit* f, const float* coords, int n, float* out, cudaStream_t st) {
   FIT_RC(fit_before_caller(f, st));
   const int C = f->C, H1 = C / 2;
   const size_t cap = (size_t)f->q_cap, wp = (size_t)f->n_small;
-  const GemmOpt gopt{false, 0};  // no PDL, 128 x 64 tiles
+  const GemmOpt gopt{false};  // no PDL
   const StepRows sr{nullptr, f->step_base, 0};
   fit_encode_kernel<2><<<(n * f->grid.n_levels * 4 + 255) / 256, 256, 0, st>>>(
-      f->grid, f->tb, f->tb.p[f->cur_buf], coords, sr, n, f->q_enc, f->ld_enc, cap * f->ld_enc, nullptr, 0.f, 0, 0);
+      f->grid, f->tb, f->tb.p[f->cur_buf], coords, sr, n, f->q_enc, f->ld_enc, cap * f->ld_enc, nullptr, 0, nullptr, 0.f, 0,
+      0);
   DVT_CUDA_OK(cudaGetLastError());
   count_launch();
   FIT_RC(fit_linear(Op{f->q_enc, f->ld_enc, cap * f->ld_enc}, n, f->Lf, Op{f->wsplit + f->W1.off, f->Lf, wp}, H1,
-                    f->sp + f->b1.off, ACT_RELU, f->q_h1, f->ld_h1, cap * f->ld_h1, true, st, gopt));
+                    f->sp + f->b1.off, ACT_RELU, f->q_h1, f->ld_h1, cap * f->ld_h1, true, nullptr, 0, st, gopt));
   FIT_RC(fit_linear(Op{f->q_h1, f->ld_h1, cap * f->ld_h1}, n, H1, Op{f->wsplit + f->W2.off, H1, wp}, C, f->sp + f->b2.off,
-                    ACT_NONE, out, C, 0, false, st, gopt));
+                    ACT_NONE, out, C, 0, false, nullptr, 0, st, gopt));
   return DVT_OK;
 }
 
@@ -1893,17 +1976,18 @@ int fit_residual(Fit* f, const float* raw, int n, float* out, cudaStream_t st) {
   FIT_RC(fit_before_caller(f, st));
   const int C = f->C, Hr = C / 4;
   const size_t cap = (size_t)f->q_cap, wp = (size_t)f->n_small;
-  const GemmOpt gopt{false, 0};  // no PDL, 128 x 64 tiles
+  const GemmOpt gopt{false};  // no PDL
   const StepRows sr{nullptr, f->step_base, 0};
-  fit_gather_rows_kernel<<<n, 192, 0, st>>>(raw, C, sr, n, f->q_raw, f->ld_raw, cap * f->ld_raw);
+  fit_gather_rows_kernel<<<(n + FIT_T_ROWS - 1) / FIT_T_ROWS, 256, 0, st>>>(raw, C, sr, n, f->q_raw, f->ld_raw,
+                                                                            cap * f->ld_raw, nullptr, 0);
   DVT_CUDA_OK(cudaGetLastError());
   count_launch();
   FIT_RC(fit_linear(Op{f->q_raw, f->ld_raw, cap * f->ld_raw}, n, C, Op{f->wsplit + f->R1.off, C, wp}, Hr, f->sp + f->rb1.off,
-                    ACT_RELU, f->q_r1, f->ld_r, cap * f->ld_r, true, st, gopt));
+                    ACT_RELU, f->q_r1, f->ld_r, cap * f->ld_r, true, nullptr, 0, st, gopt));
   FIT_RC(fit_linear(Op{f->q_r1, f->ld_r, cap * f->ld_r}, n, Hr, Op{f->wsplit + f->R2.off, Hr, wp}, Hr, f->sp + f->rb2.off,
-                    ACT_RELU, f->q_r2, f->ld_r, cap * f->ld_r, true, st, gopt));
+                    ACT_RELU, f->q_r2, f->ld_r, cap * f->ld_r, true, nullptr, 0, st, gopt));
   FIT_RC(fit_linear(Op{f->q_r2, f->ld_r, cap * f->ld_r}, n, Hr, Op{f->wsplit + f->R3.off, Hr, wp}, C, f->sp + f->rb3.off,
-                    ACT_NONE, out, C, 0, false, st, gopt));
+                    ACT_NONE, out, C, 0, false, nullptr, 0, st, gopt));
   return DVT_OK;
 }
 

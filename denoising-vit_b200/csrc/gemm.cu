@@ -7,12 +7,12 @@
 //   The accumulators are then staged through shared memory (the drained operand ring) and the eight consumer warps run
 //   the fused epilogue on 32 x 32 chunks in a coalesced layout.  Three stages (96 KB) keep two CTAs resident per SM, so
 //   one CTA's epilogue overlaps the other's main loop.
-// 3xTF32 products of the stage-1 fit (fp32 hi/lo operand planes):
-//   both operands K-major (forward linears, data gradients against the transposed weights): gemm_wgmma_x3_kernel,
-//   128 x 64 tiles of wgmma m64n64k8 TF32, two CTAs per SM
-//   an MN-major operand (weight gradients dY^T [X | 1], which read the activations in place): gemm_x3_kernel, 128 x 64 or
-//   128 x 128 tiles, 8 warps of mma.sync m16n8k8 TF32 with fragments read from the swizzled TMA tiles -- wgmma's TF32
-//   form takes K-major operands only.
+// 3xTF32 products (fp32 hi/lo operand planes):
+//   both operands K-major -- every product of the stage-1 fit: the forward linears and data gradients, and the weight
+//   gradients dY^T [X | 1], which read transposed copies of dY and X written by their producers (GemmEpi::out_t):
+//   gemm_wgmma_x3_kernel, 128 x 64 tiles of wgmma m64n64k8 TF32, two CTAs per SM
+//   an MN-major operand (dvt_gemm_f32x3 only): gemm_x3_kernel, 128 x 64 tiles, 8 warps of mma.sync m16n8k8 TF32 with
+//   fragments read from the swizzled TMA tiles -- wgmma's TF32 form takes K-major operands only.
 // K tails, M tails and N tails are handled by TMA zero-fill plus masking in the epilogue.
 //
 // Used for: patch-embed, QKV, attention out-proj, MLP fc1/fc2 (reference: timm VisionTransformer reached from
@@ -55,16 +55,15 @@ struct X3Smem {
 };
 
 // A never-taken branch at the entry of the wgmma and 3xTF32 kernels (GemmEpi::entry_guard is always null).  It does nothing
-// at run time, but nvcc 12.9 allocates registers for these kernels better with it.  Without it the three 128-wide
-// gemm_x3_kernel instantiations go from 244 / 244 / 246 registers to 255 with 12-20 bytes of spill stores, the 64-wide ones
-// from 222 / 230 / 232 to 226 / 254 / 240, the gemm_wgmma_kernel ones from 90 to 92, and gemm_wgmma_swiglu_bwd_kernel
-// spills 4 bytes.  An empty asm statement or moving tile_of() does not have the same effect.
+// at run time, but nvcc 12.9 allocates registers for these kernels better with it.  Without it (measured when it was
+// added) the gemm_x3_kernel instantiations took up to 24 more registers, the gemm_wgmma_kernel ones went from 90 to 92, and
+// gemm_wgmma_swiglu_bwd_kernel spilled 4 bytes.  An empty asm statement or moving tile_of() does not have the same effect.
 __device__ __forceinline__ void gemm_entry_guard(const GemmEpi& e) {
   if (threadIdx.x == 0 && e.entry_guard && blockIdx.x == 0) e.entry_guard[0] = 0;
 }
 
 template <bool FIT>
-__device__ __forceinline__ void epi_scalar_tail(const GemmEpi& e, const GemmShape& s, const float* scr, int pitch, int lane,
+__device__ __forceinline__ void epi_scalar_tail(const GemmEpi& e, const GemmShape& s, float* scr, int pitch, int lane,
                                                 int m0, int n, bool has_k) {
 #pragma unroll 1
   for (int jj = 0; jj < 8; ++jj) {
@@ -74,18 +73,21 @@ __device__ __forceinline__ void epi_scalar_tail(const GemmEpi& e, const GemmShap
 #pragma unroll 1
     for (int q = 0; q < 4; ++q) {
       if (n + q >= s.N) break;
-      const float x = scr[i * pitch + (lane & 7) * 4 + q];
-      epi_post1<FIT>(e, m, n + q, epi_pre<FIT>(e, m, n + q, has_k ? x : 0.0f));
+      float* x = scr + i * pitch + (lane & 7) * 4 + q;
+      const float v = epi_pre<FIT>(e, m, n + q, has_k ? *x : 0.0f);
+      epi_post1<FIT>(e, m, n + q, v);
+      if (FIT && e.out_t) *x = v;  // read back by epi_store_t
     }
   }
 }
 
 // One 32-row x 32-column chunk of an accumulator tile staged in shared memory (`scr`: the chunk's first element, rows
 // `pitch` floats apart), with the fused epilogue in the coalesced layout (each lane: 4 consecutive columns of 8 rows).
+// FIT with GemmEpi::out_t: the epilogue's values replace the accumulators in `scr`, for epi_store_t.
 // m0: global row of this lane's first row (chunk row base + lane / 8); n_base: global column of the chunk.  Everything
 // that depends on the column (bias, LayerScale, ...) is loaded once per chunk as a float4.
 template <bool FIT = false>
-__device__ __forceinline__ void epi_chunk(const GemmEpi& e, const GemmShape& s, const float* scr, int pitch, int lane,
+__device__ __forceinline__ void epi_chunk(const GemmEpi& e, const GemmShape& s, float* scr, int pitch, int lane,
                                           int n_base, int m0, bool has_k) {
   const int col4 = (lane & 7) * 4;
   const int n = n_base + col4;
@@ -194,6 +196,7 @@ __device__ __forceinline__ void epi_chunk(const GemmEpi& e, const GemmShape& s, 
         }
       }
       if (e.alpha != 1.0f) { x.x *= e.alpha; x.y *= e.alpha; x.z *= e.alpha; x.w *= e.alpha; }
+      if (FIT && e.out_t) *reinterpret_cast<float4*>(scr + i * pitch + col4) = x;
       if (!FIT && e.out_mode == OUT_F32_RESID) {
         float4 o = xin[jj];
         o.x = fmaf(g4.x, x.x, o.x); o.y = fmaf(g4.y, x.y, o.y); o.z = fmaf(g4.z, x.z, o.z); o.w = fmaf(g4.w, x.w, o.w);
@@ -305,7 +308,7 @@ __device__ __forceinline__ TileIdx tile_of(const GemmShape& s, int bn, int bk) {
 // chunks w, w + nwarps, ...  GLU: the SwiGLU-backward epilogue (epi_chunk_swiglu_bwd) instead of epi_chunk; a compile-time
 // switch, so that no other instantiation carries its code.
 template <bool FIT, int BN, bool GLU = false>
-__device__ __forceinline__ void epi_tile(const GemmEpi& e, const GemmShape& s, const float* tile, int pitch, int warp,
+__device__ __forceinline__ void epi_tile(const GemmEpi& e, const GemmShape& s, float* tile, int pitch, int warp,
                                          int nwarps, int lane, int tm, int tn, bool has_k) {
 #pragma unroll 1
   for (int c = warp; c < (BM / 32) * (BN / 32); c += nwarps) {
@@ -557,12 +560,8 @@ gemm_x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
 #pragma unroll
         for (int mi = 0; mi < 2; ++mi) {
-          // s.x3 is always 1 here.  The test stays because the compiler schedules around it: without it the 128-wide
-          // instantiations go from 244-246 registers to 255 with 120-156 bytes of spills (nvcc 12.9, sm_90a).
-          if (s.x3 == 1) {
-            mma_tf32(acc[mi][ni], al[mi], bh);  // small terms first
-            mma_tf32(acc[mi][ni], ah[mi], bl);
-          }
+          mma_tf32(acc[mi][ni], al[mi], bh);  // small terms first
+          mma_tf32(acc[mi][ni], ah[mi], bl);
           mma_tf32(acc[mi][ni], ah[mi], bh);
         }
       }
@@ -619,6 +618,30 @@ constexpr int X3W_PITCH = X3W_BN + 8;
 constexpr int X3W_SMEM = X3W_OFF_BAR + 2 * X3W_STAGES * 8 + 1024;
 static_assert(BM * X3W_PITCH * 4 <= X3W_OFF_BAR, "staged accumulators must fit in the operand ring");
 static_assert(2 * (X3W_SMEM + 1024) <= 228 * 1024, "two CTAs per SM");
+
+// GemmEpi::out_t of a tile whose epilogue values epi_tile has left in `tile` ([BM][pitch]): thread t of the 256 takes row
+// t % 128 and half t / 128 of the 64 columns, so each store of a warp writes 32 consecutive m of one transposed row.
+__device__ __forceinline__ void epi_store_t(const GemmEpi& e, const GemmShape& s, const float* tile, int pitch, int tm,
+                                            int tn) {
+  const int r = threadIdx.x & (BM - 1), m = tm * BM + r;
+  if (m >= s.M) return;
+  const int c0 = (threadIdx.x >> 7) * (X3W_BN / 2);
+#pragma unroll 2
+  for (int c = c0; c < c0 + X3W_BN / 2; c += 4) {
+    const int n = tn * X3W_BN + c;
+    if (n >= s.N) break;
+    const float4 v4 = *reinterpret_cast<const float4*>(tile + r * pitch + c);
+    const float v[4] = {v4.x, v4.y, v4.z, v4.w};
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      if (n + q >= s.N) break;
+      const float hi = tf32_hi(v[q]);
+      float* o = e.out_t + (size_t)(n + q) * e.ldt + m;
+      o[0] = hi;
+      o[e.plane_t] = v[q] - hi;
+    }
+  }
+}
 
 __global__ void __launch_bounds__(WG_THREADS, 2)
 gemm_wgmma_x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmShape s,
@@ -721,6 +744,10 @@ gemm_wgmma_x3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
     named_bar(1, 256);
   }
   epi_tile<true, X3W_BN>(e, s, tile, X3W_PITCH, warp, 8, lane, ti.tm, ti.tn, ti.kb0 < ti.kb_total);
+  if (e.out_t) {  // (OUT_F32_SPLIT: never split-K)
+    named_bar(1, 256);
+    epi_store_t(e, s, tile, X3W_PITCH, ti.tm, ti.tn);
+  }
   if (serial) {
     __threadfence();
     named_bar(1, 256);
@@ -766,8 +793,17 @@ __global__ void gemm_tn_simt_kernel(const T* __restrict__ A, int lda, const T* _
     __syncthreads();
   }
   if (m < s.M && n < s.N) {
-    if (e.mask_mode == 2) swiglu_bwd_store1(e, m, n, s.N, acc);
-    else epi_post1(e, m, n, epi_pre(e, m, n, acc));
+    if (e.mask_mode == 2) {
+      swiglu_bwd_store1(e, m, n, s.N, acc);
+    } else {
+      const float v = epi_pre(e, m, n, acc);
+      epi_post1(e, m, n, v);
+      if (e.out_t) {
+        const float hi = tf32_hi(v);
+        e.out_t[(size_t)n * e.ldt + m] = hi;
+        e.out_t[e.plane_t + (size_t)n * e.ldt + m] = v - hi;
+      }
+    }
   }
 }
 
@@ -849,15 +885,9 @@ int gemm_prepare() {
   if ((rc = set_smem(gemm_wgmma_x3_kernel, X3W_SMEM))) return rc;
   if ((rc = set_smem(gemm_x3_kernel<64, false, true>, X3Smem<64>::TOTAL))) return rc;
   if ((rc = set_smem(gemm_x3_kernel<64, true, true>, X3Smem<64>::TOTAL))) return rc;
-  if ((rc = set_smem(gemm_x3_kernel<128, false, true>, X3Smem<128>::TOTAL))) return rc;
-  if ((rc = set_smem(gemm_x3_kernel<128, true, true>, X3Smem<128>::TOTAL))) return rc;
   done = true;
   return DVT_OK;
 }
-
-// Tile width of the mma.sync 3xTF32 kernels (an MN-major operand): 128 x 128 halves the operand traffic per flop, 128 x 64 gives twice the CTAs and the
-// shorter epilogue.  The caller chooses per call (GemmShape::x3_wide_min_n; 0 = always 128 x 64).
-int gemm_x3_tile_n(int N, int wide_min_n) { return (wide_min_n > 0 && N >= wide_min_n) ? 128 : 64; }
 
 int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dtype, const GemmShape& shape,
                    const GemmEpi& epi_in, cudaStream_t stream) {
@@ -899,6 +929,8 @@ int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dty
   DVT_REQUIRE(!misaligned(epi.branch, 8), "gemm: branch must be 8-byte aligned");
   DVT_REQUIRE(!misaligned(epi.last_col_out, 4), "gemm: last_col_out must be 4-byte aligned");
   DVT_REQUIRE(epi.out_mode != OUT_F32_SPLIT || epi.out_plane % 4 == 0, "gemm: the lo plane offset must be a multiple of 4");
+  DVT_REQUIRE(epi.out_t == nullptr || (epi.out_mode == OUT_F32_SPLIT && s.x3 && !s.a_mn && !s.b_mn && epi.ldt >= s.M),
+              "gemm: a transposed output needs OUT_F32_SPLIT of a 3xTF32 product with both operands K-major and ldt >= M");
   const int elem = dtype == TMAP_BF16 ? 2 : 4;
   DVT_REQUIRE(!misaligned(A, 16) && !misaligned(B, 16), "gemm: operands must be 16-byte aligned");
   if (s.x3) {
@@ -936,12 +968,11 @@ int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dty
     int rc3;
     // both operands K-major: wgmma (gemm_wgmma_x3_kernel); an MN-major operand: mma.sync (gemm_x3_kernel)
     const bool kk = !s.a_mn && !s.b_mn;
-    const int bn3 = kk ? X3W_BN : gemm_x3_tile_n(s.N, s.x3_wide_min_n);
     if (s.a_mn) rc3 = make_tmap_3d(&tA, A, TMAP_F32, (uint64_t)s.M, (uint64_t)s.K, 2, (uint64_t)lda * 4, s.plane_a * 4, 32, 32, 2);
     else rc3 = make_tmap_3d(&tA, A, TMAP_F32, (uint64_t)s.K, (uint64_t)s.M, 2, (uint64_t)lda * 4, s.plane_a * 4, 32, BM, 2);
     if (rc3) return rc3;
     if (s.b_mn) rc3 = make_tmap_3d(&tB, B, TMAP_F32, (uint64_t)s.N, (uint64_t)s.K, 2, (uint64_t)ldb * 4, s.plane_b * 4, 32, 32, 2);
-    else rc3 = make_tmap_3d(&tB, B, TMAP_F32, (uint64_t)s.K, (uint64_t)s.N, 2, (uint64_t)ldb * 4, s.plane_b * 4, 32, bn3, 2);
+    else rc3 = make_tmap_3d(&tB, B, TMAP_F32, (uint64_t)s.K, (uint64_t)s.N, 2, (uint64_t)ldb * 4, s.plane_b * 4, 32, X3W_BN, 2);
     if (rc3) return rc3;
     if (kk) {
       const int tiles = ((s.M + BM - 1) / BM) * ((s.N + X3W_BN - 1) / X3W_BN) * s.splits;
@@ -950,10 +981,6 @@ int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dty
       count_launch();
       DVT_CUDA_OK(cudaGetLastError());
       return DVT_OK;
-    }
-    if (bn3 == 128) {
-      if (s.a_mn) return launch_x3<128, true, true>(tA, tB, s, epi, stream);
-      return launch_x3<128, false, true>(tA, tB, s, epi, stream);
     }
     if (s.a_mn) return launch_x3<64, true, true>(tA, tB, s, epi, stream);
     return launch_x3<64, false, true>(tA, tB, s, epi, stream);

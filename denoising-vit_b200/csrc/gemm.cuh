@@ -49,6 +49,9 @@ struct GemmEpi {
   int row_offset = 0;                 // prefix tokens
   unsigned* splitk_sem = nullptr;     // OUT_F32_ATOMIC with split-K, 3xTF32 kernel: one zeroed counter per output tile; the
                                       // splits of a tile then add in split order (a deterministic sum), resetting it to 0
+  float* out_t = nullptr;             // OUT_F32_SPLIT of a 3xTF32 product with both operands K-major (and the SIMT debug
+  int ldt = 0;                        // GEMM), optional: the same hi / lo values transposed, out_t[n * ldt + m] = hi,
+  size_t plane_t = 0;                 // out_t[plane_t + n * ldt + m] = lo (the K-major operand of a later product over m)
 };
 
 struct GemmShape {
@@ -62,7 +65,6 @@ struct GemmShape {
   int x3 = 0;    // 1: 3xTF32 as described
   size_t plane_a = 0, plane_b = 0;
   int pdl = 0;   // launch with programmatic stream serialisation (the kernel calls pdl_wait() after its set-up)
-  int x3_wide_min_n = 0;  // x3 with an MN-major operand (mma.sync kernel): 128 x 128 tiles when N >= this (0: always 128 x 64)
 };
 
 // FIT = true (the 3xTF32 kernels of the stage-1 fit): epilogue features only other callers use -- GELU, the bf16 mask with
@@ -211,6 +213,5 @@ int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dty
 int launch_splitk_planes_sum(const float* planes, int splits, size_t plane, int M, int N, int ldo, float* out,
                              cudaStream_t st);
 int gemm_prepare();
-int gemm_x3_tile_n(int N, int wide_min_n);  // 64 or 128: tile width launch_gemm_tn picks for a 3xTF32 product
 
 }  // namespace dvt

@@ -7,12 +7,12 @@
 namespace dvt {
 struct Vit;
 int vit_create(Vit** out, int embed, int depth, int heads, int patch, int mlp_hidden, int swiglu, int layerscale,
-               int prefix, float ln_eps, int pre_norm, int patch_bias);
+               int prefix, float ln_eps, int pre_norm, int patch_bias, int rope);
 void vit_destroy(Vit* v);
 int vit_load(Vit* v, const char* name, const float* src, size_t numel);
 int vit_reserve(Vit* v, size_t tokens, size_t patches);
 int vit_forward(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int stride, const float* pos_patch,
-                const float* prefix_rows, int layer_index, int apply_norm, float* out, int out_all_tokens,
+                const float* prefix_rows, const float* rope, int layer_index, int apply_norm, float* out, int out_all_tokens,
                 cudaStream_t stream);
 int vit_patch(const Vit* v);
 int vit_prefix(const Vit* v);
@@ -45,6 +45,8 @@ int hashgrid_bwd(int n_levels, const float* scale, const uint32_t* res, const ui
 int launch_attention_bwd(const __nv_bfloat16* qkv, const __nv_bfloat16* out, const __nv_bfloat16* dout, const float* lse,
                          __nv_bfloat16* dqkv, float* dq_acc, float* delta, int B, int N, int heads, cudaStream_t stream,
                          int head_dim);
+int launch_rope_bwd(__nv_bfloat16* dqkv, int ld, const float* rope, int M, int ntok, int prefix, int heads, int head_dim,
+                    cudaStream_t st);
 int launch_layernorm_bwd(const float* x, const float* gamma, const float* dy, float* dx_accum, float* dgamma, float* dbeta,
                          int rows, int C, float eps, cudaStream_t st);
 int launch_colsum(const void* in, bool bf16, int ld, int rows, int cols, float* out, cudaStream_t st);
@@ -96,7 +98,7 @@ using namespace dvt;
 
 extern "C" {
 
-int dvt_version(void) { return 102; }
+int dvt_version(void) { return 103; }
 
 const char* dvt_last_error(void) { return dvt::last_error(); }
 
@@ -222,6 +224,30 @@ int dvt_gemm_bf16(const void* A, int lda, int a_mn, const void* B, int ldb, int 
   return launch_gemm_tn(A, lda, B, ldb, TMAP_BF16, s, e, reinterpret_cast<cudaStream_t>(stream));
 }
 /* ---- stage-3 (distillation) operators ---- */
+int dvt_gemm_qkv_rope(const void* x_bf16, int ldx, const void* w_bf16, int ldw, int M, int C, const float* bias,
+                      const float* rope, int ntok, int prefix, int heads, int head_dim, void* qkv_bf16, int ldo, void* stream) {
+  DVT_REQUIRE(x_bf16 && w_bf16 && rope && qkv_bf16, "dvt_gemm_qkv_rope: null pointer");
+  DVT_REQUIRE(head_dim == 64, "dvt_gemm_qkv_rope: head_dim must be 64 (got %d)", head_dim);
+  DVT_REQUIRE(heads > 0 && C == heads * head_dim, "dvt_gemm_qkv_rope: C=%d must be heads * head_dim", C);
+  DVT_REQUIRE(ntok > 0 && M % ntok == 0, "dvt_gemm_qkv_rope: M=%d must be a multiple of the tokens per image %d", M, ntok);
+  DVT_REQUIRE(ldo >= 3 * C, "dvt_gemm_qkv_rope: ldo=%d must be >= 3C=%d", ldo, 3 * C);
+  GemmEpi e;
+  e.bias = bias;
+  e.out = qkv_bf16;
+  e.ldo = ldo;
+  e.out_mode = OUT_BF16;
+  e.rope = rope;
+  e.rope_cols = 2 * C;
+  e.rope_ntok = ntok;
+  e.rope_prefix = prefix;
+  GemmShape s{M, 3 * C, C, 1};
+  return launch_gemm_tn(x_bf16, ldx, w_bf16, ldw, TMAP_BF16, s, e, reinterpret_cast<cudaStream_t>(stream));
+}
+int dvt_rope_bwd(void* dqkv_bf16, int ld, const float* rope, int M, int ntok, int prefix, int heads, int head_dim,
+                 void* stream) {
+  return launch_rope_bwd(reinterpret_cast<__nv_bfloat16*>(dqkv_bf16), ld, rope, M, ntok, prefix, heads, head_dim,
+                         reinterpret_cast<cudaStream_t>(stream));
+}
 int dvt_swiglu(const void* hpre_bf16, void* out_bf16, size_t M, int Hh, void* stream) {
   return launch_swiglu(reinterpret_cast<const __nv_bfloat16*>(hpre_bf16), reinterpret_cast<__nv_bfloat16*>(out_bf16), M, Hh,
                        reinterpret_cast<cudaStream_t>(stream));
@@ -321,10 +347,10 @@ int dvt_im2col(const void* x, int x_dtype, void* out_bf16, int B, int H, int W, 
 }
 
 int dvt_vit_create(dvt_vit_t** out, int embed, int depth, int heads, int patch, int mlp_hidden, int swiglu,
-                   int layerscale, int prefix_tokens, float ln_eps, int pre_norm, int patch_bias) {
+                   int layerscale, int prefix_tokens, float ln_eps, int pre_norm, int patch_bias, int rope) {
   DVT_REQUIRE(out, "dvt_vit_create: null out");
   return vit_create(reinterpret_cast<Vit**>(out), embed, depth, heads, patch, mlp_hidden, swiglu, layerscale,
-                    prefix_tokens, ln_eps, pre_norm, patch_bias);
+                    prefix_tokens, ln_eps, pre_norm, patch_bias, rope);
 }
 void dvt_vit_destroy(dvt_vit_t* h) { vit_destroy(reinterpret_cast<Vit*>(h)); }
 int dvt_vit_load(dvt_vit_t* h, const char* timm_key, const float* src, size_t numel) {
@@ -340,10 +366,10 @@ int dvt_vit_reserve(dvt_vit_t* h, int max_batch, int H, int W, int stride) {
   return vit_reserve(v, (size_t)max_batch * (np + vit_prefix(v)), (size_t)max_batch * np);
 }
 int dvt_vit_forward(dvt_vit_t* h, const void* x, int x_dtype, int B, int H, int W, int stride,
-                    const float* pos_patch, const float* prefix_rows, int layer_index, int norm, float* out,
+                    const float* pos_patch, const float* prefix_rows, const float* rope, int layer_index, int norm, float* out,
                     int all_tokens, void* stream) {
   DVT_REQUIRE(h, "dvt_vit_forward: null handle");
-  return vit_forward(reinterpret_cast<Vit*>(h), x, x_dtype == DVT_DTYPE_BF16, B, H, W, stride, pos_patch, prefix_rows,
+  return vit_forward(reinterpret_cast<Vit*>(h), x, x_dtype == DVT_DTYPE_BF16, B, H, W, stride, pos_patch, prefix_rows, rope,
                      layer_index, norm, out, all_tokens, reinterpret_cast<cudaStream_t>(stream));
 }
 

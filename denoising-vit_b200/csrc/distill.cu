@@ -312,12 +312,63 @@ int launch_layernorm_bwd_grouped(const float* x, const float* gamma, const float
 }
 
 // ----------------------------------------------------------------------------------------------------
+// Backward of the 2-D RoPE of the QKV epilogue (gemm.cu epi_chunk_rope), in place on dqkv [M, ld] bf16: on the q and k
+// columns of every patch row, with (cos, sin) of the row's patch, per head and d < 32
+//   dx[d] = dy[d] cos + dy[d + 32] sin,   dx[d + 32] = dy[d + 32] cos - dy[d] sin      (dx = R^T dy, fp32, one bf16 store)
+// One thread per (patch row, head of q or k, 4 frequencies): no reductions, so the result does not depend on the schedule.
+// ----------------------------------------------------------------------------------------------------
+__global__ void rope_bwd_kernel(__nv_bfloat16* __restrict__ dqkv, int ld, const float* __restrict__ rope, int B, int ntok,
+                                int prefix, int qk_heads) {
+  const int np = ntok - prefix;
+  const int per_row = qk_heads * 8;
+  const size_t total = (size_t)B * np * per_row;
+  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
+    const int j = (int)(e % per_row);
+    const size_t bp = e / per_row;
+    const int p = (int)(bp % np), b = (int)(bp / np);
+    const int d = (j & 7) * 4;
+    __nv_bfloat16* lo = dqkv + ((size_t)b * ntok + prefix + p) * ld + (j >> 3) * 64 + d;
+    const uint2 ul = *reinterpret_cast<const uint2*>(lo);
+    const uint2 uh = *reinterpret_cast<const uint2*>(lo + 32);
+    const float4 c = __ldg(reinterpret_cast<const float4*>(rope + (size_t)p * 64 + d));
+    const float4 sn = __ldg(reinterpret_cast<const float4*>(rope + (size_t)p * 64 + 32 + d));
+    const float2 l01 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&ul.x));
+    const float2 l23 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&ul.y));
+    const float2 h01 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&uh.x));
+    const float2 h23 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&uh.y));
+    *reinterpret_cast<uint2*>(lo) = make_uint2(pack_bf16x2(l01.x * c.x + h01.x * sn.x, l01.y * c.y + h01.y * sn.y),
+                                               pack_bf16x2(l23.x * c.z + h23.x * sn.z, l23.y * c.w + h23.y * sn.w));
+    *reinterpret_cast<uint2*>(lo + 32) = make_uint2(pack_bf16x2(h01.x * c.x - l01.x * sn.x, h01.y * c.y - l01.y * sn.y),
+                                                    pack_bf16x2(h23.x * c.z - l23.x * sn.z, h23.y * c.w - l23.y * sn.w));
+  }
+}
+
+int launch_rope_bwd(__nv_bfloat16* dqkv, int ld, const float* rope, int M, int ntok, int prefix, int heads, int head_dim,
+                    cudaStream_t st) {
+  DVT_REQUIRE(dqkv && rope, "rope_bwd: null argument");
+  DVT_REQUIRE(head_dim == 64, "rope_bwd: head_dim must be 64 (got %d)", head_dim);
+  DVT_REQUIRE(heads > 0 && M > 0 && ntok > 0 && M % ntok == 0, "rope_bwd: bad shape M=%d tokens=%d heads=%d", M, ntok, heads);
+  DVT_REQUIRE(prefix >= 0 && prefix < ntok, "rope_bwd: needs 0 <= prefix < tokens per image (prefix=%d tokens=%d)", prefix,
+              ntok);
+  DVT_REQUIRE(ld >= 2 * heads * head_dim && ld % 4 == 0, "rope_bwd: ld=%d must be >= 2 * heads * 64 and a multiple of 4", ld);
+  DVT_REQUIRE(!misaligned(dqkv, 8) && !misaligned(rope, 16),
+              "rope_bwd: dqkv must be 8-byte aligned (4 x bf16 accesses), rope 16-byte aligned (float4 loads)");
+  const size_t total = (size_t)(M / ntok) * (ntok - prefix) * (2 * heads) * 8;
+  const int blocks = (int)std::min<size_t>((total + 255) / 256, (size_t)num_sms() * 16);
+  rope_bwd_kernel<<<blocks, 256, 0, st>>>(dqkv, ld, rope, M / ntok, ntok, prefix, 2 * heads);
+  DVT_CUDA_OK(cudaGetLastError());
+  count_launch();
+  return DVT_OK;
+}
+
+// ----------------------------------------------------------------------------------------------------
 // Token assembly of the training forward: the patch-embed GEMM with the OUT_F32_REMAP epilogue (bias + position) into the
 // token rows, then the prefix rows -- the first two steps of vit_forward (vit.cu) on caller-owned tensors.
 // ----------------------------------------------------------------------------------------------------
 int launch_vit_embed_fwd(const __nv_bfloat16* patches, int Kp, const __nv_bfloat16* w, const float* bias, const float* pos_patch,
                          const float* prefix_rows, int B, int np, int prefix, int C, float* out, cudaStream_t st) {
-  DVT_REQUIRE(patches && w && pos_patch && prefix_rows && out, "vit_embed_fwd: null argument");  // bias may be null
+  // bias may be null (CLIP), pos_patch too (the RoPE ViTs have no absolute position term)
+  DVT_REQUIRE(patches && w && prefix_rows && out, "vit_embed_fwd: null argument");
   DVT_REQUIRE(B > 0 && np > 0 && prefix >= 1 && C % 4 == 0 && Kp % 8 == 0, "vit_embed_fwd: bad shape");
   // the GEMM epilogue adds bias and pos_patch and stores out four columns at a time (the GEMM checks them too, by role)
   DVT_REQUIRE(!misaligned(out, 16) && !misaligned(bias, 16) && !misaligned(pos_patch, 16),

@@ -284,6 +284,49 @@ __device__ __forceinline__ void epi_chunk_swiglu_bwd(const GemmEpi& e, const Gem
   }
 }
 
+// epi_chunk of the QKV projection with the 2-D RoPE (GemmEpi::rope): a q / k chunk (32 columns, one half of a 64-wide head)
+// reads the matching 32 columns of the other half from the staged tile -- the 128-wide tile holds whole heads -- so the
+// rotation acts on the fp32 accumulators before the one bf16 store.  Each lane: 4 consecutive columns d of 8 rows, the
+// 4 partners d +- 32, and per patch row one float4 of cos and one of sin.
+__device__ __forceinline__ void epi_chunk_rope(const GemmEpi& e, const GemmShape& s, const float* scr, int pitch, int lane,
+                                               int n_base, int m0) {
+  const int col4 = (lane & 7) * 4;
+  const int n = n_base + col4;
+  const bool upper = (n_base & 32) != 0;   // second half of the head: out = v cos + v[d - 32] sin
+  const int dp = upper ? -32 : 32;
+  float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f), bp = b4;
+  if (e.bias) {
+    b4 = __ldg(reinterpret_cast<const float4*>(e.bias + n));
+    bp = __ldg(reinterpret_cast<const float4*>(e.bias + n + dp));
+  }
+  const float sg = upper ? 1.0f : -1.0f;
+  __nv_bfloat16* outp = reinterpret_cast<__nv_bfloat16*>(e.out);
+#pragma unroll
+  for (int jj = 0; jj < 8; ++jj) {
+    const int m = m0 + 4 * jj;
+    if (m >= s.M) continue;
+    const float* r = scr + ((lane >> 3) + 4 * jj) * pitch + col4;
+    float4 x = *reinterpret_cast<const float4*>(r);
+    x.x += b4.x; x.y += b4.y; x.z += b4.z; x.w += b4.w;
+    const int t = m % e.rope_ntok;
+    if (t >= e.rope_prefix) {
+      float4 y = *reinterpret_cast<const float4*>(r + dp);
+      y.x += bp.x; y.y += bp.y; y.z += bp.z; y.w += bp.w;
+      const float* cs = e.rope + (size_t)(t - e.rope_prefix) * 64 + (col4 & 31);
+      const float4 c = __ldg(reinterpret_cast<const float4*>(cs));
+      const float4 sn = __ldg(reinterpret_cast<const float4*>(cs + 32));
+      x.x = x.x * c.x + sg * (y.x * sn.x);
+      x.y = x.y * c.y + sg * (y.y * sn.y);
+      x.z = x.z * c.z + sg * (y.z * sn.z);
+      x.w = x.w * c.w + sg * (y.w * sn.w);
+    }
+    uint2 pk;
+    pk.x = pack_bf16x2(x.x, x.y);
+    pk.y = pack_bf16x2(x.z, x.w);
+    *reinterpret_cast<uint2*>(outp + (size_t)m * e.ldo + n) = pk;
+  }
+}
+
 
 // Tile t of a launch: (split, tile_n, tile_m), split fastest.
 struct TileIdx {
@@ -305,9 +348,9 @@ __device__ __forceinline__ TileIdx tile_of(const GemmShape& s, int bn, int bk) {
 }
 
 // Epilogue of a tile whose fp32 accumulators sit in shared memory ([BM][pitch]): warp w of `nwarps` takes the 32 x 32
-// chunks w, w + nwarps, ...  GLU: the SwiGLU-backward epilogue (epi_chunk_swiglu_bwd) instead of epi_chunk; a compile-time
-// switch, so that no other instantiation carries its code.
-template <bool FIT, int BN, bool GLU = false>
+// chunks w, w + nwarps, ...  GLU: the SwiGLU-backward epilogue (epi_chunk_swiglu_bwd) instead of epi_chunk; ROPE: the q / k
+// chunks take epi_chunk_rope.  Compile-time switches, so that no other instantiation carries their code.
+template <bool FIT, int BN, bool GLU = false, bool ROPE = false>
 __device__ __forceinline__ void epi_tile(const GemmEpi& e, const GemmShape& s, float* tile, int pitch, int warp,
                                          int nwarps, int lane, int tm, int tn, bool has_k) {
 #pragma unroll 1
@@ -315,7 +358,9 @@ __device__ __forceinline__ void epi_tile(const GemmEpi& e, const GemmShape& s, f
     const int rb = c / (BN / 32), cb = c % (BN / 32);
     const int n_base = tn * BN + cb * 32;
     if (n_base >= s.N || tm * BM + rb * 32 >= s.M) continue;  // whole chunk out of range (warp-uniform)
-    if constexpr (GLU)
+    if (ROPE && n_base < e.rope_cols)
+      epi_chunk_rope(e, s, tile + rb * 32 * pitch + cb * 32, pitch, lane, n_base, tm * BM + rb * 32 + (lane >> 3));
+    else if constexpr (GLU)
       epi_chunk_swiglu_bwd(e, s, tile + rb * 32 * pitch + cb * 32, pitch, lane, n_base, tm * BM + rb * 32 + (lane >> 3), has_k);
     else
       epi_chunk<FIT>(e, s, tile + rb * 32 * pitch + cb * 32, pitch, lane, n_base, tm * BM + rb * 32 + (lane >> 3), has_k);
@@ -323,9 +368,10 @@ __device__ __forceinline__ void epi_tile(const GemmEpi& e, const GemmShape& s, f
 }
 
 // Body of the wgmma kernels (below): gemm_wgmma_kernel<TF32, A_MN, B_MN> with the general epilogue,
-// gemm_wgmma_swiglu_bwd_kernel (bf16, B MN-major) with the SwiGLU-backward one and gemm_wgmma_planes_kernel (bf16, both
-// MN-major; PLANES: split k stores its partial tile into plane k of e.out, the OUT_F32_PLANES mode).
-template <bool TF32, bool A_MN, bool B_MN, bool GLU, bool PLANES = false>
+// gemm_wgmma_swiglu_bwd_kernel (bf16, B MN-major) with the SwiGLU-backward one, gemm_wgmma_planes_kernel (bf16, both
+// MN-major; PLANES: split k stores its partial tile into plane k of e.out, the OUT_F32_PLANES mode) and
+// gemm_wgmma_rope_kernel (bf16, both K-major; ROPE: the QKV projection with the 2-D RoPE epilogue).
+template <bool TF32, bool A_MN, bool B_MN, bool GLU, bool PLANES = false, bool ROPE = false>
 __device__ __forceinline__ void wgmma_gemm_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& s,
                                                 const GemmEpi& e) {
   static_assert(!(TF32 && (A_MN || B_MN)), "TF32 wgmma operands are K-major only");
@@ -432,7 +478,7 @@ __device__ __forceinline__ void wgmma_gemm_body(const CUtensorMap& tmA, const CU
     ep.out = reinterpret_cast<float*>(e.out) + (size_t)(blockIdx.x % s.splits) * e.out_plane;
     epi_tile<false, WG_BN, false>(ep, s, tile, EPI_PITCH, warp, 8, lane, ti.tm, ti.tn, ti.kb0 < ti.kb_total);
   } else {
-    epi_tile<false, WG_BN, GLU>(e, s, tile, EPI_PITCH, warp, 8, lane, ti.tm, ti.tn, ti.kb0 < ti.kb_total);
+    epi_tile<false, WG_BN, GLU, ROPE>(e, s, tile, EPI_PITCH, warp, 8, lane, ti.tm, ti.tn, ti.kb0 < ti.kb_total);
   }
 }
 
@@ -454,6 +500,13 @@ __global__ void __launch_bounds__(WG_THREADS, 2)
 gemm_wgmma_planes_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmShape s,
                          GemmEpi e) {
   wgmma_gemm_body<false, true, true, false, true>(tmA, tmB, s, e);
+}
+
+// QKV projection of a RoPE ViT (DINOv3): x [M, C] . Wqkv [3C, C]^T + bias, q and k of the patch rows rotated in the epilogue
+__global__ void __launch_bounds__(WG_THREADS, 2)
+gemm_wgmma_rope_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmShape s,
+                       GemmEpi e) {
+  wgmma_gemm_body<false, false, false, false, false, true>(tmA, tmB, s, e);
 }
 
 // ----------------------------------------------------------------------------------------------------
@@ -807,10 +860,36 @@ __global__ void gemm_tn_simt_kernel(const T* __restrict__ A, int lda, const T* _
   }
 }
 
-template <bool TF32, bool A_MN, bool B_MN, bool GLU = false, bool PLANES = false>
+// SIMT debug form of the RoPE epilogue: one thread per output element computes its own dot product and, on a rotated
+// column of a patch row, the one of its partner column n ^ 32 (the other half of the head), then rotates as epi_chunk_rope.
+__global__ void gemm_tn_simt_rope_kernel(const __nv_bfloat16* __restrict__ A, int lda, const __nv_bfloat16* __restrict__ B,
+                                         int ldb, GemmShape s, GemmEpi e) {
+  const int m = blockIdx.y * 16 + threadIdx.y;
+  const int n = blockIdx.x * 16 + threadIdx.x;
+  if (m >= s.M || n >= s.N) return;
+  auto dot = [&](int col) {
+    float acc = 0.0f;
+    for (int k = 0; k < s.K; ++k)
+      acc = fmaf(__bfloat162float(A[(size_t)m * lda + k]), __bfloat162float(B[(size_t)col * ldb + k]), acc);
+    return acc + (e.bias ? e.bias[col] : 0.0f);
+  };
+  float v = dot(n);
+  const int t = m % e.rope_ntok;
+  if (n < e.rope_cols && t >= e.rope_prefix) {
+    const float y = dot(n ^ 32);
+    const float* cs = e.rope + (size_t)(t - e.rope_prefix) * 64 + (n & 31);
+    v = (n & 32) ? v * cs[0] + y * cs[32] : v * cs[0] - y * cs[32];
+  }
+  reinterpret_cast<__nv_bfloat16*>(e.out)[(size_t)m * e.ldo + n] = __float2bfloat16_rn(v);
+}
+
+template <bool TF32, bool A_MN, bool B_MN, bool GLU = false, bool PLANES = false, bool ROPE = false>
 int launch_wgmma(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmShape& s, const GemmEpi& e, cudaStream_t stream) {
   const int tiles = ((s.M + BM - 1) / BM) * ((s.N + WG_BN - 1) / WG_BN) * s.splits;
-  if constexpr (PLANES)
+  if constexpr (ROPE)
+    DVT_CUDA_OK(launch_k(s.pdl != 0, gemm_wgmma_rope_kernel, dim3(tiles), dim3(WG_THREADS), (size_t)WG_SMEM, stream, tmA,
+                         tmB, s, e));
+  else if constexpr (PLANES)
     DVT_CUDA_OK(launch_k(s.pdl != 0, gemm_wgmma_planes_kernel, dim3(tiles), dim3(WG_THREADS), (size_t)WG_SMEM, stream, tmA,
                          tmB, s, e));
   else if constexpr (GLU)
@@ -882,6 +961,7 @@ int gemm_prepare() {
   if ((rc = set_smem(gemm_wgmma_kernel<false, true, true>, WG_SMEM))) return rc;
   if ((rc = set_smem(gemm_wgmma_swiglu_bwd_kernel, WG_SMEM))) return rc;
   if ((rc = set_smem(gemm_wgmma_planes_kernel, WG_SMEM))) return rc;
+  if ((rc = set_smem(gemm_wgmma_rope_kernel, WG_SMEM))) return rc;
   if ((rc = set_smem(gemm_wgmma_x3_kernel, X3W_SMEM))) return rc;
   if ((rc = set_smem(gemm_x3_kernel<64, false, true>, X3Smem<64>::TOTAL))) return rc;
   if ((rc = set_smem(gemm_x3_kernel<64, true, true>, X3Smem<64>::TOTAL))) return rc;
@@ -931,6 +1011,15 @@ int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dty
   DVT_REQUIRE(epi.out_mode != OUT_F32_SPLIT || epi.out_plane % 4 == 0, "gemm: the lo plane offset must be a multiple of 4");
   DVT_REQUIRE(epi.out_t == nullptr || (epi.out_mode == OUT_F32_SPLIT && s.x3 && !s.a_mn && !s.b_mn && epi.ldt >= s.M),
               "gemm: a transposed output needs OUT_F32_SPLIT of a 3xTF32 product with both operands K-major and ldt >= M");
+  const bool rope = epi.rope != nullptr;
+  DVT_REQUIRE(!rope || (dtype == TMAP_BF16 && !s.a_mn && !s.b_mn && !s.x3 && s.splits == 1 && epi.out_mode == OUT_BF16 &&
+                        epi.act == ACT_NONE && !epi.mask && !epi.mask_f32 && epi.alpha == 1.0f && !epi.last_col_out),
+              "gemm: the RoPE epilogue needs bf16 operands both K-major, no split-K and a plain bf16 output");
+  DVT_REQUIRE(!rope || (epi.rope_cols > 0 && epi.rope_cols % 64 == 0 && epi.rope_cols <= s.N),
+              "gemm: the RoPE columns must be whole 64-wide heads inside N (rope_cols=%d N=%d)", epi.rope_cols, s.N);
+  DVT_REQUIRE(!rope || (epi.rope_prefix >= 0 && epi.rope_prefix < epi.rope_ntok),
+              "gemm: RoPE needs 0 <= prefix < tokens per image (prefix=%d tokens=%d)", epi.rope_prefix, epi.rope_ntok);
+  DVT_REQUIRE(!misaligned(epi.rope, 16), "gemm: the RoPE table must be 16-byte aligned");
   const int elem = dtype == TMAP_BF16 ? 2 : 4;
   DVT_REQUIRE(!misaligned(A, 16) && !misaligned(B, 16), "gemm: operands must be 16-byte aligned");
   if (s.x3) {
@@ -947,7 +1036,10 @@ int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dty
 
   if (impl == GEMM_SIMT_DEBUG) {
     dim3 grid((s.N + 15) / 16, (s.M + 15) / 16), block(16, 16);
-    if (dtype == TMAP_BF16)
+    if (rope)
+      gemm_tn_simt_rope_kernel<<<grid, block, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(A), lda,
+                                                            reinterpret_cast<const __nv_bfloat16*>(B), ldb, s, epi);
+    else if (dtype == TMAP_BF16)
       gemm_tn_simt_kernel<__nv_bfloat16><<<grid, block, 0, stream>>>(
           reinterpret_cast<const __nv_bfloat16*>(A), lda, reinterpret_cast<const __nv_bfloat16*>(B), ldb, s, epi);
     else
@@ -995,6 +1087,7 @@ int launch_gemm_tn(const void* A, int lda, const void* B, int ldb, TmapDtype dty
   if (rc) return rc;
   if (dtype == TMAP_F32) return launch_wgmma<true, false, false>(tmA, tmB, s, epi, stream);
   if (glu) return launch_wgmma<false, false, true, true>(tmA, tmB, s, epi, stream);
+  if (rope) return launch_wgmma<false, false, false, false, false, true>(tmA, tmB, s, epi, stream);
   if (planes) return launch_wgmma<false, true, true, false, true>(tmA, tmB, s, epi, stream);
   if (s.a_mn) return launch_wgmma<false, true, true>(tmA, tmB, s, epi, stream);
   if (s.b_mn) return launch_wgmma<false, false, true>(tmA, tmB, s, epi, stream);

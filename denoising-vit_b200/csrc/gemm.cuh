@@ -52,6 +52,14 @@ struct GemmEpi {
   float* out_t = nullptr;             // OUT_F32_SPLIT of a 3xTF32 product with both operands K-major (and the SIMT debug
   int ldt = 0;                        // GEMM), optional: the same hi / lo values transposed, out_t[n * ldt + m] = hi,
   size_t plane_t = 0;                 // out_t[plane_t + n * ldt + m] = lo (the K-major operand of a later product over m)
+  // 2-D rotary position embedding of a QKV projection (OUT_BF16, bf16 operands both K-major, no split-K): columns
+  // [0, rope_cols) are 64-wide heads (q then k); in row m, token t = m % rope_ntok, the patch rows t >= rope_prefix get
+  //   out[d] = v[d] cos - v[d + 32] sin,  out[d + 32] = v[d + 32] cos + v[d] sin   (d < 32, v = acc + bias, fp32)
+  // with cos = rope[p * 64 + d], sin = rope[p * 64 + 32 + d], p = t - rope_prefix.  Its own kernel (gemm.cu).
+  const float* rope = nullptr;
+  int rope_cols = 0;
+  int rope_ntok = 0;
+  int rope_prefix = 0;
 };
 
 struct GemmShape {

@@ -5,7 +5,7 @@
 // Data flow per call (M = B * tokens, C = embed dim), all activations resident in HBM workspaces owned by the
 // handle; the residual stream is fp32, GEMM operands bf16 with fp32 accumulation in registers (wgmma):
 //   im2col -> [GEMM patch-embed (+ bias) + pos-embed -> x] -> prefix rows [-> norm_pre LayerNorm (CLIP: pre_norm)]
-//   per block: LN1 -> [GEMM qkv + bias] -> attention -> [GEMM proj + bias, x += ls1 * .] ->
+//   per block: LN1 -> [GEMM qkv + bias (+ 2-D RoPE on q, k of the patch rows: DINOv3)] -> attention -> [GEMM proj + bias, x += ls1 * .] ->
 //              LN2 -> [GEMM fc1 + bias + GELU] -> [GEMM fc2 + bias, x += ls2 * .]
 //   final LayerNorm + prefix strip -> NHWC fp32 (the layout main_img_denoising.py:323 permutes to)
 // Blocks after `layer_index` are skipped: the reference runs them (no stop_early) but they cannot change the
@@ -40,7 +40,7 @@ struct VitBlock {
 
 struct Vit {
   int embed, depth, heads, patch, mlp_hidden, swiglu, layerscale, prefix;
-  int head_dim, pre_norm, patch_bias;
+  int head_dim, pre_norm, patch_bias, rope;
   float ln_eps;
   int Kp;  // padded patch-embed K
   __nv_bfloat16* pe_w = nullptr;
@@ -65,7 +65,7 @@ static int dev_alloc(Vit* v, void** p, size_t bytes) {
 }
 
 int vit_create(Vit** out, int embed, int depth, int heads, int patch, int mlp_hidden, int swiglu, int layerscale,
-               int prefix, float ln_eps, int pre_norm, int patch_bias) {
+               int prefix, float ln_eps, int pre_norm, int patch_bias, int rope) {
   {
     int prc = gemm_prepare();
     if (prc) return prc;
@@ -73,10 +73,11 @@ int vit_create(Vit** out, int embed, int depth, int heads, int patch, int mlp_hi
   DVT_REQUIRE(heads > 0 && (embed == heads * 64 || embed == heads * 80),
               "vit: head_dim must be 64 or 80 (embed=%d heads=%d)", embed, heads);
   DVT_REQUIRE(embed % 8 == 0 && mlp_hidden % 8 == 0 && depth > 0 && patch > 0 && prefix >= 1, "vit: bad config");
+  DVT_REQUIRE(!rope || embed == heads * 64, "vit: RoPE needs head_dim 64 (embed=%d heads=%d)", embed, heads);
   Vit* v = new Vit();
   v->embed = embed; v->depth = depth; v->heads = heads; v->patch = patch; v->mlp_hidden = mlp_hidden;
   v->swiglu = swiglu; v->layerscale = layerscale; v->prefix = prefix; v->ln_eps = ln_eps;
-  v->head_dim = embed / heads; v->pre_norm = pre_norm ? 1 : 0; v->patch_bias = patch_bias ? 1 : 0;
+  v->head_dim = embed / heads; v->pre_norm = pre_norm ? 1 : 0; v->patch_bias = patch_bias ? 1 : 0; v->rope = rope ? 1 : 0;
   v->Kp = (3 * patch * patch + 7) / 8 * 8;
   v->blocks.resize(depth);
   const int C = embed, Hm = mlp_hidden, fc2_in = swiglu ? mlp_hidden / 2 : mlp_hidden;
@@ -193,12 +194,15 @@ int vit_reserve(Vit* v, size_t tokens, size_t patches) {
 }
 
 int vit_forward(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int stride, const float* pos_patch,
-                const float* prefix_rows, int layer_index, int apply_norm, float* out, int out_all_tokens,
+                const float* prefix_rows, const float* rope, int layer_index, int apply_norm, float* out, int out_all_tokens,
                 cudaStream_t stream) {
   const int C = v->embed, P = v->patch;
   DVT_REQUIRE(B > 0 && H >= P && W >= P && stride > 0, "vit_forward: bad input shape B=%d H=%d W=%d stride=%d", B, H, W, stride);
   DVT_REQUIRE(layer_index >= 0 && layer_index < v->depth, "vit_forward: layer_index %d out of range", layer_index);
-  DVT_REQUIRE(pos_patch && prefix_rows && out && x_in, "vit_forward: null pointer");
+  DVT_REQUIRE(prefix_rows && out && x_in, "vit_forward: null pointer");
+  DVT_REQUIRE(v->rope ? rope != nullptr : pos_patch != nullptr,
+              "vit_forward: a RoPE ViT needs the RoPE table, any other the position table");
+  DVT_REQUIRE(!misaligned(rope, 16) && !misaligned(pos_patch, 16), "vit_forward: pos_patch and rope must be 16-byte aligned");
   const int h = (H - P) / stride + 1, w = (W - P) / stride + 1;
   const int np = h * w, ntok = np + v->prefix;
   const size_t M = (size_t)B * ntok;
@@ -235,6 +239,7 @@ int vit_forward(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int 
     if (rc) return rc;
     {
       GemmEpi e; e.bias = b.qkv_b; e.out_mode = OUT_BF16; e.out = v->qkv; e.ldo = 3 * C;
+      if (v->rope) { e.rope = rope; e.rope_cols = 2 * C; e.rope_ntok = ntok; e.rope_prefix = v->prefix; }
       GemmShape s{Mi, 3 * C, C, 1};
       rc = launch_gemm_tn(v->xn, C, b.qkv_w, C, TMAP_BF16, s, e, stream);
       if (rc) return rc;

@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("DVT_LIB_PATH") or os.path.join(os.path.dirname(_HERE), "libdvt_b200.so")
 # dvt_version() of the library SIGNATURES describes.  A library with another version is refused: an entry point may keep
 # its name across versions but take other arguments, and calling it through these argtypes would pass garbage pointers.
-ABI_VERSION = 102
+ABI_VERSION = 103
 
 
 class DvtError(RuntimeError):
@@ -39,6 +39,9 @@ SIGNATURES = {
                                   c_void_p]),
     "dvt_layernorm_bwd_grouped": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                           c_float, c_int, c_int, c_void_p]),
+    "dvt_gemm_qkv_rope": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
+                                  c_int, c_void_p, c_int, c_void_p]),
+    "dvt_rope_bwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "dvt_swiglu": (c_int, [c_void_p, c_void_p, c_size_t, c_int, c_void_p]),
     "dvt_gemm_bf16_dgrad_swiglu": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p,
                                            c_int, c_void_p]),
@@ -103,12 +106,12 @@ SIGNATURES = {
     "dvt_depth_eval_sums": (c_int, [c_void_p, c_int, c_uint, c_int, c_int, c_void_p, c_int, c_int, c_float, c_float, c_int,
                                     c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "dvt_vit_create": (c_int, [POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_int,
-                               c_int]),
+                               c_int, c_int]),
     "dvt_vit_destroy": (None, [c_void_p]),
     "dvt_vit_load": (c_int, [c_void_p, c_char_p, c_void_p, c_size_t]),
     "dvt_vit_reserve": (c_int, [c_void_p, c_int, c_int, c_int, c_int]),
-    "dvt_vit_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int,
-                                c_void_p, c_int, c_void_p]),
+    "dvt_vit_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int,
+                                c_int, c_void_p, c_int, c_void_p]),
 }
 
 

@@ -53,6 +53,12 @@ MODEL_LIST = [
     "deit3_base_patch16_224.fb_in1k",
     "vit_base_patch16_384.augreg_in21k_ft_in1k",
 ]
+# DINOv3 (LVD-1689M weights), after the reference's list: 2-D RoPE ViTs, DINOV3_ARCHS below
+MODEL_LIST.extend([
+    "vit_small_patch16_dinov3.lvd1689m",
+    "vit_base_patch16_dinov3.lvd1689m",
+    "vit_large_patch16_dinov3.lvd1689m",
+])
 
 IMAGENET_MEAN, IMAGENET_STD = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)
 HALF_MEAN, HALF_STD = (0.5, 0.5, 0.5), (0.5, 0.5, 0.5)
@@ -61,10 +67,10 @@ OPENAI_CLIP_STD = (0.26862954, 0.26130258, 0.27577711)
 
 
 def _arch(embed, depth, heads, img, mlp=None, swiglu=False, ls=False, reg=0, no_embed_class=False,
-          mean=IMAGENET_MEAN, std=IMAGENET_STD, pre_norm=False, patch_bias=True, ln_eps=1e-6):
+          mean=IMAGENET_MEAN, std=IMAGENET_STD, pre_norm=False, patch_bias=True, ln_eps=1e-6, rope=False):
     return dict(embed=embed, depth=depth, heads=heads, img=img, mlp=mlp or 4 * embed, swiglu=swiglu, ls=ls, reg=reg,
                 no_embed_class=no_embed_class, mean=mean, std=std, pre_norm=pre_norm, patch_bias=patch_bias,
-                ln_eps=ln_eps)
+                ln_eps=ln_eps, rope=rope)
 
 
 # Pre-LN ViTs with head_dim 64 or 80 (what the CUDA path implements).  The CLIP towers are timm's pre_norm=True,
@@ -96,6 +102,89 @@ ARCHS = {
     "deit3_base_patch16_224.fb_in1k": _arch(768, 12, 12, 224, ls=True, no_embed_class=True),
     "vit_base_patch16_384.augreg_in21k_ft_in1k": _arch(768, 12, 12, 384, mean=HALF_MEAN, std=HALF_STD),
 }
+
+# DINOv3 ViT-S/B/L/16 (transformers DINOv3ViTModel): pre-LN blocks with LayerScale and a GELU MLP (ratio 4), LayerNorm eps
+# 1e-5, 4 register tokens, no absolute position embedding but a 2-D RoPE on q and k of the patch tokens (rope=True: fused
+# into the QKV GEMM epilogue, DESIGN.md section 8), q and v biases and no k bias (key_bias=False: the k slice of attn.qkv.bias
+# stays zero, in training too), ImageNet normalisation.
+DINOV3_ARCHS = {
+    "vit_small_patch16_dinov3.lvd1689m": _arch(384, 12, 6, 224, ls=True, reg=4, no_embed_class=True, ln_eps=1e-5, rope=True),
+    "vit_base_patch16_dinov3.lvd1689m": _arch(768, 12, 12, 224, ls=True, reg=4, no_embed_class=True, ln_eps=1e-5, rope=True),
+    "vit_large_patch16_dinov3.lvd1689m": _arch(1024, 24, 16, 224, ls=True, reg=4, no_embed_class=True, ln_eps=1e-5,
+                                               rope=True),
+}
+
+ROPE_BASE = 100.0   # DINOv3ViTConfig.rope_theta
+
+
+def arch_of(identifier: str) -> dict:
+    """The architecture entry of a backbone identifier, from ARCHS or DINOV3_ARCHS; NotImplementedError for the listed
+    identifiers the H100 path does not run (EVA02)."""
+    a = ARCHS.get(identifier) or DINOV3_ARCHS.get(identifier)
+    if a is None:
+        raise NotImplementedError(
+            f"{identifier}: architecture outside the pre-LN ViT family (head_dim 64 / 80) is not "
+            "implemented by the H100 path (see DESIGN.md, out of scope)")
+    return a
+
+
+def rope_table(h: int, w: int, head_dim: int = 64, base: float = ROPE_BASE) -> torch.Tensor:
+    """f32 [h * w, head_dim] (CPU): row p = (cos | sin) of the head_dim / 2 angles of patch p on the token grid (h, w), as
+    transformers DINOv3ViTRopePositionEmbedding computes them in eval mode: patch centres ((i + 0.5) / h, (j + 0.5) / w)
+    mapped to [-1, 1], angles = 2 pi coord (x) inv_freq flattened y-then-x, inv_freq = 1 / base ** arange(0, 1, 4 /
+    head_dim), all in fp32.  (HF tiles the angles twice; the kernels pair columns d and d + head_dim / 2 instead.)"""
+    inv_freq = 1.0 / base ** torch.arange(0, 1, 4 / head_dim, dtype=torch.float32)
+    ch = torch.arange(0.5, h, dtype=torch.float32) / h
+    cw = torch.arange(0.5, w, dtype=torch.float32) / w
+    coords = 2.0 * torch.stack(torch.meshgrid(ch, cw, indexing="ij"), dim=-1).flatten(0, 1) - 1.0
+    angles = (2 * math.pi * coords[:, :, None] * inv_freq[None, None, :]).flatten(1, 2)
+    return torch.cat([torch.cos(angles), torch.sin(angles)], dim=1).contiguous()
+
+
+_HF_LAYER = re.compile(r"^(?:model\.)?layer\.(\d+)\.(.+)$")
+_HF_BLOCK_KEYS = {"norm1.weight": "norm1.weight", "norm1.bias": "norm1.bias", "norm2.weight": "norm2.weight",
+                  "norm2.bias": "norm2.bias", "attention.o_proj.weight": "attn.proj.weight",
+                  "attention.o_proj.bias": "attn.proj.bias", "layer_scale1.lambda1": "ls1.gamma",
+                  "layer_scale2.lambda1": "ls2.gamma", "mlp.up_proj.weight": "mlp.fc1.weight",
+                  "mlp.up_proj.bias": "mlp.fc1.bias", "mlp.down_proj.weight": "mlp.fc2.weight",
+                  "mlp.down_proj.bias": "mlp.fc2.bias"}
+
+
+def is_hf_dinov3_state_dict(sd) -> bool:
+    return any(k.startswith("embeddings.") for k in sd)
+
+
+def hf_dinov3_to_container(sd) -> dict:
+    """`DINOv3ViTModel.state_dict()` keys -> the container's (timm-like) keys: q / k / v projections stacked into attn.qkv
+    with a zero k-bias slice (key_bias=False), LayerScale lambda1 -> gamma, up / down_proj -> fc1 / fc2; mask_token (a
+    pretraining-only parameter) is dropped.  Accepts the layer keys with or without HF's `model.` prefix."""
+    out, qkv = {}, {}
+    for k, v in sd.items():
+        if k == "embeddings.cls_token":
+            out["cls_token"] = v
+        elif k == "embeddings.register_tokens":
+            out["reg_token"] = v
+        elif k.startswith("embeddings.patch_embeddings."):
+            out["patch_embed.proj." + k[len("embeddings.patch_embeddings."):]] = v
+        elif k == "embeddings.mask_token":
+            continue
+        elif k in ("norm.weight", "norm.bias"):
+            out[k] = v
+        else:
+            m = _HF_LAYER.match(k)
+            if m is None:
+                raise KeyError(f"unexpected key in a DINOv3 state dict: {k}")
+            i, rest = int(m.group(1)), m.group(2)
+            if rest.startswith("attention.") and rest[len("attention.")] in "qkv" and rest[len("attention.") + 1:].startswith("_proj."):
+                qkv.setdefault(i, {})[rest[len("attention."):]] = v
+            elif rest in _HF_BLOCK_KEYS:
+                out[f"blocks.{i}.{_HF_BLOCK_KEYS[rest]}"] = v
+            else:
+                raise KeyError(f"unexpected key in a DINOv3 state dict: {k}")
+    for i, d in qkv.items():
+        out[f"blocks.{i}.attn.qkv.weight"] = torch.cat([d["q_proj.weight"], d["k_proj.weight"], d["v_proj.weight"]])
+        out[f"blocks.{i}.attn.qkv.bias"] = torch.cat([d["q_proj.bias"], torch.zeros_like(d["q_proj.bias"]), d["v_proj.bias"]])
+    return out
 
 
 class _LayerScale(nn.Module):
@@ -143,7 +232,8 @@ class _PatchEmbed(nn.Module):
 
 
 class B200VisionTransformer(nn.Module):
-    """Parameter container with timm's VisionTransformer attribute and state-dict names; the forward is CUDA."""
+    """Parameter container with timm's VisionTransformer attribute and state-dict names; the forward is CUDA.  A RoPE
+    arch (DINOv3) has no pos_embed, and `load_state_dict` also takes transformers' DINOv3ViTModel layout."""
 
     def __init__(self, identifier: str, patch: int, a: dict):
         super().__init__()
@@ -154,6 +244,7 @@ class B200VisionTransformer(nn.Module):
         self.num_prefix_tokens = 1 + a["reg"]
         self.num_reg_tokens = a["reg"]
         self.no_embed_class = a["no_embed_class"]
+        self.rope = bool(a.get("rope", False))
         self.dynamic_img_size = True
         grid = a["img"] // patch
         self.native_grid = (grid, grid)
@@ -161,8 +252,9 @@ class B200VisionTransformer(nn.Module):
         self.cls_token = nn.Parameter(torch.zeros(1, 1, dim))
         if a["reg"]:
             self.reg_token = nn.Parameter(torch.zeros(1, a["reg"], dim))
-        n_pos = grid * grid + (0 if a["no_embed_class"] else 1)
-        self.pos_embed = nn.Parameter(torch.randn(1, n_pos, dim) * 0.02)
+        if not self.rope:
+            n_pos = grid * grid + (0 if a["no_embed_class"] else 1)
+            self.pos_embed = nn.Parameter(torch.randn(1, n_pos, dim) * 0.02)
         eps = a["ln_eps"]
         if a["pre_norm"]:  # timm pre_norm=True (CLIP): LayerNorm over the assembled tokens before the first block
             self.norm_pre = nn.LayerNorm(dim, eps=eps)
@@ -195,10 +287,12 @@ class B200VisionTransformer(nn.Module):
         self._pos_cache = {}
         return super()._apply(fn, *a, **k)
 
-    def load_state_dict(self, *a, **k):
+    def load_state_dict(self, state_dict, *a, **k):
+        if self.rope and is_hf_dinov3_state_dict(state_dict):
+            state_dict = hf_dinov3_to_container(state_dict)
         self._dirty = True
         self._pos_cache = {}
-        return super().load_state_dict(*a, **k)
+        return super().load_state_dict(state_dict, *a, **k)
 
     def mark_dirty(self):
         """Call after editing parameters in place."""
@@ -217,7 +311,7 @@ class B200VisionTransformer(nn.Module):
             h = c_void_p()
             check(lib().dvt_vit_create(byref(h), a["embed"], a["depth"], a["heads"], self.patch_embed.patch_size[0],
                                        a["mlp"], int(a["swiglu"]), int(a["ls"]), self.num_prefix_tokens, a["ln_eps"],
-                                       int(a["pre_norm"]), int(a["patch_bias"])), "dvt_vit_create")
+                                       int(a["pre_norm"]), int(a["patch_bias"]), int(self.rope)), "dvt_vit_create")
             self._handle = h
         if not self._dirty:
             return
@@ -237,10 +331,23 @@ class B200VisionTransformer(nn.Module):
         except Exception:
             pass
 
-    def _pos_tables(self, h: int, w: int, device) -> Tuple[torch.Tensor, torch.Tensor]:
+    def _rope_table(self, h: int, w: int, device) -> torch.Tensor:
+        """The RoPE table f32 [h*w, 64] of the token grid (h, w) on `device` (`rope_table`), cached like the position
+        tables."""
+        key = ("rope", h, w, str(device))
+        if key not in self._pos_cache:
+            self._pos_cache[key] = rope_table(h, w, self.embed_dim // self.arch["heads"]).to(device)
+        return self._pos_cache[key]
+
+    def _pos_tables(self, h: int, w: int, device) -> Tuple[Optional[torch.Tensor], torch.Tensor]:
         """(pos_patch [h*w, C], prefix_rows [prefix, C]) following timm 1.0.7 `_pos_embed` + resample_abs_pos_embed
-        (bicubic, antialias, fp32; reference restatement evaluation/vitdet/vision_transformer.py:120-138)."""
+        (bicubic, antialias, fp32; reference restatement evaluation/vitdet/vision_transformer.py:120-138).  RoPE archs:
+        (None, [cls, registers])."""
         key = (h, w, str(device))
+        if key not in self._pos_cache and self.rope:
+            with torch.no_grad():
+                rows = [self.cls_token.detach().float().to(device)[0], self.reg_token.detach().float().to(device)[0]]
+                self._pos_cache[key] = (None, torch.cat(rows, 0).contiguous())
         if key not in self._pos_cache:
             with torch.no_grad():
                 pos = self.pos_embed.detach().float().to(device)
@@ -261,8 +368,10 @@ class B200VisionTransformer(nn.Module):
                 self._pos_cache[key] = (grid[0].contiguous(), torch.cat(rows, 0).contiguous())
         return self._pos_cache[key]
 
-    def _pos_tables_train(self, h: int, w: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    def _pos_tables_train(self, h: int, w: int) -> Tuple[Optional[torch.Tensor], torch.Tensor]:
         """`_pos_tables` inside the autograd graph: gradients reach pos_embed, cls_token and reg_token."""
+        if self.rope:
+            return None, torch.cat([self.cls_token.float()[0], self.reg_token.float()[0]], 0)
         pos = self.pos_embed.float()
         npre = 0 if self.no_embed_class else 1
         pre, grid = pos[:, :npre], pos[:, npre:]
@@ -296,12 +405,14 @@ class B200VisionTransformer(nn.Module):
         h, w = (H - P) // stride + 1, (W - P) // stride + 1
         prefix, ntok, C = self.num_prefix_tokens, self.num_prefix_tokens + h * w, self.embed_dim
         pos_patch, prefix_rows = self._pos_tables_train(h, w)
+        rope = (self._rope_table(h, w, x.device), prefix) if self.rope else None
         eps = self.arch["ln_eps"]
         t = train_ops.vit_embed(x, self.patch_embed.proj.weight, self.patch_embed.proj.bias, pos_patch, prefix_rows, stride)
         if self.arch["pre_norm"]:
             t = train_ops.vit_layernorm(t, self.norm_pre.weight, self.norm_pre.bias, eps)
         for i in range(layer_index + 1):
-            t = train_ops.vit_block_forward(t, self.blocks[i], self.arch["heads"], B, checkpoint=self._grad_ckpt, eps=eps)
+            t = train_ops.vit_block_forward(t, self.blocks[i], self.arch["heads"], B, checkpoint=self._grad_ckpt, eps=eps,
+                                            rope=rope)
         if norm:
             y = train_ops.vit_norm_strip(t, self.norm.weight, self.norm.bias, ntok, prefix, eps)
         else:
@@ -322,6 +433,7 @@ class B200VisionTransformer(nn.Module):
         stride = int(self.patch_embed.proj.stride[0])
         h, w = (H - P) // stride + 1, (W - P) // stride + 1
         pos_patch, prefix_rows = self._pos_tables(h, w, x.device)
+        rope = self._rope_table(h, w, x.device) if self.rope else None
         C = self.embed_dim
         shape = (B, self.num_prefix_tokens + h * w, C) if all_tokens else (B, h, w, C)
         if out is None:
@@ -329,7 +441,7 @@ class B200VisionTransformer(nn.Module):
         else:  # caller-provided destination (e.g. a slice of the stage-1 feature bank)
             assert tuple(out.shape) == shape and out.dtype == torch.float32 and out.is_contiguous() and out.is_cuda
         check(lib().dvt_vit_forward(self._handle, ptr(x), 0 if x.dtype == torch.bfloat16 else 1, B, H, W, stride,
-                                    ptr(pos_patch), ptr(prefix_rows), layer_index, int(norm), ptr(out),
+                                    ptr(pos_patch), ptr(prefix_rows), ptr(rope), layer_index, int(norm), ptr(out),
                                     int(all_tokens), cur_stream()), "dvt_vit_forward")
         return out
 
@@ -393,7 +505,7 @@ class PretrainedViTWrapper(nn.Module):
 
     @property
     def n_output_dims(self) -> int:
-        return self.model.pos_embed.shape[-1]
+        return self.model.embed_dim
 
     @property
     def num_blocks(self) -> int:
@@ -405,11 +517,7 @@ class PretrainedViTWrapper(nn.Module):
 
     def create_model(self, model_identifier: str, **kwargs):
         from torchvision import transforms
-        if model_identifier not in ARCHS:
-            raise NotImplementedError(
-                f"{model_identifier}: architecture outside the pre-LN ViT family (head_dim 64 / 80) is not "
-                "implemented by the H100 path (see DESIGN.md, out of scope)")
-        a = dict(ARCHS[model_identifier])
+        a = dict(arch_of(model_identifier))
         patch = int(kwargs.pop("patch_size", self.patch_size))
         if "img_size" in kwargs:
             a["img"] = int(kwargs.pop("img_size"))
@@ -425,7 +533,8 @@ class PretrainedViTWrapper(nn.Module):
         self.pretrained_loaded = False
         if path and os.path.isfile(path):
             sd = torch.load(path, map_location="cpu")
-            sd = {k[len("model."):] if k.startswith("model.") else k: v for k, v in sd.items()}
+            if not is_hf_dinov3_state_dict(sd):   # (HF's DINOv3 layout has `model.layer.*` keys of its own)
+                sd = {k[len("model."):] if k.startswith("model.") else k: v for k, v in sd.items()}
             model.load_state_dict(sd, strict=True)
             self.pretrained_loaded = True
         elif allow_random:
@@ -447,7 +556,7 @@ class PretrainedViTWrapper(nn.Module):
     def set_trainable(self, flag: bool = True):
         """Opt in to the training path (stage-3 distillation): with gradients enabled, `get_intermediate_layers` returns a
         differentiable result (one layer, no prefix tokens), for every backbone of `ARCHS`, the SwiGLU ViT-g/14 ones
-        included.  Off by default: the frozen-backbone callers keep the inference forward even when their parameters
+        included, and of `DINOV3_ARCHS`.  Off by default: the frozen-backbone callers keep the inference forward even when their parameters
         require grad."""
         self.model._trainable = bool(flag)
         return self

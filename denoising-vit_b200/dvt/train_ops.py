@@ -406,14 +406,14 @@ class _VitEmbedFn(torch.autograd.Function):
         patches = ops.im2col(img.detach().contiguous(), P, stride)
         wpad = torch.nn.functional.pad(pe_w.detach().float().reshape(C, K), (0, Kp - K)).to(torch.bfloat16).contiguous()
         out = torch.empty((B * (np_ + prefix), C), device=img.device, dtype=torch.float32)
-        pp = pos_patch.detach().float().contiguous()
+        pp = None if pos_patch is None else pos_patch.detach().float().contiguous()   # None: RoPE ViTs
         pr = prefix_rows.detach().float().contiguous()
         bias = None if pe_b is None else pe_b.detach().float().contiguous()   # None: patch embedding without bias (CLIP)
         check(lib().dvt_vit_embed_fwd(ptr(patches), Kp, ptr(wpad), ptr(bias), ptr(pp), ptr(pr), B, np_, prefix, C, ptr(out),
                                       cur_stream()), "dvt_vit_embed_fwd")
         ctx.save_for_backward(patches)
         ctx.meta = (B, prefix, C, P, K)
-        ctx.has_bias = pe_b is not None
+        ctx.has_bias, ctx.has_pos = pe_b is not None, pos_patch is not None
         return out
 
     @staticmethod
@@ -422,12 +422,12 @@ class _VitEmbedFn(torch.autograd.Function):
         B, prefix, C, P, K = ctx.meta
         dpatch, dpos, dprefix, dbias = vit_embed_bwd(dx0.detach().float().contiguous(), B, prefix)
         gw = wgrad(dpatch, patches)[:, :K].reshape(C, 3, P, P)
-        return None, gw, (dbias if ctx.has_bias else None), dpos, dprefix, None
+        return None, gw, (dbias if ctx.has_bias else None), (dpos if ctx.has_pos else None), dprefix, None
 
 
 def vit_embed(img: torch.Tensor, patch_embed_w, patch_embed_b, pos_patch, prefix_rows, stride: int) -> torch.Tensor:
     """Token rows f32 [B * (prefix + h*w), C] of images [B, 3, H, W] (f32 or bf16).  patch_embed_b None: no bias (and no
-    bias gradient)."""
+    bias gradient); pos_patch None: no position term (the RoPE ViTs)."""
     return _VitEmbedFn.apply(img, patch_embed_w, patch_embed_b, pos_patch, prefix_rows, stride)
 
 
@@ -459,19 +459,45 @@ def vit_layernorm(x: torch.Tensor, w, b, eps: float = 1e-6) -> torch.Tensor:
     return _VitLayerNormFn.apply(x, w, b, eps)
 
 
+def gemm_qkv_rope(x: torch.Tensor, w: torch.Tensor, bias, rope: torch.Tensor, batch: int, prefix: int,
+                  heads: int) -> torch.Tensor:
+    """qkv bf16 [M, 3C] = x bf16 [M, C] @ w bf16 [3C, C]^T + bias with the 2-D RoPE of the patch rows (rope f32 [np, 64],
+    rows (cos | sin)) fused into the GEMM epilogue (dvt_gemm_qkv_rope)."""
+    assert x.dtype == w.dtype == torch.bfloat16 and x.is_contiguous() and w.is_contiguous()
+    assert rope.dtype == torch.float32 and rope.is_contiguous()
+    M, C = x.shape
+    out = torch.empty((M, 3 * C), device=x.device, dtype=torch.bfloat16)
+    check(lib().dvt_gemm_qkv_rope(ptr(x), C, ptr(w), C, M, C, ptr(bias), ptr(rope), M // batch, prefix, heads, C // heads,
+                                  ptr(out), 3 * C, cur_stream()), "dvt_gemm_qkv_rope")
+    return out
+
+
+def rope_bwd_(dqkv: torch.Tensor, rope: torch.Tensor, batch: int, prefix: int, heads: int) -> torch.Tensor:
+    """In place on the q / k columns of dqkv bf16 [M, 3C]: the gradient w.r.t. the pre-rotation q / k (dvt_rope_bwd)."""
+    assert dqkv.dtype == torch.bfloat16 and dqkv.is_contiguous() and rope.is_contiguous()
+    M, C3 = dqkv.shape
+    check(lib().dvt_rope_bwd(ptr(dqkv), C3, ptr(rope), M, M // batch, prefix, heads, C3 // 3 // heads, cur_stream()),
+          "dvt_rope_bwd")
+    return dqkv
+
+
 def _is_swiglu(w1: torch.Tensor, w2: torch.Tensor) -> bool:
     """SwiGLUPacked MLP (ViT-g/14): fc2's input width is half of fc1's output width."""
     return 2 * w2.shape[1] == w1.shape[0]
 
 
-def _vit_block_fwd(x0, wts, heads: int, batch: int, keep: bool, eps: float = 1e-6):
+def _vit_block_fwd(x0, wts, heads: int, batch: int, keep: bool, eps: float = 1e-6, rope=None):
     """Forward of one pre-LN ViT block on prepared weights; returns (x2, activations for the backward or None).  The MLP is
-    GELU, or SwiGLU when fc2's input width is half of fc1's output width."""
+    GELU, or SwiGLU when fc2's input width is half of fc1's output width.  rope: (table f32 [np, 64], prefix) of a RoPE
+    ViT, fused into the QKV GEMM, or None."""
     n1w, n1b, wq, qkvb, wp, projb, ls1, n2w, n2b, w1, fc1b, w2, fc2b, ls2 = wts
     M, C = x0.shape
     N = M // batch
     xn1 = ops.layernorm(x0, n1w, n1b, eps, out_dtype=torch.bfloat16)
-    qkv = ops.gemm_tn(xn1, wq, qkvb, None, torch.bfloat16)
+    if rope is not None:
+        qkv = gemm_qkv_rope(xn1, wq, qkvb, rope[0], batch, rope[1], heads)
+    else:
+        qkv = ops.gemm_tn(xn1, wq, qkvb, None, torch.bfloat16)
     att, lse = attention_fwd_lse(qkv.view(batch, N, 3 * C), heads, C // heads)
     att = att.view(M, C)
     branch = lambda g: torch.empty((M, C), device=x0.device, dtype=torch.bfloat16) if (keep and g is not None) else None  # noqa
@@ -492,11 +518,14 @@ class _VitBlockFn(torch.autograd.Function):
     the CUDA kernels; bf16 GEMM operands, fp32 residual stream and fp32 master weights, as `_BlockFn`.  Saved for the
     backward: what `_BlockFn` saves, plus the bf16 pre-LayerScale branch values of the two residual GEMMs (LayerScale blocks
     only); for SwiGLU the MLP pair is the fc1 output [g | u] (bf16 [M, 2 Hh]) and silu(g) * u (bf16 [M, Hh]).
-    checkpoint=True saves the block input only and recomputes the forward during the backward."""
+    checkpoint=True saves the block input only and recomputes the forward during the backward.
+    rope (RoPE ViTs, DINOv3): (table f32 [np, 64], prefix); q and k of the patch rows are rotated in the QKV GEMM epilogue and
+    the backward rotates their gradients back (dvt_rope_bwd) before the QKV weight / bias / data gradients.  These ViTs
+    have no key bias: the k slice of the qkv bias gradient is zero."""
 
     @staticmethod
     def forward(ctx, x0, n1w, n1b, qkvw, qkvb, projw, projb, ls1, n2w, n2b, fc1w, fc1b, fc2w, fc2b, ls2, heads: int, batch: int,
-                checkpoint: bool, eps: float):
+                checkpoint: bool, eps: float, rope=None):
         if not x0.is_cuda:
             raise _lib.DvtError("dvt_b200 ViT training needs CUDA tensors (no CPU fallback)")
         f32 = lambda t: None if t is None else t.detach().float().contiguous()      # noqa: E731
@@ -504,18 +533,18 @@ class _VitBlockFn(torch.autograd.Function):
         wts = (f32(n1w), f32(n1b), b16(qkvw), f32(qkvb), b16(projw), f32(projb), f32(ls1), f32(n2w), f32(n2b), b16(fc1w),
                f32(fc1b), b16(fc2w), f32(fc2b), f32(ls2))
         x0 = x0.detach().float().contiguous()
-        x2, acts = _vit_block_fwd(x0, wts, heads, batch, keep=not checkpoint, eps=eps)
-        ctx.wts, ctx.heads, ctx.batch, ctx.checkpoint, ctx.eps = wts, heads, batch, checkpoint, eps
+        x2, acts = _vit_block_fwd(x0, wts, heads, batch, keep=not checkpoint, eps=eps, rope=rope)
+        ctx.wts, ctx.heads, ctx.batch, ctx.checkpoint, ctx.eps, ctx.rope = wts, heads, batch, checkpoint, eps, rope
         ctx.save_for_backward(x0, *(acts if acts is not None else ()))
         return x2
 
     @staticmethod
     def backward(ctx, dx2):
         x0, *acts = ctx.saved_tensors
-        wts, heads, batch, eps = ctx.wts, ctx.heads, ctx.batch, ctx.eps
+        wts, heads, batch, eps, rope = ctx.wts, ctx.heads, ctx.batch, ctx.eps, ctx.rope
         n1w, _, wq, _, wp, _, ls1, n2w, _, w1, _, w2, _, ls2 = wts
         if ctx.checkpoint:
-            _, acts = _vit_block_fwd(x0, wts, heads, batch, keep=True, eps=eps)
+            _, acts = _vit_block_fwd(x0, wts, heads, batch, keep=True, eps=eps, rope=rope)
         x1, xn1, qkv, att, lse, br1, xn2, hpre, hid, br2 = acts
         M, C = x0.shape
         N = M // batch
@@ -538,24 +567,29 @@ class _VitBlockFn(torch.autograd.Function):
         datt = dgrad(d1, wp, torch.bfloat16)
         dqkv = attention_bwd(qkv.view(batch, N, 3 * C), att.view(batch, N, C), datt.view(batch, N, C), lse, heads,
                              C // heads).view(M, 3 * C)
+        if rope is not None:
+            rope_bwd_(dqkv, rope[0], batch, rope[1], heads)
         g_qkvw = wgrad(dqkv, xn1)
         g_qkvb = colsum(dqkv)
+        if rope is not None:
+            g_qkvb[C:2 * C] = 0
         dxn1 = dgrad(dqkv, wq, torch.float32)
         dx0 = dx1
         g_n1w, g_n1b = layernorm_bwd_(dx0, x0, n1w, dxn1, eps)
         return (dx0, g_n1w, g_n1b, g_qkvw, g_qkvb, g_projw, g_projb, g_ls1, g_n2w, g_n2b, g_fc1w, g_fc1b, g_fc2w, g_fc2b, g_ls2,
-                None, None, None, None)
+                None, None, None, None, None)
 
 
 def vit_block_forward(x: torch.Tensor, blk, heads: int, batch: int, checkpoint: bool = False,
-                      eps: float = 1e-6) -> torch.Tensor:
+                      eps: float = 1e-6, rope=None) -> torch.Tensor:
     """x f32 [batch * tokens, C] through one ViT block (`blk`: module with timm Block parameter names; ls1 / ls2 either
-    LayerScale modules with `gamma` or identities).  head_dim = C / heads (64 or 80); eps of both LayerNorms."""
+    LayerScale modules with `gamma` or identities).  head_dim = C / heads (64 or 80); eps of both LayerNorms.  rope: (RoPE
+    table f32 [np, 64], prefix tokens) of a RoPE ViT (head_dim 64), or None."""
     ls1 = getattr(blk.ls1, "gamma", None)
     ls2 = getattr(blk.ls2, "gamma", None)
     return _VitBlockFn.apply(x, blk.norm1.weight, blk.norm1.bias, blk.attn.qkv.weight, blk.attn.qkv.bias, blk.attn.proj.weight,
                              blk.attn.proj.bias, ls1, blk.norm2.weight, blk.norm2.bias, blk.mlp.fc1.weight, blk.mlp.fc1.bias,
-                             blk.mlp.fc2.weight, blk.mlp.fc2.bias, ls2, heads, batch, checkpoint, eps)
+                             blk.mlp.fc2.weight, blk.mlp.fc2.bias, ls2, heads, batch, checkpoint, eps, rope)
 
 
 class _VitNormStripFn(torch.autograd.Function):

@@ -105,9 +105,11 @@ typedef struct dvt_vit dvt_vit_t;
 /* prefix_tokens = 1 (cls) + number of register tokens.  head_dim = embed / heads is 64 or 80.  pre_norm != 0: a
  * LayerNorm `norm_pre` (weights loaded as "norm_pre.weight" / "norm_pre.bias") over all token rows between the token
  * assembly and the first block (timm pre_norm=True: the CLIP towers).  patch_bias == 0: the patch embedding has no bias
- * ("patch_embed.proj.bias" is not a key).  ln_eps applies to every LayerNorm. */
+ * ("patch_embed.proj.bias" is not a key).  ln_eps applies to every LayerNorm.  rope != 0: 2-D rotary position embedding
+ * (DINOv3; head_dim 64) on q and k of the patch tokens, fused into the epilogue of the QKV GEMM, and no absolute position
+ * term (dvt_vit_forward takes the RoPE table instead of pos_patch). */
 int dvt_vit_create(dvt_vit_t** out, int embed, int depth, int heads, int patch, int mlp_hidden, int swiglu,
-                   int layerscale, int prefix_tokens, float ln_eps, int pre_norm, int patch_bias);
+                   int layerscale, int prefix_tokens, float ln_eps, int pre_norm, int patch_bias, int rope);
 void dvt_vit_destroy(dvt_vit_t* h);
 /* Loads one fp32 tensor by its timm state-dict key (without the wrapper's "model." prefix), e.g.
  * "blocks.3.attn.qkv.weight".  `src` may be host or device memory.  cls_token / reg_token / pos_embed are not
@@ -116,12 +118,14 @@ int dvt_vit_load(dvt_vit_t* h, const char* timm_key, const float* src, size_t nu
 /* Pre-sizes the activation workspaces (otherwise grown on first use). */
 int dvt_vit_reserve(dvt_vit_t* h, int max_batch, int H, int W, int stride);
 /* x: [B,3,H,W] f32 or bf16.  pos_patch: f32 [h*w, C] position embedding of the patch tokens for this grid
- * (already resampled).  prefix_rows: f32 [prefix_tokens, C] rows written in front of the patches (cls + its
- * position, register tokens).  Runs blocks 0..layer_index, applies the final LayerNorm if `norm`.
- * out (f32): all_tokens == 0 -> [B, h, w, C] (prefix stripped, NHWC); all_tokens == 1 -> [B, prefix + h*w, C]. */
+ * (already resampled; NULL for a RoPE ViT).  prefix_rows: f32 [prefix_tokens, C] rows written in front of the patches
+ * (cls + its position, register tokens).  rope (RoPE ViTs only, else NULL): f32 [h*w, 64], row p = (cos | sin) of the 32
+ * angles of patch p (dvt_gemm_qkv_rope).  16-byte aligned tables.  Runs blocks 0..layer_index, applies the final
+ * LayerNorm if `norm`.  out (f32): all_tokens == 0 -> [B, h, w, C] (prefix stripped, NHWC); all_tokens == 1 ->
+ * [B, prefix + h*w, C]. */
 int dvt_vit_forward(dvt_vit_t* h, const void* x, int x_dtype, int B, int H, int W, int stride,
-                    const float* pos_patch, const float* prefix_rows, int layer_index, int norm, float* out,
-                    int all_tokens, void* stream);
+                    const float* pos_patch, const float* prefix_rows, const float* rope, int layer_index, int norm,
+                    float* out, int all_tokens, void* stream);
 
 /* General form of dvt_gemm_tn for bf16 operands, no bias or activation: a_mn / b_mn = 1 reads the operand from its
  * transposed storage ([K, M] / [K, N] row-major, "MN-major") without a copy.  Supported: (a_mn, b_mn) in {(0,0), (0,1),
@@ -271,7 +275,8 @@ int dvt_layerscale_bwd(const float* dx, int ldx, const void* branch_bf16, const 
 /* Token assembly of the ViT forward on caller-owned tensors: out [B, prefix + np, C] f32 = patch rows
  * patches (bf16 [B*np, Kp], dvt_im2col) . w^T (bf16 [C, Kp], zero-padded conv weight) + bias + pos_patch[p] after
  * `prefix` rows copied from prefix_rows [prefix, C] (what dvt_vit_forward does before the first block).  bias may be
- * NULL: a patch embedding without bias (the CLIP towers).  out, bias and pos_patch 16-byte aligned. */
+ * NULL: a patch embedding without bias (the CLIP towers); pos_patch may be NULL: no position term (the RoPE ViTs).
+ * out, bias and pos_patch 16-byte aligned. */
 int dvt_vit_embed_fwd(const void* patches_bf16, int Kp, const void* w_bf16, const float* bias, const float* pos_patch,
                       const float* prefix_rows, int B, int np, int prefix, int C, float* out, void* stream);
 /* Backward of dvt_vit_embed_fwd w.r.t. everything but the image: from dx0 (f32 [B, ntok, C], ntok = prefix + np) writes
@@ -286,6 +291,23 @@ int dvt_vit_embed_bwd(const float* dx0, int B, int ntok, int prefix, int C, void
  * x, gamma, dy and dx_accum 16-byte aligned. */
 int dvt_layernorm_bwd_grouped(const float* x, const float* gamma, const float* dy, float* dx_accum, float* dgamma, float* dbeta,
                               float* workspace, int rows, int C, float eps, int in_group, int skip, void* stream);
+/* QKV projection of a RoPE ViT (DINOv3) with the 2-D rotary position embedding in the GEMM epilogue: qkv bf16 [M, 3C]
+ * (row pitch ldo >= 3C) = x (bf16 [M, C], pitch ldx) . w^T (bf16 [3C, C], pitch ldw) + bias (f32 [3C], may be NULL); then
+ * on the q and k columns (64-wide heads, C = heads * head_dim, head_dim 64) of every row whose token t = m % ntok is a patch
+ * token (t >= prefix, patch p = t - prefix), per head and d < 32, in fp32 before the bf16 store:
+ *   q[d] <- q[d] cos - q[d + 32] sin,   q[d + 32] <- q[d + 32] cos + q[d] sin,   cos = rope[p, d], sin = rope[p, 32 + d]
+ * rope f32 [ntok - prefix, 64] (16-byte aligned; rows (cos | sin) of the angles 2 pi coord_y inv_freq then 2 pi coord_x
+ * inv_freq, transformers DINOv3ViTRopePositionEmbedding).  M % ntok == 0, 0 <= prefix < ntok.  The operand and output rules
+ * of dvt_gemm_tn apply.  The tensor-core and the SIMT debug kernels (dvt_set_debug_impl) both fuse the rotation.
+ * Replaces: q_proj / k_proj / v_proj and apply_rotary_pos_emb of transformers DINOv3ViTAttention. */
+int dvt_gemm_qkv_rope(const void* x_bf16, int ldx, const void* w_bf16, int ldw, int M, int C, const float* bias,
+                      const float* rope, int ntok, int prefix, int heads, int head_dim, void* qkv_bf16, int ldo, void* stream);
+/* Backward of the rotation of dvt_gemm_qkv_rope, in place on the q and k columns of dqkv (bf16 [M, >= 2 * heads * 64], row
+ * pitch ld a multiple of 4, 8-byte aligned): on patch rows dx[d] = dy[d] cos + dy[d + 32] sin, dx[d + 32] = dy[d + 32] cos -
+ * dy[d] sin (the transpose of the forward rotation; fp32, one bf16 rounding).  Prefix rows and the v columns are not
+ * touched.  Same rope table and shape rules as dvt_gemm_qkv_rope; head_dim must be 64.  No reductions: deterministic. */
+int dvt_rope_bwd(void* dqkv_bf16, int ld, const float* rope, int M, int ntok, int prefix, int heads, int head_dim,
+                 void* stream);
 /* SwiGLU MLP (timm SwiGLUPacked, ViT-g/14): out [M, Hh] = silu(g) * u with [g | u] = hpre [M, 2 Hh] (bf16, contiguous), the
  * kernel of the inference forward, so a training forward produces the same bits. */
 int dvt_swiglu(const void* hpre_bf16, void* out_bf16, size_t M, int Hh, void* stream);

@@ -134,9 +134,8 @@ def main(args):
     m = re.search(r"patch(\d+)", args.model)
     patch = int(m.group(1))
     from dvt.models import vit_wrapper as VW
-    if args.model not in VW.ARCHS:
-        raise NotImplementedError(f"{args.model}: architecture outside the supported ViT family")
-    args.feat_dim = VW.ARCHS[args.model]["embed"]
+    arch = VW.arch_of(args.model)   # NotImplementedError outside the supported ViT families
+    args.feat_dim = arch["embed"]
     pos_h = (args.input_size[0] - patch) // args.stride_size + 1
     pos_w = (args.input_size[1] - patch) // args.stride_size + 1
     args.noise_map_height, args.noise_map_width = pos_h, pos_w
@@ -154,7 +153,6 @@ def main(args):
         packed = torch.load(args.collated, map_location="cpu")
         train_dataset = dataset.InMemoryPairs(packed["raw_feats"].to(device), packed["denoised_feats"].to(device))
     else:
-        arch = VW.ARCHS[args.model]
         train_dataset = dataset.FeatureStoreDataset(
             data_root=args.data_root, feat_root=args.feat_root, data_list=args.data_list_path,
             transform=transforms.Compose([transforms.Resize(args.input_size, interpolation=Image.BICUBIC, antialias=True),

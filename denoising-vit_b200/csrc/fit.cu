@@ -1255,17 +1255,22 @@ int fit_get_param(Fit* f, const char* name_c, float* dst, size_t numel) {
     DVT_CUDA_OK(cudaMemcpy(dst, src, numel * 4, cudaMemcpyDefault));
     return DVT_OK;
   }
+  // "<name>.m" / "<name>.v": the Adam moments of a small tensor, in the parameter's own layout
+  const size_t dot = name.size() > 2 ? name.size() - 2 : 0;
+  const bool moment = dot > 0 && (name.compare(dot, 2, ".m") == 0 || name.compare(dot, 2, ".v") == 0);
+  const std::string base = moment ? name.substr(0, dot) : name;
+  const float* buf = !moment ? f->sp : name[dot + 1] == 'm' ? f->sm : f->sv;
   Seg* s = nullptr;
-  DVT_REQUIRE(fit_find(f, name, &s), "fit_get_param: unknown parameter %s", name_c);
+  DVT_REQUIRE(fit_find(f, base, &s), "fit_get_param: unknown parameter %s", name_c);
   DVT_REQUIRE(numel == (size_t)s->rows * s->cols, "fit_get_param: %s size mismatch", name_c);
-  if (name == "G") {
+  if (base == "G") {
     int rc = fit_stage(f, numel);
     if (rc) return rc;
-    fit_transpose_kernel<<<256, 256>>>(f->sp + s->off, f->q_stage, f->hw, f->C);
+    fit_transpose_kernel<<<256, 256>>>(buf + s->off, f->q_stage, f->hw, f->C);
     DVT_CUDA_OK(cudaGetLastError());
     DVT_CUDA_OK(cudaMemcpy(dst, f->q_stage, numel * 4, cudaMemcpyDefault));
   } else {
-    DVT_CUDA_OK(cudaMemcpy(dst, f->sp + s->off, numel * 4, cudaMemcpyDefault));
+    DVT_CUDA_OK(cudaMemcpy(dst, buf + s->off, numel * 4, cudaMemcpyDefault));
   }
   return DVT_OK;
 }

@@ -186,6 +186,9 @@ void dvt_fit_destroy(dvt_fit_t* h);
 /* Parameters by name, fp32, host or device: "G" (shared_artifacts [1,C,gh,gw]), "res.{0,2,4}.{weight,bias}"
  * (residual_predictor), "table" (tcnn params, [entries*8]), "mlp.{0,2}.{weight,bias}" (NeuralFeatureField.mlp). */
 int dvt_fit_set_param(dvt_fit_t* h, const char* name, const float* src, size_t numel, void* stream);
+/* dvt_fit_get_param also reads the optimiser state: "<name>.m" / "<name>.v" are the Adam moments of any of the names
+ * above, in the parameter's own layout ("G.m" / "G.v" as [1,C,gh,gw]); "table.next" is the table buffer the next sweep
+ * writes. */
 int dvt_fit_get_param(dvt_fit_t* h, const char* name, float* dst, size_t numel);   /* blocks */
 /* Fresh parameters for the next fit, drawn on the device from a counter-based generator: what constructing new
  * SingleImageDenoiser / NeuralFeatureField modules does per image in the reference (main_img_denoising.py:39-47):

@@ -533,33 +533,3 @@ def test_simt_debug_path_every_entry_point():
         run_x3(M, 133, K, (1, 1), g, splits=2, last_col=True)
         run_swiglu(M, 132, K, g)
     assert _L().device_error() == 0
-
-
-# ------------------------------------------------------------------------------------------------ 128-wide 3xTF32 tile
-@pytest.mark.gpu
-def test_fit_x3_wide_tile_matches_narrow(monkeypatch):
-    """The fit's 3xTF32 GEMMs with 128 x 128 tiles everywhere (DVT_FIT_X3_WIDE_MIN_N=1,1) against 128 x 64 tiles
-    everywhere (0,0), six steps at the headline size: the same computation up to fp32 summation order."""
-    import test_fit_gpu as TF
-    from dvt.fit import FitEngine
-    cfg = dict(TF._FULL, num_iters=6, warmup_iters=2)
-    runs = []
-    for wide in ("0,0", "1,1"):
-        monkeypatch.setenv("DVT_FIT_X3_WIDE_MIN_N", wide)      # read by dvt_fit_create
-        feats, coords, init, idx, den, field, _ = TF._setup(cfg)
-        eng = FitEngine(cfg["C"], cfg["h"], cfg["w"], cfg["bsz"], field.meta)
-        eng.fit(den, field, feats.reshape(-1, cfg["C"]).cuda().contiguous(), coords.reshape(-1, 2).cuda().contiguous(), idx,
-                graph_steps=2, lr=cfg["lr"], min_lr=cfg["min_lr"], warmup_iters=cfg["warmup_iters"],
-                freeze_after=cfg["freeze_after"], weight_decay=cfg["weight_decay"], loss_scale=cfg["loss_scale"])
-        torch.cuda.synchronize()
-        assert _L().device_error() == 0
-        runs.append((eng.get_param("table", init["table"]).cpu() - init["table"], eng.losses().copy()))
-        del eng
-    (ta, la), (tb, lb) = runs
-    for j in range(5):
-        assert abs(lb[0, j] - la[0, j]) <= 1e-5 * abs(la[0, j]) + 1e-9, f"step 0 loss[{j}] {lb[0, j]} vs {la[0, j]}"
-    for s in range(6):
-        for j in range(5):
-            assert abs(lb[s, j] - la[s, j]) <= 1e-3 * abs(la[s, j]) + 1e-6, f"step {s} loss[{j}] {lb[s, j]} vs {la[s, j]}"
-    cos = torch.nn.functional.cosine_similarity(ta.flatten().double(), tb.flatten().double(), dim=0).item()
-    assert cos > 0.9999, f"table update cosine between tile widths {cos}"

@@ -64,13 +64,14 @@ class InMemoryPairs(torch.utils.data.Dataset):
 
 
 class InfiniteSampler(torch.utils.data.Sampler):
-    """0, 1, ..., n-1, 0, 1, ... for ever (single-process training)."""
+    """0, 1, ..., n-1, 0, 1, ... for ever (single-process training).  `start` is the number of indices already consumed
+    (a resumed run): the stream is entered at that position, without walking through the consumed part."""
 
-    def __init__(self, data_source):
-        self.n = len(data_source)
+    def __init__(self, data_source, start: int = 0):
+        self.n, self.start = len(data_source), int(start)
 
     def __iter__(self) -> Iterator[int]:
-        i = 0
+        i = self.start % self.n
         while True:
             yield i
             i = (i + 1) % self.n
@@ -78,11 +79,14 @@ class InfiniteSampler(torch.utils.data.Sampler):
 
 class DistributedInfiniteSampler(torch.utils.data.Sampler):
     """Rank r owns the indices r, r + world, ...; it shuffles them once (numpy default_rng seeded with the epoch) and then
-    cycles through that order for ever."""
+    cycles through that order for ever.  `start` is the number of indices this rank has already consumed: the same
+    shuffled order is entered at `start` modulo the length of the rank's shard (which is `num_samples`, or one less on
+    the trailing ranks when world does not divide n)."""
 
-    def __init__(self, data_source, num_replicas: int, rank: int):
+    def __init__(self, data_source, num_replicas: int, rank: int, start: int = 0):
         self.n, self.num_replicas, self.rank, self.epoch = len(data_source), num_replicas, rank, 0
         self.num_samples = math.ceil(self.n / num_replicas)
+        self.start = int(start)
 
     def set_epoch(self, epoch: int):
         self.epoch = epoch
@@ -95,5 +99,7 @@ class DistributedInfiniteSampler(torch.utils.data.Sampler):
         shards = [list(range(self.n))[i::self.num_replicas] for i in range(self.num_replicas)]
         mine = shards[self.rank]
         rng.shuffle(mine)
+        if mine:
+            yield from mine[self.start % len(mine):]
         while True:
             yield from mine

@@ -10,8 +10,10 @@ hand-written sm_90a kernels (dvt/train_ops.py, dvt/optim.py); data parallelism i
 gradient buffer per step (the reference wraps the model in DistributedDataParallel, :137-140).  Launch with torchrun
 (RANK / WORLD_SIZE / LOCAL_RANK from the environment), one process per GPU.
 
-H100 extension: `--collated <file.pt>` trains straight from the tensors stage 1 gathered with its all-gather
-(`main_img_denoising.py --collate_out`), held in HBM, instead of re-reading the `.npy` store.
+H100 extensions: `--collated <file.pt>` trains straight from the tensors stage 1 gathered with its all-gather
+(`main_img_denoising.py --collate_out`), held in HBM, instead of re-reading the `.npy` store.  `--resume <ckpt>`
+continues a run: the sampler enters the sample stream where the checkpointed step left it, so under `--deterministic`
+a resumed run continues the uninterrupted one bit for bit when seed, batch size and world size are unchanged.
 The PCA visualisation (reference :266-275) is outside the hot path and not produced."""
 import argparse
 import datetime
@@ -158,8 +160,12 @@ def main(args):
             transform=transforms.Compose([transforms.Resize(args.input_size, interpolation=Image.BICUBIC, antialias=True),
                                           transforms.ToTensor(), transforms.Normalize(arch["mean"], arch["std"])]))
     print(f"Dataset size: {len(train_dataset)}")
-    sampler = (dataset.DistributedInfiniteSampler(train_dataset, num_replicas=world, rank=rank) if world > 1
-               else dataset.InfiniteSampler(train_dataset))
+    ck = torch.load(args.resume, map_location=device) if args.resume else None
+    start_step = int(ck["step"]) + 1 if ck is not None else 0
+    # a resumed run enters this rank's sample stream after the samples of steps 0 .. start_step - 1
+    start_sample = start_step * args.batch_size
+    sampler = (dataset.DistributedInfiniteSampler(train_dataset, world, rank, start=start_sample) if world > 1
+               else dataset.InfiniteSampler(train_dataset, start=start_sample))
     in_memory = isinstance(train_dataset, dataset.InMemoryPairs)
     data_loader = torch.utils.data.DataLoader(train_dataset, batch_size=args.batch_size, sampler=sampler,
                                               num_workers=0 if in_memory else args.num_workers,
@@ -170,12 +176,9 @@ def main(args):
     optimizer = FusedAdamW(model.parameters(), betas=(0.9, 0.999), weight_decay=args.weight_decay)
     sched = dict(base_value=args.lr, final_value=args.min_lr, total_iters=args.num_iterations,
                  warmup_iters=int(args.num_iterations * 0.15), start_warmup_value=0)
-    start_step = 0
-    if args.resume:
-        ck = torch.load(args.resume, map_location=device)
+    if ck is not None:
         model.load_state_dict(ck["denoiser"], strict=False)
         optimizer.load_state_dict(ck["optimizer"])
-        start_step = int(ck["step"]) + 1
         print(f"Resumed from {args.resume} at step {start_step}")
 
     model.train()

@@ -16,9 +16,12 @@ dvt/optim.py); data parallelism is ONE NCCL all-reduce of the flat gradient buff
 in DistributedDataParallel, :146-151).  Launch with torchrun (RANK / WORLD_SIZE / LOCAL_RANK from the environment), one
 process per GPU.  Images are decoded and resized by CPU DataLoader workers, as in the reference.
 
-Extensions: `--resume <ckpt>` continues a run, `--log_freq` sets how often the losses are read back (the only host
-synchronisation of the loop).  The PCA visualisation of the reference (:275-283) is not produced: it needs imageio and
-matplotlib, which this build does not ship."""
+Extensions: `--resume <ckpt>` continues a run: the sampler enters the sample stream where the checkpointed step left
+it and the DataLoader's flip draws are replayed (dvt/dataset/resume.py), so under `--deterministic` a resumed run
+continues the uninterrupted one bit for bit when seed, batch size, world size and worker count are unchanged (with
+others it is a well-defined continuation, not the uninterrupted run).  `--log_freq` sets how often the losses are read
+back (the only host synchronisation of the loop).  The PCA visualisation of the reference (:275-283) is not produced:
+it needs imageio and matplotlib, which this build does not ship."""
 import argparse
 import datetime
 import math
@@ -181,8 +184,10 @@ def main(args):
         normalizer,
     ]))
     print(f"Dataset size: {len(train_dataset)}")
-    sampler = (dataset.DistributedInfiniteSampler(train_dataset, num_replicas=world, rank=rank) if world > 1
-               else dataset.InfiniteSampler(train_dataset))
+    # a resumed run enters this rank's sample stream after the samples of steps 0 .. start_step - 1
+    start_sample = start_step * args.batch_size
+    sampler = (dataset.DistributedInfiniteSampler(train_dataset, world, rank, start=start_sample) if world > 1
+               else dataset.InfiniteSampler(train_dataset, start=start_sample))
     steps_per_epoch = len(train_dataset) // (args.batch_size * world)
     print(f"steps_per_epoch: {steps_per_epoch}")
     if args.num_iterations is None:
@@ -203,7 +208,7 @@ def main(args):
     # ---- loop (:209-285) ----
     end = start = time.time()
     window = []
-    it = iter(data_loader)
+    it = dataset.resumed_iter(data_loader, start_step)   # RandomHorizontalFlip: one torch.rand(1) per sample
     for step in range(start_step, args.num_iterations):
         samples = next(it)[0].to(device, non_blocking=True)
         data_time = time.time() - end

@@ -14,6 +14,9 @@ int vit_reserve(Vit* v, size_t tokens, size_t patches);
 int vit_forward(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int stride, const float* pos_patch,
                 const float* prefix_rows, const float* rope, int layer_index, int apply_norm, float* out, int out_all_tokens,
                 cudaStream_t stream);
+int vit_forward_layers(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int stride, const float* pos_patch,
+                       const float* prefix_rows, const float* rope, int n_layers, const int* layers, int apply_norm,
+                       float* const* out, int ldo, int out_all_tokens, float* const* prefix_out, cudaStream_t stream);
 int vit_patch(const Vit* v);
 int vit_prefix(const Vit* v);
 struct Fit;
@@ -98,7 +101,7 @@ using namespace dvt;
 
 extern "C" {
 
-int dvt_version(void) { return 103; }
+int dvt_version(void) { return 104; }
 
 const char* dvt_last_error(void) { return dvt::last_error(); }
 
@@ -371,6 +374,38 @@ int dvt_vit_forward(dvt_vit_t* h, const void* x, int x_dtype, int B, int H, int 
   DVT_REQUIRE(h, "dvt_vit_forward: null handle");
   return vit_forward(reinterpret_cast<Vit*>(h), x, x_dtype == DVT_DTYPE_BF16, B, H, W, stride, pos_patch, prefix_rows, rope,
                      layer_index, norm, out, all_tokens, reinterpret_cast<cudaStream_t>(stream));
+}
+// Every check that does not need the handle comes before the null-handle check, so that a test without a GPU (no handle can
+// be created there) sees each refusal.
+int dvt_vit_forward_layers(dvt_vit_t* h, const void* x, int x_dtype, int B, int H, int W, int stride,
+                           const float* pos_patch, const float* prefix_rows, const float* rope, int n_layers,
+                           const int* layer_indices, int norm, float* const* out, int ldo, int all_tokens,
+                           float* const* prefix_out, void* stream) {
+  DVT_REQUIRE(x, "dvt_vit_forward_layers: x is null");
+  DVT_REQUIRE(prefix_rows, "dvt_vit_forward_layers: prefix_rows is null");
+  DVT_REQUIRE(n_layers > 0 && layer_indices, "dvt_vit_forward_layers: layer_indices must list n_layers >= 1 layers (n_layers=%d)",
+              n_layers);
+  DVT_REQUIRE(layer_indices[0] >= 0, "dvt_vit_forward_layers: layer_indices[0]=%d is negative", layer_indices[0]);
+  for (int l = 1; l < n_layers; ++l)
+    DVT_REQUIRE(layer_indices[l] > layer_indices[l - 1],
+                "dvt_vit_forward_layers: layer_indices must be strictly ascending (layer_indices[%d]=%d after %d)", l,
+                layer_indices[l], layer_indices[l - 1]);
+  DVT_REQUIRE(ldo > 0 && ldo % 4 == 0, "dvt_vit_forward_layers: ldo=%d must be a positive multiple of 4", ldo);
+  DVT_REQUIRE(out, "dvt_vit_forward_layers: out is null");
+  for (int l = 0; l < n_layers; ++l) {
+    DVT_REQUIRE(out[l], "dvt_vit_forward_layers: out[%d] is null", l);
+    DVT_REQUIRE(!misaligned(out[l], 16), "dvt_vit_forward_layers: out[%d] must be 16-byte aligned", l);
+  }
+  DVT_REQUIRE(!(all_tokens && prefix_out),
+              "dvt_vit_forward_layers: prefix_out with all_tokens (out already holds the prefix rows)");
+  for (int l = 0; prefix_out && l < n_layers; ++l) {
+    DVT_REQUIRE(prefix_out[l], "dvt_vit_forward_layers: prefix_out[%d] is null", l);
+    DVT_REQUIRE(!misaligned(prefix_out[l], 16), "dvt_vit_forward_layers: prefix_out[%d] must be 16-byte aligned", l);
+  }
+  DVT_REQUIRE(h, "dvt_vit_forward_layers: null handle");
+  return vit_forward_layers(reinterpret_cast<Vit*>(h), x, x_dtype == DVT_DTYPE_BF16, B, H, W, stride, pos_patch, prefix_rows,
+                            rope, n_layers, layer_indices, norm, out, ldo, all_tokens, prefix_out,
+                            reinterpret_cast<cudaStream_t>(stream));
 }
 
 int dvt_gemm_f32x3(const float* A, int lda, size_t plane_a, int a_mn, const float* B, int ldb, size_t plane_b, int b_mn,

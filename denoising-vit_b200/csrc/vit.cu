@@ -7,9 +7,10 @@
 //   im2col -> [GEMM patch-embed (+ bias) + pos-embed -> x] -> prefix rows [-> norm_pre LayerNorm (CLIP: pre_norm)]
 //   per block: LN1 -> [GEMM qkv + bias (+ 2-D RoPE on q, k of the patch rows: DINOv3)] -> attention -> [GEMM proj + bias, x += ls1 * .] ->
 //              LN2 -> [GEMM fc1 + bias + GELU] -> [GEMM fc2 + bias, x += ls2 * .]
-//   final LayerNorm + prefix strip -> NHWC fp32 (the layout main_img_denoising.py:323 permutes to)
-// Blocks after `layer_index` are skipped: the reference runs them (no stop_early) but they cannot change the
-// requested output.
+//   final LayerNorm + prefix strip -> NHWC fp32 (the layout main_img_denoising.py:323 permutes to), after every requested
+//   block (vit_tap): one pass serves any number of layers
+// Blocks after the last requested layer are skipped: the reference runs them (no stop_early) but they cannot change the
+// requested outputs.
 #include "common.cuh"
 
 #include <cstdlib>
@@ -193,13 +194,43 @@ int vit_reserve(Vit* v, size_t tokens, size_t patches) {
   return DVT_OK;
 }
 
-int vit_forward(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int stride, const float* pos_patch,
-                const float* prefix_rows, const float* rope, int layer_index, int apply_norm, float* out, int out_all_tokens,
-                cudaStream_t stream) {
+// Final LayerNorm (or plain copy) of the residual stream v->x after a block: the patch rows (all rows with all_tokens) into
+// `out` at row pitch ldo; with prefix_out, also the prefix rows of every image into prefix_out [B, prefix, C].  The prefix
+// rows go through the same per-row kernel as the patch rows, so they carry the bits an all_tokens tap gives them.
+static int vit_tap(Vit* v, int B, int ntok, bool norm, float* out, int ldo, bool all_tokens, float* prefix_out,
+                   cudaStream_t stream) {
+  const int C = v->embed, Mi = B * ntok, skip = all_tokens ? 0 : v->prefix;
+  if (norm) {
+    int rc = launch_layernorm(v->x, C, v->norm_w, v->norm_b, out, ldo, false, Mi, C, v->ln_eps, ntok, skip, stream);
+    if (rc) return rc;
+  } else {
+    strip_copy_kernel<<<Mi, 256, 0, stream>>>(v->x, C, out, ldo, Mi, C, ntok, skip);
+    DVT_CUDA_OK(cudaGetLastError());
+    count_launch();
+  }
+  if (!prefix_out) return DVT_OK;
+  for (int p = 0; p < v->prefix; ++p) {  // row b of launch p: token p of image b
+    const float* src = v->x + (size_t)p * C;
+    float* dst = prefix_out + (size_t)p * C;
+    if (norm) {
+      int rc = launch_layernorm(src, ntok * C, v->norm_w, v->norm_b, dst, v->prefix * C, false, B, C, v->ln_eps, 1, 0, stream);
+      if (rc) return rc;
+    } else {
+      strip_copy_kernel<<<B, 256, 0, stream>>>(src, ntok * C, dst, v->prefix * C, B, C, 1, 0);
+      DVT_CUDA_OK(cudaGetLastError());
+      count_launch();
+    }
+  }
+  return DVT_OK;
+}
+
+// Runs blocks 0..layers[n_layers - 1] once and taps the residual stream into out[l] after block layers[l] (vit_tap).
+// The caller has checked that layers is strictly ascending within [0, depth) and the destinations.
+static int vit_run(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int stride, const float* pos_patch,
+                   const float* prefix_rows, const float* rope, int n_layers, const int* layers, int apply_norm,
+                   float* const* out, int ldo, int out_all_tokens, float* const* prefix_out, cudaStream_t stream) {
   const int C = v->embed, P = v->patch;
   DVT_REQUIRE(B > 0 && H >= P && W >= P && stride > 0, "vit_forward: bad input shape B=%d H=%d W=%d stride=%d", B, H, W, stride);
-  DVT_REQUIRE(layer_index >= 0 && layer_index < v->depth, "vit_forward: layer_index %d out of range", layer_index);
-  DVT_REQUIRE(prefix_rows && out && x_in, "vit_forward: null pointer");
   DVT_REQUIRE(v->rope ? rope != nullptr : pos_patch != nullptr,
               "vit_forward: a RoPE ViT needs the RoPE table, any other the position table");
   DVT_REQUIRE(!misaligned(rope, 16) && !misaligned(pos_patch, 16), "vit_forward: pos_patch and rope must be 16-byte aligned");
@@ -233,7 +264,7 @@ int vit_forward(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int 
   // No programmatic dependent launch along the block stack: these kernels are long, so the hidden launch latency is worth
   // little, and CTAs that are resident early but blocked in griddepcontrol.wait take SM slots from the fit running beside
   // the forwards.  The fit's short kernels are where PDL pays (fit.cu).
-  for (int i = 0; i <= layer_index; ++i) {
+  for (int i = 0, tap = 0; i <= layers[n_layers - 1]; ++i) {
     const VitBlock& b = v->blocks[i];
     rc = launch_layernorm(v->x, C, b.n1w, b.n1b, v->xn, C, true, Mi, C, v->ln_eps, 1, 0, stream);
     if (rc) return rc;
@@ -278,17 +309,34 @@ int vit_forward(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int 
       rc = launch_gemm_tn(fc2_in, fc2_k, b.fc2_w, fc2_k, TMAP_BF16, s, e, stream);
       if (rc) return rc;
     }
-  }
-  const int skip = out_all_tokens ? 0 : v->prefix;
-  if (apply_norm) {
-    rc = launch_layernorm(v->x, C, v->norm_w, v->norm_b, out, C, false, Mi, C, v->ln_eps, ntok, skip, stream);
-    if (rc) return rc;
-  } else {
-    strip_copy_kernel<<<Mi, 256, 0, stream>>>(v->x, C, out, C, Mi, C, ntok, skip);
-    DVT_CUDA_OK(cudaGetLastError());
-    count_launch();
+    if (i == layers[tap]) {
+      rc = vit_tap(v, B, ntok, apply_norm != 0, out[tap], ldo, out_all_tokens != 0, prefix_out ? prefix_out[tap] : nullptr,
+                   stream);
+      if (rc) return rc;
+      ++tap;
+    }
   }
   return DVT_OK;
+}
+
+int vit_forward(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int stride, const float* pos_patch,
+                const float* prefix_rows, const float* rope, int layer_index, int apply_norm, float* out, int out_all_tokens,
+                cudaStream_t stream) {
+  DVT_REQUIRE(layer_index >= 0 && layer_index < v->depth, "vit_forward: layer_index %d out of range", layer_index);
+  DVT_REQUIRE(prefix_rows && out && x_in, "vit_forward: null pointer");
+  return vit_run(v, x_in, x_bf16, B, H, W, stride, pos_patch, prefix_rows, rope, 1, &layer_index, apply_norm, &out,
+                 v->embed, out_all_tokens, nullptr, stream);
+}
+
+// dvt_vit_forward_layers has checked everything that does not need the handle (api.cu)
+int vit_forward_layers(Vit* v, const void* x_in, bool x_bf16, int B, int H, int W, int stride, const float* pos_patch,
+                       const float* prefix_rows, const float* rope, int n_layers, const int* layers, int apply_norm,
+                       float* const* out, int ldo, int out_all_tokens, float* const* prefix_out, cudaStream_t stream) {
+  DVT_REQUIRE(layers[n_layers - 1] < v->depth, "dvt_vit_forward_layers: layer_indices[%d]=%d out of range [0, %d)",
+              n_layers - 1, layers[n_layers - 1], v->depth);
+  DVT_REQUIRE(ldo >= v->embed, "dvt_vit_forward_layers: ldo=%d must be >= C=%d", ldo, v->embed);
+  return vit_run(v, x_in, x_bf16, B, H, W, stride, pos_patch, prefix_rows, rope, n_layers, layers, apply_norm, out, ldo,
+                 out_all_tokens, prefix_out, stream);
 }
 
 }  // namespace dvt

@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("DVT_LIB_PATH") or os.path.join(os.path.dirname(_HERE), "libdvt_b200.so")
 # dvt_version() of the library SIGNATURES describes.  A library with another version is refused: an entry point may keep
 # its name across versions but take other arguments, and calling it through these argtypes would pass garbage pointers.
-ABI_VERSION = 103
+ABI_VERSION = 104
 
 
 class DvtError(RuntimeError):
@@ -112,6 +112,9 @@ SIGNATURES = {
     "dvt_vit_reserve": (c_int, [c_void_p, c_int, c_int, c_int, c_int]),
     "dvt_vit_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int,
                                 c_int, c_void_p, c_int, c_void_p]),
+    "dvt_vit_forward_layers": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                       c_int, POINTER(c_int), c_int, POINTER(c_void_p), c_int, c_int, POINTER(c_void_p),
+                                       c_void_p]),
 }
 
 

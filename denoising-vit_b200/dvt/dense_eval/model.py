@@ -5,9 +5,10 @@ The backbone is frozen and in eval mode, and its input is zero-padded to whole p
 forward pre-hook of the reference).  A ViT gives the timm model's own `get_intermediate_layers(n=out_indices,
 reshape=True)` (misc.py:53-77 binds `backbone_model.model.get_intermediate_layers`), whose `norm` defaults to False in
 timm 1.0.7: the blocks' outputs WITHOUT the final LayerNorm.  A Denoiser gives `[denoiser(x)] * 4` (its forward does
-apply the final norm before the denoiser blocks).  The BNHead then keeps only the entries `in_index` selects.  The
-wrapper runs one full pass per requested layer, so `ProbeBackbone` asks it for the selected layers only: the same
-tensors, a quarter of the blocks for the linear configs (layer 11 of out_indices [8, 9, 10, 11])."""
+apply the final norm before the denoiser blocks).  The BNHead then keeps only the entries `in_index` selects, so
+`ProbeBackbone` asks for the selected layers only, all of them from one pass over the blocks
+(`forward_layers_concat`), written side by side in channels as `resize_concat` concatenates them: the same tensors, and
+for the four-layer head (in_index [0, 1, 2, 3] of out_indices [8, 9, 10, 11]) 12 blocks instead of 9 + 10 + 11 + 12."""
 from __future__ import annotations
 
 import logging
@@ -59,9 +60,10 @@ class ProbeBackbone(nn.Module):
     """Frozen feature extractor of the probe: x [B, 3, H, W] -> NHWC [B, h, w, C * len(in_index)] (the `resize_concat`
     input of the BNHead; the selected maps all share one grid, so the resize is the identity).
 
-    The depth probe (`return_cls=True`, `norm=final_norm`) reads the ViT with `get_intermediate_layers(...,
-    return_prefix_tokens=True, norm=norm)` and the Denoiser with `denoiser(x, return_class_token=True, norm=norm)`, and
-    returns (features, cls [B, C * len(in_index)]) with prefix token 0 (the cls token, registers or not) per map."""
+    A ViT's maps come from `forward_layers_concat` (one pass, the maps written side by side; bit for bit the maps of
+    `get_intermediate_layers`).  The depth probe (`return_cls=True`, `norm=final_norm`) also takes prefix token 0 (the
+    cls token, registers or not) of each layer from it, and the Denoiser's `denoiser(x, return_class_token=True,
+    norm=norm)`, and returns (features, cls [B, C * len(in_index)])."""
 
     def __init__(self, model: nn.Module, out_indices: Sequence[int], in_index: Sequence[int], return_cls: bool = False,
                  norm: bool = False):
@@ -78,24 +80,15 @@ class ProbeBackbone(nn.Module):
     @torch.no_grad()
     def forward(self, x: torch.Tensor):
         x = self.pad(x)
+        if not self.is_denoiser:
+            return self.model.model.forward_layers_concat(x, self.layers, norm=self.norm, return_cls=self.return_cls)
         if self.return_cls:
-            if self.is_denoiser:
-                f, c = self.model(x, return_class_token=True, norm=self.norm)
-                feats, cls = [f] * len(self.in_index), [c] * len(self.in_index)
-            else:
-                outs = self.model.get_intermediate_layers(x, n=self.layers, reshape=True, return_prefix_tokens=True,
-                                                          norm=self.norm)
-                feats, cls = [o[0].permute(0, 2, 3, 1) for o in outs], [o[1][:, 0] for o in outs]
-            if len(feats) == 1:
-                return feats[0], cls[0]
-            return torch.cat(feats, dim=-1), torch.cat(cls, dim=-1)
-        if self.is_denoiser:
-            f = self.model(x)                                  # [B, h, w, C]
-            feats = [f] * len(self.in_index)
-        else:
-            outs = self.model.get_intermediate_layers(x, n=self.layers, reshape=True, norm=False)
-            feats = [o.permute(0, 2, 3, 1) for o in outs]
-        return feats[0] if len(feats) == 1 else torch.cat(feats, dim=-1)
+            f, c = self.model(x, return_class_token=True, norm=self.norm)
+            if len(self.in_index) == 1:
+                return f, c
+            return torch.cat([f] * len(self.in_index), dim=-1), torch.cat([c] * len(self.in_index), dim=-1)
+        f = self.model(x)                                      # [B, h, w, C]
+        return f if len(self.in_index) == 1 else torch.cat([f] * len(self.in_index), dim=-1)
 
 
 class LinearSegHead(nn.Module):

@@ -18,7 +18,7 @@ import logging
 import math
 import os
 import re
-from ctypes import byref, c_void_p
+from ctypes import byref, c_int, c_void_p
 from typing import List, Optional, Tuple, Union
 
 import torch
@@ -420,20 +420,27 @@ class B200VisionTransformer(nn.Module):
         return y.reshape(B, h, w, C)
 
     # ---- forward --------------------------------------------------------------------------------------
-    def _run(self, x: torch.Tensor, layer_index: int, norm: bool, all_tokens: bool,
-             out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def _prep(self, x: torch.Tensor):
+        """(x as a contiguous f32 / bf16 CUDA tensor, stride, h, w, pos_patch, prefix_rows, rope) of one inference forward,
+        with the handle's weights up to date."""
         if not x.is_cuda:
             raise _lib.DvtError("dvt_b200 ViT forward needs a CUDA tensor (no CPU fallback)")
         if x.dtype not in (torch.float32, torch.bfloat16):
             x = x.float()
         x = x.contiguous()
         self._sync()
-        B, _, H, W = x.shape
+        _, _, H, W = x.shape
         P = self.patch_embed.patch_size[0]
         stride = int(self.patch_embed.proj.stride[0])
         h, w = (H - P) // stride + 1, (W - P) // stride + 1
         pos_patch, prefix_rows = self._pos_tables(h, w, x.device)
         rope = self._rope_table(h, w, x.device) if self.rope else None
+        return x, stride, h, w, pos_patch, prefix_rows, rope
+
+    def _run(self, x: torch.Tensor, layer_index: int, norm: bool, all_tokens: bool,
+             out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        x, stride, h, w, pos_patch, prefix_rows, rope = self._prep(x)
+        B, _, H, W = x.shape
         C = self.embed_dim
         shape = (B, self.num_prefix_tokens + h * w, C) if all_tokens else (B, h, w, C)
         if out is None:
@@ -444,6 +451,48 @@ class B200VisionTransformer(nn.Module):
                                     ptr(pos_patch), ptr(prefix_rows), ptr(rope), layer_index, int(norm), ptr(out),
                                     int(all_tokens), cur_stream()), "dvt_vit_forward")
         return out
+
+    def _run_layers(self, x: torch.Tensor, layers: List[int], norm: bool, all_tokens: bool = False, concat: bool = False,
+                    prefix: bool = False):
+        """One dvt_vit_forward_layers pass over `layers` (strictly ascending).  Returns (maps, prefix_rows): maps is one
+        [B, h, w, L*C] tensor with the layers' maps side by side in channels (concat), else a list of one tensor per layer,
+        [B, h, w, C] ([B, prefix + h*w, C] with all_tokens); prefix_rows is [L, B, prefix, C] (prefix) or None."""
+        x, stride, h, w, pos_patch, prefix_rows, rope = self._prep(x)
+        B, _, H, W = x.shape
+        C, L, npre = self.embed_dim, len(layers), self.num_prefix_tokens
+        f32 = dict(device=x.device, dtype=torch.float32)
+        if concat:
+            maps = torch.empty(B, h, w, L * C, **f32)
+            dst, ldo = [maps[..., l * C:] for l in range(L)], L * C
+        else:
+            maps = [torch.empty((B, npre + h * w, C) if all_tokens else (B, h, w, C), **f32) for _ in range(L)]
+            dst, ldo = maps, C
+        pre = torch.empty(L, B, npre, C, **f32) if prefix else None
+        pre_ptrs = (c_void_p * L)(*[pre[l].data_ptr() for l in range(L)]) if prefix else None
+        check(lib().dvt_vit_forward_layers(self._handle, ptr(x), 0 if x.dtype == torch.bfloat16 else 1, B, H, W, stride,
+                                           ptr(pos_patch), ptr(prefix_rows), ptr(rope), L, (c_int * L)(*layers), int(norm),
+                                           (c_void_p * L)(*[t.data_ptr() for t in dst]), ldo, int(all_tokens), pre_ptrs,
+                                           cur_stream()), "dvt_vit_forward_layers")
+        return maps, pre
+
+    @torch.no_grad()
+    def forward_layers_concat(self, x: torch.Tensor, layers: List[int], *, norm: bool, return_cls: bool = False):
+        """The maps of `layers` (negative indices count from the end) side by side in channels, in the order given: NHWC
+        [B, h, w, len(layers) * C], the `resize_concat` input of the linear probes, from one pass of the blocks.  With
+        return_cls also prefix token 0 of each layer, [B, len(layers) * C].  Each map has the bits of
+        `get_intermediate_layers` for its layer."""
+        depth = len(self.blocks)
+        layers = [i if i >= 0 else depth + i for i in layers]
+        uniq = sorted(set(layers))
+        maps, pre = self._run_layers(x, uniq, norm, concat=True, prefix=return_cls)
+        if layers != uniq:  # another order or repeated layers: pick the channel blocks
+            pick = torch.tensor([uniq.index(i) for i in layers], device=maps.device)
+            B, h, w, _ = maps.shape
+            maps = maps.view(B, h, w, len(uniq), -1).index_select(3, pick).reshape(B, h, w, -1)
+            pre = pre.index_select(0, pick) if return_cls else None
+        if not return_cls:
+            return maps
+        return maps, pre[:, :, 0].transpose(0, 1).reshape(maps.shape[0], -1)
 
     def forward_intermediates(self, x, indices=None, return_prefix_tokens=False, norm=False, stop_early=False,
                               output_fmt="NCHW", intermediates_only=False):
@@ -466,17 +515,22 @@ class B200VisionTransformer(nn.Module):
             return self._forward_intermediates_infer(x, take, return_prefix_tokens, norm, output_fmt)
 
     def _forward_intermediates_infer(self, x, take, return_prefix_tokens, norm, output_fmt):
-        outs = []
-        for idx in take:  # one pass per requested layer (DVT asks for a single layer)
+        if not take:
+            return []
+        uniq = sorted(set(take))  # one pass over the blocks serves every requested layer
+        maps, _ = self._run_layers(x, uniq, norm, all_tokens=return_prefix_tokens)
+        of = dict(zip(uniq, maps))
+        outs, seen = [], set()
+        for idx in take:
+            t = of[idx] if idx not in seen else of[idx].clone()  # a repeated layer gets a tensor of its own
+            seen.add(idx)
             if return_prefix_tokens:
-                t = self._run(x, idx, norm, all_tokens=True)
                 prefix, feat = t[:, :self.num_prefix_tokens], t[:, self.num_prefix_tokens:]
                 if output_fmt == "NCHW":
                     H, W = self.patch_embed.dynamic_feat_size((x.shape[2], x.shape[3]))
                     feat = feat.reshape(x.shape[0], H, W, -1).permute(0, 3, 1, 2)
                 outs.append((feat, prefix))
-            else:
-                t = self._run(x, idx, norm, all_tokens=False)  # [B, h, w, C]
+            else:  # [B, h, w, C]
                 outs.append(t.permute(0, 3, 1, 2) if output_fmt == "NCHW" else t.reshape(t.shape[0], -1, t.shape[-1]))
         return outs
 

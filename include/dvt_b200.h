@@ -126,6 +126,18 @@ int dvt_vit_reserve(dvt_vit_t* h, int max_batch, int H, int W, int stride);
 int dvt_vit_forward(dvt_vit_t* h, const void* x, int x_dtype, int B, int H, int W, int stride,
                     const float* pos_patch, const float* prefix_rows, const float* rope, int layer_index, int norm,
                     float* out, int all_tokens, void* stream);
+/* dvt_vit_forward for several layers in one pass: runs blocks 0..layer_indices[n_layers-1] once and, after block
+ * layer_indices[l], writes the map of that layer (final LayerNorm if `norm`, as dvt_vit_forward) into out[l] at row pitch
+ * `ldo` floats (ldo >= C, a multiple of 4; out[l] 16-byte aligned): all_tokens == 0 -> [B, h, w, C] rows, all_tokens == 1
+ * -> [B, prefix + h*w, C] rows.  layer_indices (host array) is strictly ascending within [0, depth); out and prefix_out
+ * are host arrays of n_layers device pointers.  With ldo = n_layers*C and out[l] = base + l*C the maps land
+ * channel-concatenated, [B, h, w, n_layers*C].  prefix_out (optional, not with all_tokens): prefix_out[l] receives the
+ * prefix rows of layer l, [B, prefix_tokens, C] at pitch C, normalised like out[l].  Each map has the bits dvt_vit_forward
+ * gives for that layer. */
+int dvt_vit_forward_layers(dvt_vit_t* h, const void* x, int x_dtype, int B, int H, int W, int stride,
+                           const float* pos_patch, const float* prefix_rows, const float* rope, int n_layers,
+                           const int* layer_indices, int norm, float* const* out, int ldo, int all_tokens,
+                           float* const* prefix_out, void* stream);
 
 /* General form of dvt_gemm_tn for bf16 operands, no bias or activation: a_mn / b_mn = 1 reads the operand from its
  * transposed storage ([K, M] / [K, N] row-major, "MN-major") without a copy.  Supported: (a_mn, b_mn) in {(0,0), (0,1),
